@@ -4,10 +4,18 @@
 // (/root/reference/src/feature_extractor.cpp:443-570).  Defined semantics = the sequential
 // ascending cell order (the reference's parallel_for_ body races on `mask`, SURVEY.md 2.1).
 //
-//   fast_cells_kernel   (F1, parallel over cells x frames)  FAST-9/16 score + 3x3 NMS inside each
+//   fast_cells_kernel   (F1, one CTA per cell x frame)  FAST-9/16 score + 3x3 NMS inside each
 //                       cell ROI exactly as cv::FastFeatureDetector(th, true, TYPE_9_16) on
 //                       im(hroi) does (3-px dead border per cell), candidates in scan order,
 //                       pre-filtered by the CV_32F-mask byte aliasing (cell-local x % 4 in {2,3}).
+//                       Bound by the integer pipe: the exact score of EVERY interior pixel is
+//                       computed densely, two horizontally adjacent pixels per 32-bit register
+//                       (16-bit lanes) with packed (DPX) min/max.  At threshold 10 about a fifth
+//                       of the pixels of a textured frame are corners, so a sparse filter +
+//                       compaction in front of the score removes too little to pay for itself.
+//                       On an H100 SXM (700 W limit) the three-way VIMNMX3 issues at half the rate
+//                       of a two-way VIMNMX (1.7 vs 3.5 warp instructions / clock / SM), so the
+//                       count that matters is two-way-equivalent min/max per pixel pair (~96).
 //   fast_sweep_kernel   (F2, one warp per frame)  the order-dependent part: occupancy, mask discs
 //                       (cv::circle midpoint rasterisation) kept as a 1-bit/pixel bitmap in shared
 //                       memory, per-cell mask filter -> libstdc++ std::sort top-1 -> response >= 20
@@ -31,8 +39,11 @@ constexpr int MAX_CELL = 128;
 constexpr int MAX_RADIUS = MAX_CELL / 4;
 
 // FAST ring, clockwise from 12 o'clock (SURVEY.md A.1)
-__constant__ int c_ring_dx[16] = {0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1};
-__constant__ int c_ring_dy[16] = {-3, -3, -2, -1, 0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3};
+__host__ __device__ constexpr int ring_dx(int k) {
+    constexpr int dx[16] = {0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1};
+    return dx[k];
+}
+__host__ __device__ constexpr int ring_dy(int k) { return ring_dx((k + 12) & 15); }
 
 struct FastArgs {
     const uint8_t* img; int w, h, pitch; long long fstride;   // level 0
@@ -41,7 +52,23 @@ struct FastArgs {
     uint32_t* cand;             // [count][ncells][cap]  (resp << 16) | (ky << 8) | kx
     int32_t* cand_n;            // [count][ncells]
     int32_t* overflow;          // set to 1 if a cell had more than cap candidates
-    int score_mode;             // 0: bisection on the 9-run bit test, 1: sliding-window min (sparse table)
+};
+
+// Shared-memory layout of fast_cells_kernel (bytes), shared by the kernel and its launch.
+//   stage  rp x cs bytes: the staged box (TMA destination; the cell's ROI starts (x0 & 15) bytes into each row)
+//   pairs  cs rows x pp words: pairs[y][x] = roi[y][x] | roi[y][x + 1] << 16, even x in words [0, hh), odd x in [hh, 2 hh)
+//   sc     cs rows x scp u16: score s of a corner at th, 0 elsewhere (the 3-px border and non-corners)
+//   keep   (cs - 6) rows x nk words over the stage (dead after the widening; (cs - 6)(cs - 2) < rp cs bytes): NMS survivors,
+//          word k = the pixel pair x = 4k + 2, 4k + 3 (s in a survivor's lane, else 0)
+struct FastSmem {
+    int nk, scp, pairs, sc, bytes;
+    __host__ __device__ FastSmem(int cs, int rp, int pp) {
+        nk = (cs - 6) / 4 + 1;
+        scp = 4 * nk + 4;                 // whole 8-byte pairs of words; word 2k + 2 of the last k stays in the row
+        pairs = (rp * cs + 127) & ~127;
+        sc = pairs + 4 * cs * pp;
+        bytes = sc + 2 * cs * scp;
+    }
 };
 
 // ---- TMA staging (sm_90a): one elected thread issues a single cp.async.bulk.tensor that lands
@@ -72,219 +99,178 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 }
 
 // ---------------------------------------------------------------------------------- F1
-// roi pitch `rp`: cs on the plain-load path, the TMA box width (64 / 128) when the tile is staged by TMA
+// Per polarity: the best arc extreme over the 16 arcs of 9 contiguous ring pixels, on two pixels at once.  e[k] = d[k] + 256
+// in each 16-bit lane (d = centre - ring, so every lane lies in [1, 511] and the signed s16x2 forms are exact).
+// Bright (DARK = false): max over arcs of the arc minimum; dark: min over arcs of the arc maximum.  The arcs starting at 2j
+// and 2j + 1 share the 8 pixels w_j = e[2j + 1 .. 2j + 8], so their better one is min(w_j, max(e[2j], e[2j + 9])) (bright):
+// 8 + 8 two-way ops for the w_j (windows of 2, then 4), 8 for the end pairs, 8 three-way ops for the pair of arcs, and a
+// three-way tree over the 8 pairs: 36 VIMNMX per polarity.
+template <bool DARK>
+__device__ __forceinline__ uint32_t best_arc(const uint32_t (&e)[16]) {
+    auto in2 = [](uint32_t a, uint32_t b) { if constexpr (DARK) return __vmaxs2(a, b); else return __vmins2(a, b); };
+    auto out2 = [](uint32_t a, uint32_t b) { if constexpr (DARK) return __vmins2(a, b); else return __vmaxs2(a, b); };
+    auto in3 = [](uint32_t a, uint32_t b, uint32_t c) {
+        if constexpr (DARK) return __vimax3_s16x2(a, b, c); else return __vimin3_s16x2(a, b, c);
+    };
+    auto out3 = [](uint32_t a, uint32_t b, uint32_t c) {
+        if constexpr (DARK) return __vimin3_s16x2(a, b, c); else return __vimax3_s16x2(a, b, c);
+    };
+    uint32_t p2[8], p4[8], y[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) p2[j] = in2(e[2 * j + 1], e[(2 * j + 2) & 15]);          // e[2j + 1 .. 2j + 2]
+#pragma unroll
+    for (int j = 0; j < 8; ++j) p4[j] = in2(p2[j], p2[(j + 1) & 7]);                    // e[2j + 1 .. 2j + 4]
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = in3(p4[j], p4[(j + 2) & 7], out2(e[2 * j], e[(2 * j + 9) & 15]));
+    const uint32_t a = out3(y[0], y[1], y[2]), b = out3(y[3], y[4], y[5]);
+    return out3(out3(a, b, y[6]), y[7], y[7]);
+}
+
+// HH: words per parity half of a pairs row (32 for cs <= 64, 64 above); the row pitch is a compile-time constant so every
+// ring load is an immediate offset from one base register.  PP = 2 HH + 22: 22 (mod 32) makes a warp that wraps from one
+// row to the next read 32 distinct banks at the default cell size 50 (22 pixel pairs per row).
+// `rp`: width of the staged box (the TMA box, or the same box loaded by plain loads), a multiple of 16.
+template <int HH>
 __global__ void fast_cells_kernel(FastArgs A, const __grid_constant__ CUtensorMap tmap, int use_tma, int rp) {
+    constexpr int PP = 2 * HH + 22;
     extern __shared__ __align__(128) uint8_t smem[];
-    const int cs = A.cs;
-    const uint8_t* roi = smem;                              // rp * cs (TMA destination: 128-byte aligned)
-    const int roi_bytes = (rp * cs + 127) & ~127;
-    const int cs2p = (cs * cs + 3) & ~3;                    // padded to whole words (the emission scans keep[] as words)
-    uint8_t* sc = smem + roi_bytes;                         // cs*cs: score s (0 = not a corner at th)
-    uint8_t* keep = sc + cs2p;                              // cs*cs: NMS survivor under the mask rule
-    uint16_t* clist = (uint16_t*)(keep + cs2p);             // corners, (y << 8) | x cell-local (compacted)
-    uint16_t* qlist = clist + (cs - 6) * (cs - 6);          // pixels that pass the compass pre-test (compacted)
-    __shared__ int s_nq;
-    __shared__ int s_ncorner;
     __shared__ __align__(8) uint64_t s_bar;
+    const int cs = A.cs, tid = threadIdx.x, nthr = blockDim.x;
+    const FastSmem L(cs, rp, PP);
+    uint32_t* pairs = reinterpret_cast<uint32_t*>(smem + L.pairs);
+    uint16_t* sc = reinterpret_cast<uint16_t*>(smem + L.sc);
+    uint32_t* keep = reinterpret_cast<uint32_t*>(smem);
     const int cell = blockIdx.x, fr = blockIdx.y;
     const int r = cell / A.nwc, c = cell - r * A.nwc;
     const int x0 = c * cs, y0 = r * cs;
     int32_t* out_n = A.cand_n + (size_t)fr * (A.nwc * A.nhc) + cell;
     // cells the reference never searches (feature_extractor.cpp:510)
     if (!(x0 + cs < A.w - 1 && y0 + cs < A.h - 1)) {
-        if (threadIdx.x == 0) *out_n = 0;
+        if (tid == 0) *out_n = 0;
         return;
     }
     const int th = A.th[fr];
+    // a uint8 tiled box must START on a 16-byte boundary in the innermost dimension, so the box starts at x0 & ~15 and the
+    // cell's ROI begins `off` bytes into each staged row.  Box columns beyond the image are zero.
+    const int off = x0 & 15;
+    if (use_tma && tid == 0) {
+        mbar_init(&s_bar, 1);
+        mbar_expect_tx(&s_bar, (uint32_t)(rp * cs));
+        tma_load_3d(smem, &tmap, &s_bar, x0 - off, y0, A.first + fr);
+    }
+    {
+        uint32_t* scw = reinterpret_cast<uint32_t*>(sc);
+        for (int i = tid; i < cs * L.scp / 2; i += nthr) scw[i] = 0;
+    }
     if (use_tma) {
-        if (threadIdx.x == 0) {
-            mbar_init(&s_bar, 1);
-            mbar_expect_tx(&s_bar, (uint32_t)(rp * cs));
-            // a uint8 tiled box must START on a 16-byte boundary in the innermost dimension, so the box starts at x0 & ~15
-            // and the cell's ROI begins (x0 & 15) bytes into each staged row.  Box columns beyond the
-            // image are zero-filled and never read.
-            tma_load_3d(smem, &tmap, &s_bar, x0 & ~15, y0, A.first + fr);
-        }
-        roi = smem + (x0 & 15);
-        for (int i = threadIdx.x; i < cs2p; i += blockDim.x) { sc[i] = 0; keep[i] = 0; }
         __syncthreads();             // barrier init visible to every waiter
         mbar_wait(&s_bar, 0);
     } else {
-        const uint8_t* img = A.img + A.fstride * (A.first + fr) + (size_t)y0 * A.pitch + x0;
-        for (int i = threadIdx.x; i < cs2p; i += blockDim.x) {
-            int yy = i / cs, xx = i - yy * cs;
-            if (i < cs * cs) smem[yy * rp + xx] = __ldg(img + (size_t)yy * A.pitch + xx);
-            sc[i] = 0;
-            keep[i] = 0;
+        const uint8_t* img = A.img + A.fstride * (A.first + fr) + (size_t)y0 * A.pitch + (x0 - off);
+        const int avail = A.w - (x0 - off);
+        for (int i = tid; i < rp * cs; i += nthr) {
+            const int yy = i / rp, u = i - yy * rp;
+            smem[i] = u < avail ? __ldg(img + (size_t)yy * A.pitch + u) : (uint8_t)0;
         }
+        __syncthreads();
     }
-    if (threadIdx.x == 0) { s_ncorner = 0; s_nq = 0; }
-    __syncthreads();
-    const int in_w = cs - 6;
-    // pass 1a (every interior pixel): compass pre-test, survivors compacted into qlist.  Every 9-arc of
-    // the 16-ring contains two ADJACENT compass points {0,4,8,12}, so a corner needs two adjacent compass
-    // pixels brighter than v + th (or darker than v - th).  Doing the full ring test here instead would
-    // run it for nearly every warp (one passing lane is enough): ncu showed the 180-instruction ring block
-    // executed by 92 % of the warp iterations.  (y, x) advance incrementally: no division per pixel.
+    // widen: pairs[y][x] for x in [0, cs); item (y, j) writes x = 2j (even half) and x = 2j + 1 (odd half) from the staged
+    // bytes at u = off + 2j .. off + 2j + 2 (the odd half's entry for x = cs is never read)
     {
-        const int npx = in_w * in_w, lane = threadIdx.x & 31;
-        int i = threadIdx.x;
-        int yy = i / in_w, xx = i - yy * in_w;
-        const int sy = (int)blockDim.x / in_w, sx = (int)blockDim.x - sy * in_w;
-        for (int base = 0; base < npx; base += blockDim.x) {      // uniform trip count: ballots below
-            bool pass = false;
-            if (i < npx) {
-                const uint8_t* p = roi + (yy + 3) * rp + (xx + 3);
-                const int v = *p;
-                const int c0 = v - (int)p[-3 * rp], c4 = v - (int)p[3], c8 = v - (int)p[3 * rp], c12 = v - (int)p[-3];
-                const bool b0 = c0 > th, b4 = c4 > th, b8 = c8 > th, b12 = c12 > th;
-                const bool d0 = c0 < -th, d4 = c4 < -th, d8 = c8 < -th, d12 = c12 < -th;
-                pass = ((b0 || b8) && (b4 || b12)) || ((d0 || d8) && (d4 || d12));   // two adjacent compass points
-            }
-            const unsigned m = __ballot_sync(FULL, pass);
-            if (m) {
-                const int leader = __ffs(m) - 1;
-                int slot = 0;
-                if (lane == leader) slot = atomicAdd(&s_nq, __popc(m));
-                slot = __shfl_sync(FULL, slot, leader);
-                if (pass) qlist[slot + __popc(m & ((1u << lane) - 1u))] = (uint16_t)(((yy + 3) << 8) | (xx + 3));
-            }
-            i += blockDim.x;
-            xx += sx; yy += sy;
-            if (xx >= in_w) { xx -= in_w; yy++; }
+        const int nq = rp >> 2, hw = (cs + 1) >> 1;
+        const uint32_t* sw = reinterpret_cast<const uint32_t*>(smem);
+        int y = tid / hw, j = tid - y * hw;
+        const int sy = nthr / hw, sj = nthr - sy * hw;
+        for (int i = tid; i < cs * hw; i += nthr) {
+            const int u = off + 2 * j, q = u >> 2;
+            const uint32_t* row = sw + y * nq;
+            const uint32_t b4 = __funnelshift_r(row[q], row[q + 1 < nq ? q + 1 : q], 8 * (u & 3));   // bytes u .. u + 3
+            uint32_t* prow = pairs + y * PP + j;
+            prow[0] = __byte_perm(b4, 0u, 0x4140);
+            prow[HH] = __byte_perm(b4, 0u, 0x4241);
+            j += sj; y += sy;
+            if (j >= hw) { j -= hw; y++; }
         }
     }
     __syncthreads();
-    // ring offsets for this pitch, once per thread (they were 16 IMADs per tested pixel)
-    int roff[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) roff[k] = c_ring_dy[k] * rp + c_ring_dx[k];
-    // pass 1b (dense over the survivors): the 16-pixel ring test
-    const int nq = s_nq;
-    for (int q = threadIdx.x; q < nq; q += blockDim.x) {
-        const int yx = qlist[q];
-        const uint8_t* p = roi + (yx >> 8) * rp + (yx & 255);
-        const int v = *p;
-        const int vlo = v - th, vhi = v + th;              // bright: ring < v - th, dark: ring > v + th
-        unsigned bright = 0, dark = 0;
-#pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const int rk = (int)p[roff[k]];
-            bright |= (unsigned)(rk < vlo) << k;
-            dark |= (unsigned)(rk > vhi) << k;
-        }
-        unsigned b = bright | (bright << 16), dk = dark | (dark << 16);
-        b &= b >> 1; b &= b >> 2; b &= b >> 4; b &= b >> 1;
-        dk &= dk >> 1; dk &= dk >> 2; dk &= dk >> 4; dk &= dk >> 1;
-        if ((b | dk) & 0xFFFFu) {
-            int pos = atomicAdd(&s_ncorner, 1);
-            clist[pos] = (uint16_t)yx;
-        }
-    }
-    __syncthreads();
-    // pass 2 (dense over the corners): exact score s = max over the 16 arcs of min(d) / min(-d)
-    // = the largest t for which a 9-run of (d >= t) or (d <= -t) exists: bisection on t.
-    const int ncorner = s_ncorner;
-    for (int i = threadIdx.x; i < ncorner; i += blockDim.x) {
-        const int yx = clist[i];
-        const int pi = (yx >> 8) * cs + (yx & 255);
-        const uint8_t* p = roi + (yx >> 8) * rp + (yx & 255);
-        const int v = *p;
-        int d[16];
-#pragma unroll
-        for (int k = 0; k < 16; ++k) d[k] = v - (int)p[roff[k]];
-        int lo;
-        if (A.score_mode == 1) {
-            // s = max_k min(d[k..k+8]) (bright) / max_k min(-d[k..k+8]) (dark) with a sparse table:
-            // m2 = windows of 2, m4 of 4, m8 of 8, then one more element -> 9.  inline PTX min/max keeps
-            // this as written (see DESIGN.md: a naive 16x8 min/max nest was folded into VIMNMX3 chains
-            // that returned max(d)).
-            int best = 0;
-#pragma unroll
-            for (int pol = 0; pol < 2; ++pol) {
-                int e[16], m2[16], m4[16];
-#pragma unroll
-                for (int k = 0; k < 16; ++k) e[k] = pol ? -d[k] : d[k];
-#pragma unroll
-                for (int k = 0; k < 16; ++k) asm("min.s32 %0, %1, %2;" : "=r"(m2[k]) : "r"(e[k]), "r"(e[(k + 1) & 15]));
-#pragma unroll
-                for (int k = 0; k < 16; ++k) asm("min.s32 %0, %1, %2;" : "=r"(m4[k]) : "r"(m2[k]), "r"(m2[(k + 2) & 15]));
-#pragma unroll
-                for (int k = 0; k < 16; ++k) {
-                    int m8, m9;
-                    asm("min.s32 %0, %1, %2;" : "=r"(m8) : "r"(m4[k]), "r"(m4[(k + 4) & 15]));
-                    asm("min.s32 %0, %1, %2;" : "=r"(m9) : "r"(m8), "r"(e[(k + 8) & 15]));
-                    asm("max.s32 %0, %1, %2;" : "=r"(best) : "r"(best), "r"(m9));
-                }
-            }
-            lo = best;
-        } else {
-        lo = th + 1;
-        int hi = 256;   // P(lo) holds (corner at th), P(256) cannot
-        while (hi - lo > 1) {
-            const int mid = (lo + hi) >> 1;
-            unsigned bm = 0, dm = 0;
+    // score: pixel pairs (x, x + 1), x = 3 + 2j odd, over the interior [3, cs - 3)^2; an odd interior width leaves the last
+    // pair half outside (its upper lane is computed from in-smem bytes and not stored)
+    const int in_w = cs - 6, npair = (in_w + 1) >> 1;
+    {
+        const uint32_t th1 = (uint32_t)(min(max(th, -1), 255) + 257) * 0x00010001u;      // th + 257 per lane, th clamped to [-1, 255]
+        int yy = tid / npair, jj = tid - yy * npair;
+        const int sy = nthr / npair, sj = nthr - sy * npair;
+        for (int i = tid; i < in_w * npair; i += nthr) {
+            const int y = yy + 3, x = 2 * jj + 3;
+            const uint32_t* ctr = pairs + y * PP + HH + (x >> 1);      // x odd: the odd half
+            const uint32_t vb = ctr[0] + 0x01000100u;
+            uint32_t e[16];
 #pragma unroll
             for (int k = 0; k < 16; ++k) {
-                bm |= (unsigned)(d[k] >= mid) << k;
-                dm |= (unsigned)(d[k] <= -mid) << k;
+                // ring pixel (x + dx, y + dy): even dx stays in the odd half, odd dx lands in the even half
+                const int dx = ring_dx(k), dy = ring_dy(k);
+                const int o = dy * PP + ((dx & 1) ? -HH + ((dx + 1) >> 1) : (dx >> 1));
+                e[k] = vb - ctr[o];                 // d + 256 per lane, no borrow between lanes: each lane is in [1, 511]
             }
-            bm |= bm << 16; dm |= dm << 16;
-            bm &= bm >> 1; bm &= bm >> 2; bm &= bm >> 4; bm &= bm >> 1;
-            dm &= dm >> 1; dm &= dm >> 2; dm &= dm >> 4; dm &= dm >> 1;
-            if ((bm | dm) & 0xFFFFu) lo = mid; else hi = mid;
+            const uint32_t bright = best_arc<false>(e), dark = best_arc<true>(e);
+            // s + 256 = max(bright, 512 - dark, 256) per lane: s = max(best bright arc, best dark arc, 0)
+            const uint32_t s2 = __vimax3_s16x2(bright, 0x02000200u - dark, 0x01000100u);
+            // corner at th: s > th, i.e. s + 256 >= th1 (bit 15 of each biased lane); no borrow crosses a lane
+            const uint32_t ge = ((s2 | 0x80008000u) - th1) & (x + 1 < cs - 3 ? 0x80008000u : 0x00008000u);
+            const uint32_t sv = (s2 - 0x01000100u) & ((ge >> 15) * 0xFFFFu);
+            uint16_t* o = sc + y * L.scp + x;
+            o[0] = (uint16_t)sv;
+            o[1] = (uint16_t)(sv >> 16);                           // 0 for the upper half of a half pair (outside the interior)
+            jj += sj; yy += sy;
+            if (jj >= npair) { jj -= npair; yy++; }
         }
-        }
-        sc[pi] = (uint8_t)lo;   // th < s <= 255
     }
     __syncthreads();
-    // 3x3 NMS on response = s - 1 (non-corners count 0): strictly greater than all 8 neighbours
-    for (int i = threadIdx.x; i < ncorner; i += blockDim.x) {
-        const int yx = clist[i];
-        const int xx = yx & 255, pi = (yx >> 8) * cs + xx;
-        const int resp = (int)sc[pi] - 1;
-        bool ok = true;
-#pragma unroll
-        for (int dy = -1; dy <= 1; ++dy)
-#pragma unroll
-            for (int dx = -1; dx <= 1; ++dx) {
-                if (dx == 0 && dy == 0) continue;
-                int sn = sc[pi + dy * cs + dx];
-                int rn = sn ? sn - 1 : 0;
-                ok = ok && (resp > rn);
-            }
-        // CV_32F mask read as bytes: only cell-local x % 4 in {2,3} can see a non-zero byte of 1.0f
-        if (ok && (xx & 2)) keep[pi] = 1;
+    // 3x3 NMS on response = s - 1 (non-corners count 0), strictly greater than all 8 neighbours: s > max(neighbours' s, 1).
+    // Only cell-local x % 4 in {2, 3} (the CV_32F mask read as bytes): one keep word per pixel pair x = 4k + 2, 4k + 3,
+    // which is sc word 2k + 1 of its row.
+    const int nk = L.nk, nkeep = in_w * nk, scw = L.scp / 2;
+    {
+        const uint32_t* s32 = reinterpret_cast<const uint32_t*>(sc);
+        int yy = tid / nk, kk = tid - yy * nk;
+        const int sy = nthr / nk, sk = nthr - sy * nk;
+        for (int t = tid; t < nkeep; t += nthr) {
+            const uint32_t* w = s32 + (yy + 3) * scw + 2 * kk;
+            const uint2 a0 = *reinterpret_cast<const uint2*>(w - scw), a1 = *reinterpret_cast<const uint2*>(w),
+                        a2 = *reinterpret_cast<const uint2*>(w + scw);
+            const uint32_t ca = __vimax3_u16x2(a0.x, a1.x, a2.x);                 // column maxima at x = 4k, 4k + 1
+            const uint32_t cc = __vimax3_u16x2(w[2 - scw], w[2], w[2 + scw]);    // at x = 4k + 4, 4k + 5
+            const uint32_t vb = __vmaxu2(a0.y, a2.y);                            // above / below x = 4k + 2, 4k + 3
+            const uint32_t cb = __vmaxu2(vb, a1.y);
+            const uint32_t left = __byte_perm(ca, cb, 0x5432), right = __byte_perm(cb, cc, 0x5432);   // x - 1, x + 1
+            const uint32_t m = __vimax3_u16x2(__vimax3_u16x2(left, right, vb), 0x00010001u, 0x00010001u);
+            const uint32_t s = a1.y;
+            const uint32_t gt = ((s | 0x80008000u) - (m + 0x00010001u)) & 0x80008000u;   // bit 15 of a lane: s > m
+            keep[t] = s & ((gt >> 15) * 0xFFFFu);
+            kk += sk; yy += sy;
+            if (kk >= nk) { kk -= nk; yy++; }
+        }
     }
     __syncthreads();
-    // ordered emission (row-major scan order) by warp 0: keep[] is scanned as 32-bit words (almost all
-    // zero); the few non-zero words are expanded serially, so the output order is the scan order
-    if (threadIdx.x < 32) {
+    // ordered emission (row-major scan order) by warp 0, 32 keep words per step
+    if (tid < 32) {
         uint32_t* out = A.cand + ((size_t)fr * (A.nwc * A.nhc) + cell) * A.cap;
-        const uint32_t* kw = reinterpret_cast<const uint32_t*>(keep);
-        const int nw = cs2p >> 2, lane = threadIdx.x;
-        const unsigned rcs = 0xFFFFFFFFu / (unsigned)cs + 1u;          // ceil(2^32 / cs): floor(pi * rcs / 2^32) == pi / cs for pi < 2^16
+        const int lane = tid;
+        const unsigned below = (1u << lane) - 1u;
+        const unsigned rnk = 0xFFFFFFFFu / (unsigned)nk + 1u;          // ceil(2^32 / nk): t / nk == umulhi(t, rnk) for t < 2^16, nk > 1
         int n = 0;
-        for (int base = 0; base < nw; base += 32) {
-            const int wi = base + lane;
-            const uint32_t w = wi < nw ? kw[wi] : 0u;
-            unsigned m = __ballot_sync(FULL, w != 0u);
-            while (m) {                                    // uniform
-                const int L = __ffs(m) - 1;
-                m &= m - 1;
-                const uint32_t ww = __shfl_sync(FULL, w, L);
-#pragma unroll
-                for (int b = 0; b < 4; ++b) {
-                    if ((ww >> (8 * b)) & 0xFFu) {
-                        if (lane == 0 && n < A.cap) {
-                            const int pi = (base + L) * 4 + b;
-                            const int yy = (int)__umulhi((unsigned)pi, rcs), xx = pi - yy * cs;   // pi / cs, exact for pi < 2^16
-                            out[n] = ((uint32_t)(sc[pi] - 1) << 16) | ((uint32_t)yy << 8) | (uint32_t)xx;
-                        }
-                        n++;
-                    }
-                }
+        for (int base = 0; base < nkeep; base += 32) {
+            const uint32_t w = base + lane < nkeep ? keep[base + lane] : 0u;
+            const uint32_t s0 = w & 0xFFFFu, s1 = w >> 16;
+            const unsigned m0 = __ballot_sync(FULL, s0 != 0u), m1 = __ballot_sync(FULL, s1 != 0u);
+            if (w) {
+                const int p = n + __popc(m0 & below) + __popc(m1 & below);
+                const unsigned t = base + lane, yy = nk > 1 ? __umulhi(t, rnk) : t, kk = t - yy * nk;
+                const uint32_t yx = ((yy + 3u) << 8) | (4u * kk + 2u);
+                if (s0 && p < A.cap) out[p] = ((s0 - 1u) << 16) | yx;
+                if (s1 && p + (s0 != 0u) < A.cap) out[p + (s0 != 0u)] = ((s1 - 1u) << 16) | (yx + 1u);
             }
+            n += __popc(m0) + __popc(m1);
         }
         if (lane == 0) {
             if (n > A.cap) { atomicExch(A.overflow, 1); n = A.cap; }
@@ -715,7 +701,7 @@ void circle_halfwidths(int radius, int* hw) {
 
 // Host side of the TMA staging: a 3-D tiled tensor map {W, H, frames} over the level-0 images, box
 // {rp, cs, 1} (rp = cs + 15 rounded up to 16 bytes: the box starts on the 16-byte boundary at or below the cell).  Falls back to plain loads
-// when the images do not meet the TMA alignment rules (user-aliased level 0 with an odd pitch).
+// of the same box when the images do not meet the TMA alignment rules (user-aliased level 0 with an odd pitch).
 typedef CUresult (*ov2_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -731,32 +717,39 @@ static ov2_encode_tiled_fn tma_encoder() {
     return fn;
 }
 
+template <int HH>
+static ov2_status launch_fast_cells_hh(ov2_ctx* ctx, const FastArgs& FA, int nframes_grid, const CUtensorMap& tmap, int use_tma,
+                                      int rp) {
+    const int cs = FA.cs;
+    const int threads = cs > 24 ? 128 : 32;
+    const FastSmem L(cs, rp, 2 * HH + 22);
+    if (L.bytes > 48 * 1024)
+        OV2_CUDA(ctx, cudaFuncSetAttribute(fast_cells_kernel<HH>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.bytes));
+    OV2_LAUNCH(ctx, "fast_cells_kernel",
+               fast_cells_kernel<HH><<<dim3(FA.nwc * FA.nhc, nframes_grid), threads, L.bytes, ctx->stream>>>(FA, tmap, use_tma, rp));
+    return OV2_OK;
+}
+
 static ov2_status launch_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, const FastArgs& FA, int nframes_grid) {
     const int cs = FA.cs;
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
-    int use_tma = 0, rp = cs;
+    int use_tma = 0;
+    const int rp = (cs + 15 + 15) & ~15;      // staged box width, TMA or not
     const char* env = getenv("OV2_NO_TMA");
     ov2_encode_tiled_fn enc = (env && atoi(env)) ? nullptr : tma_encoder();
     if (enc && ((uintptr_t)FA.img % 16) == 0 && FA.pitch % 16 == 0 && FA.fstride % 16 == 0) {
-        const int box_w = (cs + 15 + 15) & ~15;
         cuuint64_t dims[3] = {(cuuint64_t)FA.w, (cuuint64_t)FA.h, (cuuint64_t)pyr->batch};
         cuuint64_t strides[2] = {(cuuint64_t)FA.pitch, (cuuint64_t)FA.fstride};
-        cuuint32_t box[3] = {(cuuint32_t)box_w, (cuuint32_t)cs, 1};
+        cuuint32_t box[3] = {(cuuint32_t)rp, (cuuint32_t)cs, 1};
         cuuint32_t estr[3] = {1, 1, 1};
         CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)FA.img, dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r == CUDA_SUCCESS) { use_tma = 1; rp = box_w; }
+        if (r == CUDA_SUCCESS) use_tma = 1;
     }
-    const int threads = cs > 24 ? 128 : 32;
-    const size_t roi_bytes = ((size_t)rp * cs + 127) & ~(size_t)127;
-    const size_t smem = roi_bytes + (size_t)2 * ((cs * cs + 3) & ~3) + (size_t)4 * (cs - 6) * (cs - 6);
-    if (smem > 48 * 1024)
-        OV2_CUDA(ctx, cudaFuncSetAttribute(fast_cells_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    OV2_LAUNCH(ctx, "fast_cells_kernel",
-               fast_cells_kernel<<<dim3(FA.nwc * FA.nhc, nframes_grid), threads, smem, ctx->stream>>>(FA, tmap, use_tma, rp));
-    return OV2_OK;
+    return cs <= 64 ? launch_fast_cells_hh<32>(ctx, FA, nframes_grid, tmap, use_tma, rp)
+                    : launch_fast_cells_hh<64>(ctx, FA, nframes_grid, tmap, use_tma, rp);
 }
 
 
@@ -834,7 +827,6 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     FA.img = pyr->l0; FA.w = W; FA.h = H; FA.pitch = (int)pyr->l0_pitch; FA.fstride = (long long)pyr->l0_fstride;
     FA.first = first; FA.cs = cellsize; FA.nwc = nwc; FA.nhc = nhc; FA.cap = cap;
     FA.th = d_th; FA.cand = d_cand; FA.cand_n = d_candn; FA.overflow = d_ovf;
-    FA.score_mode = getenv("OV2_FAST_SCORE") ? atoi(getenv("OV2_FAST_SCORE")) : 1;
     if ((st = launch_fast_cells(ctx, pyr, FA, count)) != OV2_OK) return st;
     SweepArgs SA;
     SA.w = W; SA.h = H; SA.cs = cellsize; SA.nwc = nwc; SA.nhc = nhc; SA.cap = cap;
@@ -922,7 +914,6 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
     if ((st = ov2_scratch(ctx, sizeof(int32_t), &o)) != OV2_OK) return st;
     FA.overflow = (int32_t*)o;
     OV2_CUDA(ctx, cudaMemsetAsync(FA.overflow, 0, sizeof(int32_t), ctx->stream));
-    FA.score_mode = getenv("OV2_FAST_SCORE") ? atoi(getenv("OV2_FAST_SCORE")) : 1;
     if ((st = launch_fast_cells(ctx, pyr, FA, 1)) != OV2_OK) return st;
     return ov2_end(ctx);
 }

@@ -1,0 +1,59 @@
+"""The per-cell FAST candidate lists of stage F1 (ov2_debug_fast_cells) against oracle/image_ref.py::fast_detect_ref.
+
+The grid tests only see one winner per cell; this pins every candidate: position, response and scan order, after the
+CV_32F-mask byte filter (cell-local x % 4 in {2, 3}).  Cell sizes cover the default 50, odd interior widths (35, 65), the
+32-thread CTA (8, 16) and both pair-row layouts of the kernel (<= 64 and above, up to 128); thresholds go down to 0, and a
+high-contrast frame with 0 / 255 pixels drives scores to 255.
+"""
+import numpy as np
+import pytest
+
+from ov2slam_b200 import api, synth
+from oracle import image_ref as R
+
+pytestmark = pytest.mark.gpu
+
+W, H = 640, 480
+THRESHOLDS = (10, 6, 3, 1, 0)
+
+
+def _frames():
+    tex = synth.make_frame(30, W, H)
+    hc = np.where(synth.make_frame(31, W, H) > 127, 255, 0).astype(np.uint8)
+    rng = np.random.default_rng(31)
+    salt = rng.random((H, W))
+    hc[salt < 0.01] = 0
+    hc[salt > 0.99] = 255
+    return {"textured": tex, "high_contrast": hc}
+
+
+def _cap(cs):
+    in_w = cs - 6
+    return min(128, max(4, ((in_w + 1) // 2) ** 2))
+
+
+@pytest.mark.parametrize("staging", ["tma", "plain"])
+@pytest.mark.parametrize("cs", [50, 35, 16, 8, 64, 65, 128])
+def test_fast_cell_candidates_match_oracle(ctx, monkeypatch, cs, staging):
+    if staging == "plain":
+        monkeypatch.setenv("OV2_NO_TMA", "1")
+    nw, cap = W // cs, _cap(cs)
+    top = 0
+    for name, im in _frames().items():
+        pyr = api.Pyramid(ctx, 1, W, H, 0)
+        pyr.build(im[None])
+        fe = api.FeatureExtractor(ctx)
+        for th in THRESHOLDS:
+            cells = fe.debug_fast_cells(pyr, 0, cs, th)
+            assert len(cells) == (H // cs) * nw
+            for ci, got in enumerate(cells):
+                x, y = (ci % nw) * cs, (ci // nw) * cs
+                if not (x + cs < W - 1 and y + cs < H - 1):
+                    assert got == [], (name, th, ci)
+                    continue
+                ref = [k for k in R.fast_detect_ref(im[y:y + cs, x:x + cs], th) if k[0] % 4 in (2, 3)]
+                assert got == ref[:cap], (name, th, ci, got[:6], ref[:6], len(got), len(ref))
+                if got:
+                    top = max(top, max(k[2] for k in got))
+        pyr.close()
+    assert top == 254.0            # response = score - 1: the 0 / 255 frame reaches the largest score
