@@ -112,6 +112,35 @@ OV2_API ov2_status ov2_clahe(ov2_ctx* ctx, const uint8_t* src, uint8_t* dst, int
 OV2_API ov2_status ov2_preprocess(ov2_ctx* ctx, const ov2_pyr* raw, ov2_pyr* out, int first, int count, int use_clahe,
                           double clip_limit, int tiles_x, int tiles_y);
 
+/* ------------------------------------------------------------------ R: rectification / undistortion
+ * Replaces CameraCalibration::rectifyImage(img, rect) (/root/reference/src/camera_calibration.cpp:233-241), i.e.
+ * cv::remap(img, rect, undist_map_x_, undist_map_y_, cv::INTER_LINEAR) with the default BORDER_CONSTANT 0, which the
+ * reference runs on every incoming image when `bdo_stereo_rect` or `bdo_undist` is set (src/ov2slam.cpp:239-243, 252-257).
+ * 8-bit single-channel images, bit-exact with cv::remap.  A map is built once per camera (its maps come from
+ * CameraCalibration::setUndistStereoMap, CV_16SC2 + CV_16UC1, src/camera_calibration.cpp:141, or setUndistMap, two CV_32FC1,
+ * :92; fisheye maps are the same data) and has the image's size.
+ *   map_type OV2_MAP_16SC2: map1 = int16 (x, y) pairs, map2 = uint16 interpolation-table indices (cv::convertMaps' layout);
+ *            OV2_MAP_32FC1: map1 = float x, map2 = float y.  The values equal OpenCV's type codes (CV_16SC2, CV_32FC1).
+ *   Strides in bytes; maps host or device (copied and converted at creation, then no longer needed).
+ *   width or height above 2046 -> OV2_ERR_CAPACITY.
+ * A map belongs to the device of the creating context and may be used by every context on that device; destroy it after
+ * their last use. */
+#define OV2_MAP_16SC2 11
+#define OV2_MAP_32FC1 5
+typedef struct ov2_remap_map ov2_remap_map;
+OV2_API ov2_status ov2_remap_create(ov2_ctx* ctx, int map_type, int width, int height, const void* map1, size_t map1_stride,
+                                    const void* map2, size_t map2_stride, ov2_remap_map** out);
+OV2_API void       ov2_remap_destroy(ov2_remap_map* map);
+/* `count` images of the map's size, frame k at src + k*src_frame_stride (likewise dst), host or device.  A host dst may alias
+ * the host src (the reference calls rectifyImage(im0, im0), src/ov2slam.cpp:255-256); a device dst may not. */
+OV2_API ov2_status ov2_remap(ov2_ctx* ctx, const ov2_remap_map* map, const uint8_t* src, size_t src_row_stride, size_t src_frame_stride,
+                             uint8_t* dst, size_t dst_row_stride, size_t dst_frame_stride, int count);
+/* ov2_pyr_build with the rectification fused in: the unrectified images (host: uploaded once; device: read in place) are
+ * remapped into the pyramid's OWN level 0 of frame slots [first, first+count), then its levels are built.  ov2_preprocess, the
+ * detectors, ov2_describe and ov2_fb_klt run on that pyramid unchanged.  The map must have the pyramid's level-0 size. */
+OV2_API ov2_status ov2_pyr_build_remap(ov2_ctx* ctx, ov2_pyr* pyr, const ov2_remap_map* map, const uint8_t* images, size_t row_stride,
+                                       size_t frame_stride, int first, int count);
+
 /* ------------------------------------------------------------------ K: forward/backward KLT
  * Replaces FeatureTracker::fbKltTracking(vprevpyr, vcurpyr, nwinsize, nbpyrlvl, ferr,
  * fmax_fbklt_dist, vkps, vpriorkps, vkpstatus) (/root/reference/src/feature_tracker.cpp:35-137;

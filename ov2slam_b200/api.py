@@ -30,6 +30,7 @@ ABI_SYMBOLS = [
     "ov2_batch_begin", "ov2_batch_end",
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
+    "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
     "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_sharded", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
@@ -124,6 +125,11 @@ def load():
     lib.ov2_pyr_download.argtypes = [vp, vp, i32, i32, vp, C.POINTER(i32), C.POINTER(i32)]
     lib.ov2_clahe.argtypes = [vp, vp, vp, i32, i32, sz, sz, i32, C.c_double, i32, i32]
     lib.ov2_preprocess.argtypes = [vp, vp, vp, i32, i32, i32, C.c_double, i32, i32]
+    lib.ov2_remap_create.argtypes = [vp, i32, i32, i32, vp, sz, vp, sz, C.POINTER(vp)]
+    lib.ov2_remap_destroy.argtypes = [vp]
+    lib.ov2_remap_destroy.restype = None
+    lib.ov2_remap.argtypes = [vp, vp, vp, sz, sz, vp, sz, sz, i32]
+    lib.ov2_pyr_build_remap.argtypes = [vp, vp, vp, vp, sz, sz, i32, i32]
     lib.ov2_fb_klt.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp]
     lib.ov2_grid_fast.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_detect_single_scale.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, i32]
@@ -253,6 +259,16 @@ class Pyramid:
         if hasattr(images, "data_ptr"):
             self._keepalive = images
 
+    def build_remap(self, rmap: "RemapMap", images, first: int = 0, count: int | None = None, row_stride=None, frame_stride=None):
+        """ov2_pyr_build_remap: rectify the unrectified `images` through `rmap` into this pyramid's own level 0 and build its
+        levels (what CameraCalibration::rectifyImage followed by the pyramid build computes).  images: (count, H, W) uint8
+        numpy array (host, uploaded once) or CUDA torch tensor (read in place)."""
+        if count is None:
+            count = images.shape[0] if images.ndim == 3 else 1
+        rs = int(row_stride if row_stride is not None else self.w)
+        fs = int(frame_stride if frame_stride is not None else rs * self.h)
+        self.ctx.check(self.ctx.lib.ov2_pyr_build_remap(self.ctx.h, self.h_, rmap.h_, _ptr(images), rs, fs, first, count))
+
     def download(self, frame: int, level: int) -> np.ndarray:
         lw, lh = self.w, self.h
         for _ in range(level):
@@ -290,6 +306,52 @@ def clahe(ctx: Context, src, dst, width: int, height: int, count: int = 1, clip_
     rs = int(row_stride if row_stride is not None else width)
     fs = int(frame_stride if frame_stride is not None else rs * height)
     ctx.check(ctx.lib.ov2_clahe(ctx.h, _ptr(src), _ptr(dst), width, height, rs, fs, count, float(clip_limit), tx, ty))
+
+
+class RemapMap:
+    """ov2_remap_map: a rectification / undistortion map on the device (CameraCalibration's undist_map_x_ / undist_map_y_),
+    built once per camera.  map1 / map2: int16 [H, W, 2] + uint16 [H, W] (CV_16SC2 + CV_16UC1, what setUndistStereoMap
+    builds) or float32 [H, W] x / y (CV_32FC1, setUndistMap); numpy arrays or CUDA tensors."""
+
+    MAP_16SC2, MAP_32FC1 = 11, 5
+
+    def __init__(self, ctx: Context, map1, map2):
+        self.ctx = ctx
+        is_float = str(map1.dtype).endswith("float32")
+        if not is_float and not str(map1.dtype).endswith("int16"):
+            raise Ov2Error(f"map1 must be int16 (CV_16SC2) or float32 (CV_32FC1), not {map1.dtype}")
+        self.type = self.MAP_32FC1 if is_float else self.MAP_16SC2
+        self.h, self.w = int(map1.shape[0]), int(map1.shape[1])
+        s1 = self.w * 4
+        s2 = self.w * (4 if is_float else 2)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.ov2_remap_create(ctx.h, self.type, self.w, self.h, _ptr(map1), s1, _ptr(map2), s2, C.byref(h)))
+        self.h_ = h
+        ctx._pyramids.append(weakref.ref(self))      # destroyed before the context, like the pyramids
+
+    def close(self):
+        if self.h_ and self.ctx.h:
+            self.ctx.lib.ov2_remap_destroy(self.h_)
+        self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def remap(ctx: Context, rmap: RemapMap, src, dst, count: int | None = None, src_row_stride=None, src_frame_stride=None,
+          dst_row_stride=None, dst_frame_stride=None):
+    """ov2_remap: CameraCalibration::rectifyImage (cv::remap INTER_LINEAR, BORDER_CONSTANT 0) on `count` images of the map's size
+    (numpy arrays or CUDA tensors, (count, H, W) or (H, W)); a host dst may be the host src."""
+    if count is None:
+        count = src.shape[0] if src.ndim == 3 else 1
+    srs = int(src_row_stride if src_row_stride is not None else rmap.w)
+    sfs = int(src_frame_stride if src_frame_stride is not None else srs * rmap.h)
+    drs = int(dst_row_stride if dst_row_stride is not None else rmap.w)
+    dfs = int(dst_frame_stride if dst_frame_stride is not None else drs * rmap.h)
+    ctx.check(ctx.lib.ov2_remap(ctx.h, rmap.h_, _ptr(src), srs, sfs, _ptr(dst), drs, dfs, int(count)))
 
 
 def preprocess(ctx: Context, raw: "Pyramid", out: "Pyramid", first: int = 0, count: int | None = None, use_clahe: bool = True,

@@ -29,6 +29,7 @@ SOURCES = {
     "frontend_clahe.cu": ["-fmad=false"],
     "frontend_sscale.cu": ["-fmad=false"],
     "frontend_sad.cu": ["-fmad=false"],
+    "frontend_remap.cu": [],
     "frontend_step.cu": [],
     "ba_solver.cu": [],
     "ba_lm.cu": [],
@@ -100,6 +101,7 @@ def build_host_shims(verbose: bool = False) -> Path:
     subprocess.check_call(["g++", "-o", str(LIB / "clahe_selftest"), *objs[3:], "-L", str(LIB), "-lov2b200", "-lpthread",
                            "-Wl,-rpath,$ORIGIN"])
     build_optimizer_shim(verbose)
+    build_rect_shim(verbose)
     return exe
 
 
@@ -167,6 +169,28 @@ def build_stereo_shim(verbose: bool = False) -> Path:
             subprocess.check_call(cmd)
         objs.append(str(obj))
     exe = LIB / "stereo_selftest"
+    subprocess.check_call(["g++", "-o", str(exe), *objs, "-L", str(LIB), "-lov2b200", "-lpthread", "-Wl,-rpath,$ORIGIN"])
+    return exe
+
+
+def build_rect_shim(verbose: bool = False) -> Path:
+    """Compile the drop-in CameraCalibration::rectifyImage (host/camera_calibration_rect_gpu.cpp) against the stand-in
+    calibration / OpenCV headers and link its self-test driver."""
+    host = ROOT / "host"
+    build()
+    objs = []
+    deps = list((host / "standin").rglob("*"))
+    for name in ("camera_calibration_rect_gpu.cpp", "rect_selftest.cpp"):
+        obj = LIB / "obj" / (name + ".o")
+        src = host / name
+        if _newer(src, obj) or any(d.is_file() and _newer(d, obj) for d in deps):
+            cmd = ["g++", "-std=c++17", "-O2", "-Wall", "-fPIC", "-I", str(host / "standin" / "ref"), "-I", str(host / "standin"),
+                   "-c", str(src), "-o", str(obj)]
+            if verbose:
+                print(" ".join(cmd), flush=True)
+            subprocess.check_call(cmd)
+        objs.append(str(obj))
+    exe = LIB / "rect_selftest"
     subprocess.check_call(["g++", "-o", str(exe), *objs, "-L", str(LIB), "-lov2b200", "-lpthread", "-Wl,-rpath,$ORIGIN"])
     return exe
 

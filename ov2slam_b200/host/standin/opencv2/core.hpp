@@ -12,6 +12,9 @@
 #define OV2_STANDIN_OPENCV 1
 #define CV_8U 0
 #define CV_8UC1 0
+#define CV_16UC1 2
+#define CV_32FC1 5
+#define CV_16SC2 11
 
 namespace cv {
 
@@ -36,23 +39,32 @@ struct TermCriteria {
 
 template <typename T> using Ptr = std::shared_ptr<T>;
 
-// 8-bit single-channel matrix with shared, ref-counted storage (what the shim needs of cv::Mat)
+// matrix with shared, ref-counted storage (what the shims need of cv::Mat): 8-bit images, and the CV_16SC2 / CV_16UC1 /
+// CV_32FC1 rectification maps
 class Mat {
 public:
     int rows = 0, cols = 0;
     size_t step = 0;
     unsigned char* data = nullptr;
     Mat() {}
-    Mat(int r, int c, int /*type*/) : rows(r), cols(c), step((size_t)c), buf_(new unsigned char[(size_t)r * c], std::default_delete<unsigned char[]>()) { data = buf_.get(); }
-    Mat(int r, int c, int /*type*/, void* ext, size_t st = 0) : rows(r), cols(c), step(st ? st : (size_t)c), data((unsigned char*)ext) {}
+    Mat(int r, int c, int type) { create(r, c, type); }
+    Mat(int r, int c, int type, void* ext, size_t st = 0) : rows(r), cols(c), step(st ? st : (size_t)c * esz(type)), data((unsigned char*)ext), type_(type) {}
+    void create(int r, int c, int type) {
+        if (data && r == rows && c == cols && type == type_) return;
+        rows = r; cols = c; type_ = type; step = (size_t)c * esz(type);
+        buf_.reset(new unsigned char[(size_t)r * step], std::default_delete<unsigned char[]>());
+        data = buf_.get();
+    }
     bool empty() const { return data == nullptr || rows == 0 || cols == 0; }
-    int type() const { return CV_8UC1; }
+    int type() const { return type_; }
     Size size() const { return Size(cols, rows); }
     unsigned char* ptr(int r = 0) { return data + (size_t)r * step; }
     const unsigned char* ptr(int r = 0) const { return data + (size_t)r * step; }
-    Mat row(int r) const { Mat m; m.rows = 1; m.cols = cols; m.step = step; m.data = data + (size_t)r * step; m.buf_ = buf_; return m; }
+    Mat row(int r) const { Mat m; m.rows = 1; m.cols = cols; m.step = step; m.data = data + (size_t)r * step; m.buf_ = buf_; m.type_ = type_; return m; }
 private:
+    static size_t esz(int type) { return type == CV_16UC1 ? 2 : (type == CV_32FC1 || type == CV_16SC2) ? 4 : 1; }
     std::shared_ptr<unsigned char> buf_;
+    int type_ = CV_8UC1;
 };
 
 class CLAHE { public: virtual ~CLAHE() {} virtual void apply(const Mat&, Mat&) = 0; };

@@ -48,6 +48,11 @@ public:
     cv::Point2f projectCamToImageDist(const Eigen::Vector3d& pt) const {
         return cv::Point2f((float)(fx_ * pt.x() / pt.z() + cx_), (float)(fy_ * pt.y() / pt.z() + cy_));
     }
+    // rectification (camera_calibration.hpp:67,116,120): the maps setUndistStereoMap / setUndistMap build, and the lock
+    // rectifyImage takes; the body is the drop-in of host/camera_calibration_rect_gpu.cpp
+    void rectifyImage(const cv::Mat& img, cv::Mat& rect) const;
+    cv::Mat undist_map_x_, undist_map_y_;
+    mutable std::mutex intrinsic_mutex_, extrinsic_mutex_;
 };
 
 struct Keypoint {
