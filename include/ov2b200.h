@@ -160,7 +160,11 @@ typedef struct {
  * or NULL to use nbpyrlvl_all for every keypoint.  kps = vkps (n x 2 float), priors_inout =
  * vpriorkps (in: initial guess, out: forward result), status_out = vkpstatus (n bytes, 0/1).
  * Keypoints with x < 0 are empty-slot markers of fixed-stride batches (the detectors pad with (-1, -1)):
- * status 0, prior untouched. */
+ * status 0, prior untouched.
+ * Depths are clamped as the reference clamps nbpyrlvl (feature_tracker.cpp:50-52): to the depth
+ * cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), levels - 1) reaches, i.e. never to a level
+ * whose width or height is <= win.  On small images that is shallower than the pyramid's levels
+ * (96x72 and 64x48: 2, 40x30: 1, 17x16: 0); the levels themselves stay exact pyrDown images. */
 OV2_API ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
                       int n, const int32_t* frame_idx, int first_frame, int per_frame,
                       const uint8_t* nbpyrlvl, int nbpyrlvl_all,

@@ -82,8 +82,28 @@ def stdsort_desc(resp) -> np.ndarray:
 
 # ------------------------------------------------------------------ P: pyramid + Scharr
 def _reflect101(idx, n):
-    idx = np.abs(idx)
-    return np.where(idx >= n, 2 * (n - 1) - idx, idx)
+    """cv::borderInterpolate(idx, n, BORDER_REFLECT_101): reflected until inside [0, n) (an index can overshoot by
+    more than n on a level narrower than the window); n == 1 maps everything to 0."""
+    idx = np.asarray(idx)
+    if n == 1:
+        return np.zeros_like(idx)
+    while True:
+        idx = np.abs(idx)
+        over = idx >= n
+        if not over.any():
+            return idx
+        idx = np.where(over, 2 * (n - 1) - idx, idx)
+
+
+def optflow_levels(w: int, h: int, win: int = 9, maxlevel: int = 3) -> int:
+    """The pyramid depth cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), maxlevel) reaches (its return value): it
+    stops before a level whose width or height would be <= win.  calcOpticalFlowPyrLK tracks from that depth, and the
+    reference clamps nbpyrlvl to it (feature_tracker.cpp:50-52)."""
+    for level in range(maxlevel):
+        w, h = (w + 1) // 2, (h + 1) // 2
+        if w <= win or h <= win:
+            return level
+    return maxlevel
 
 
 def pyr_down_ref(img: np.ndarray) -> np.ndarray:
@@ -552,7 +572,8 @@ def _fb_klt(lk, prev, cur, kps, priors, win, nbpyrlvl, ferr, fb_dist, maxit, eps
     if n == 0:
         return pri, status
     h, w = cur.shape
-    nbpyrlvl = min(int(nbpyrlvl), 3)  # pyramid built with 3 extra levels (feature_tracker.cpp:50-52)
+    # pyramid built with at most 3 extra levels, fewer on small images (feature_tracker.cpp:50-52)
+    nbpyrlvl = min(int(nbpyrlvl), optflow_levels(w, h, win, 3))
     fwd, st, err = lk(prev, cur, kps, pri, nbpyrlvl, win, maxit, eps)
     pri[:] = fwd  # vpriorkps is in/out
     idx = []

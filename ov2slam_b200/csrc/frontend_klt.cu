@@ -604,6 +604,15 @@ ov2_status launch_klt(ov2_ctx* ctx, KltArgs& A, bool persistent) {
     return OV2_OK;
 }
 
+// Depth cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), maxlevel) reaches: it stops before a level whose width or
+// height would be <= win.  calcOpticalFlowPyrLK tracks from there, and the reference clamps nbpyrlvl to it
+// (feature_tracker.cpp:50-52), so on small images the tracker starts at a shallower level than the pyramid holds.
+int optflow_levels(const ov2_pyr* p, int win, int maxlevel) {
+    for (int l = 0; l < maxlevel; ++l)
+        if (p->w[l + 1] <= win || p->h[l + 1] <= win) return l;
+    return maxlevel;
+}
+
 }  // namespace
 
 extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
@@ -623,6 +632,8 @@ extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_py
     KltArgs A;
     A.prev = make_view(prev);
     A.cur = make_view(cur);
+    // every depth clamp of the kernels reads prev.nlev
+    A.prev.nlev = A.cur.nlev = optflow_levels(prev, prm->win, A.prev.nlev - 1) + 1;
     A.n = n;
     A.first_frame = first_frame;
     A.per_frame = per_frame;

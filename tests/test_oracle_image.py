@@ -64,15 +64,30 @@ def test_golden_klt(gold):
 
 @needs_cv2
 def test_pyramid_and_scharr_vs_cv2():
+    """pyrDown levels and Scharr planes, from the working sizes down to the 16 x 16 minimum of ov2_pyr_create (odd sizes,
+    levels of 1 - 2 px at 4 extra levels); the depth buildOpticalFlowPyramid reaches (optflow_levels); reflect-101
+    indices that overshoot by more than the image size."""
     import cv2
-    for w, h in ((640, 480), (333, 245)):
+    sizes = [(640, 480), (333, 245), (1241, 376), (161, 83), (100, 70), (57, 64), (56, 64), (96, 72), (64, 48), (40, 30)]
+    sizes += [(w, h) for w in range(16, 40, 3) for h in (16, 17, 23, 31)]
+    for w, h in sizes:
         im = synth.make_frame(7, w, h)
-        for a, b in zip(R.build_pyramid_ref(im), R.build_pyramid_cv2(im)):
-            assert np.array_equal(a, b)
+        ref = R.build_pyramid_ref(im, 4)
+        for l, (a, b) in enumerate(zip(ref, R.build_pyramid_cv2(im, 4))):
+            assert np.array_equal(a, b), (w, h, l)
         n, pyr = cv2.buildOpticalFlowPyramid(im, (9, 9), 3)
-        for l in range(4):
-            ix, iy = R.scharr_ref(R.build_pyramid_ref(im)[l])
-            assert np.array_equal(pyr[2 * l + 1][..., 0], ix) and np.array_equal(pyr[2 * l + 1][..., 1], iy)
+        assert n == R.optflow_levels(w, h) and len(pyr) == 2 * (n + 1), (w, h, n)
+        for l in range(n + 1):
+            ix, iy = R.scharr_ref(ref[l])
+            assert np.array_equal(pyr[2 * l + 1][..., 0], ix) and np.array_equal(pyr[2 * l + 1][..., 1], iy), (w, h, l)
+    zero = np.zeros((1, 1), np.uint8)
+    for w in range(16, 205):
+        for h in (16, 17, 19, 20, 23, 37, 38, 39, 40, 41, 75, 76, 77, 150, 199):
+            n, _ = cv2.buildOpticalFlowPyramid(np.broadcast_to(zero, (h, w)).copy(), (9, 9), 3, withDerivatives=False)
+            assert R.optflow_levels(w, h) == n, (w, h, n)
+    for n in (1, 2, 3, 5, 12):
+        idx = np.arange(-40, 41)
+        assert np.array_equal(R._reflect101(idx, n), [cv2.borderInterpolate(int(i), n, cv2.BORDER_REFLECT_101) for i in idx]), n
 
 
 @needs_cv2
@@ -161,6 +176,23 @@ def test_klt_vs_cv2():
         tb, sb = R.fb_klt_ref(prev, cur, kps, pri, 9, lvl)
         assert np.array_equal(sa, sb)
         assert np.abs(ta - tb).max() <= 1e-3
+    # small images: buildOpticalFlowPyramid stops before a level <= 9 px, so calcOpticalFlowPyrLK tracks from fewer levels
+    # than asked (96 x 72 and 64 x 48: 2, 40 x 30: 1, 17 x 16: 0), and windows overshoot the narrow levels by more than
+    # one reflection.  Statuses identical, tracked positions within the GPU suite's cv2 tolerance (1e-2 px; a lost track
+    # can end anywhere).
+    for w, h in ((17, 16), (40, 30), (64, 48), (96, 72), (161, 83), (333, 245)):
+        prev, cur, _ = synth.make_pair(7, w, h)
+        rng = np.random.default_rng(w)
+        kps = (rng.random((150, 2)) * [w, h]).astype(np.float32)
+        kps[:4] = [[1.0, 1.0], [w - 1.0, h / 2], [w / 2, h - 1.0], [w - 1.5, h - 1.5]]
+        pri = (kps + rng.uniform(-1.5, 1.5, kps.shape)).astype(np.float32)
+        for lvl in (1, 3):
+            ta, sa = R.fb_klt_cv2(prev, cur, kps, pri, 9, lvl)
+            tb, sb = R.fb_klt_ref(prev, cur, kps, pri, 9, lvl)
+            assert np.array_equal(sa, sb), (w, h, lvl, np.nonzero(sa != sb)[0])
+            ok = sa.astype(bool)
+            assert ok.sum() >= 10, (w, h, lvl)
+            assert np.abs(ta[ok] - tb[ok]).max() <= 1e-2, (w, h, lvl, np.abs(ta[ok] - tb[ok]).max())
 
 
 @needs_cv2
