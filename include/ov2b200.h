@@ -203,8 +203,14 @@ OV2_API ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, int
                          double* quality_inout, int max_per_frame,
                          float* out_pts, int32_t* out_counts, int32_t* out_pts_int, int do_subpix);
 
+/* Largest number of FAST candidates (strict 3x3 maxima at cell-local x % 4 in {2, 3}) a cell of `cellsize` can hold:
+ * ((cellsize - 6) / 4 + 1) * ((cellsize - 5) / 2), e.g. 264 at 50 and 1891 at 128; 0 outside [8, 128].  ov2_grid_fast
+ * keeps that many per cell, so no input is refused for its content. */
+OV2_API int ov2_fast_cell_capacity(int cellsize);
+
 /* Test hook: stage F1 alone (per-cell FAST-9/16 + NMS candidates of one frame, pre-filtered by the
- * mask byte rule), for cell-by-cell parity against cv::FastFeatureDetector. */
+ * mask byte rule), for cell-by-cell parity against cv::FastFeatureDetector.  cap_in >= ov2_fast_cell_capacity(cellsize)
+ * words per cell. */
 OV2_API ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int frame, int cellsize, int fast_th,
                                 uint32_t* cand_out, int32_t* cand_n_out, int cap_in, int* cap_out);
 
@@ -300,7 +306,7 @@ OV2_API ov2_status ov2_match_to_map(ov2_ctx* ctx, const ov2_match_problem* p, in
  * host or device as everywhere; n_kps = count * kps_per_frame; cellsize <= 0 skips F/B(new).
  * The step is captured into a CUDA graph per distinct argument block (at most 16 are kept per context): zero the struct
  * before filling it (its padding bytes are part of the cache key), and reuse argument blocks - a block that changes every
- * call runs eagerly.  A detector cell that exceeds its candidate capacity makes the call return OV2_ERR_CAPACITY. */
+ * call runs eagerly. */
 typedef struct {
     const uint8_t* prev_images; const uint8_t* cur_images; size_t row_stride, frame_stride; int count;
     ov2_klt_params klt; int n_kps, kps_per_frame; const uint8_t* nbpyrlvl; int nbpyrlvl_all;

@@ -243,12 +243,13 @@ def _cv_round(v) -> int:
     return int(np.rint(np.float32(v)))
 
 
-def detect_grid_fast_nosubpix(im: np.ndarray, cellsize: int, curkps, fast_th: int, use_cv2: bool):
+def detect_grid_fast_nosubpix(im: np.ndarray, cellsize: int, curkps, fast_th: int, use_cv2: bool, stats=None):
     """FeatureExtractor::detectGridFAST up to (not including) cornerSubPix
     (feature_extractor.cpp:443-552), with the *sequential* ascending cell order as the defined
     semantics (the reference's parallel_for_ body races on `mask`; SURVEY.md section 2.1).
 
-    Returns (pts int32[N, 2] in cell order, new_fast_th, nbempty).
+    Returns (pts int32[N, 2] in cell order, new_fast_th, nbempty).  `stats`, if a list, receives
+    (cell, survivors, survivors with the maximal response) for every cell that had a survivor.
     """
     rows, cols = im.shape
     r4 = cellsize // 4
@@ -289,6 +290,9 @@ def detect_grid_fast_nosubpix(im: np.ndarray, cellsize: int, curkps, fast_th: in
                     cand.append((kx, ky, resp))
         if not cand:
             continue
+        if stats is not None:
+            top = max(k[2] for k in cand)
+            stats.append((i, len(cand), sum(k[2] == top for k in cand)))
         order = stdsort_desc([k[2] for k in cand])
         best = cand[int(order[0])]
         if best[2] >= 20:

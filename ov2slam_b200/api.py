@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_sharded", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_sharded", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -134,6 +134,8 @@ def load():
     lib.ov2_grid_fast.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_detect_single_scale.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_pnp_solve.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, C.c_float, i32, i32, vp, vp, vp]
+    lib.ov2_fast_cell_capacity.argtypes = [i32]
+    lib.ov2_fast_cell_capacity.restype = i32
     lib.ov2_debug_fast_cells.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, C.POINTER(i32)]
     lib.ov2_describe.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp]
     lib.ov2_describe_config.argtypes = [vp, i32, vp]
@@ -461,15 +463,22 @@ class FeatureExtractor:
         return pts[:cnt[0]].copy(), ipts[:cnt[0]].copy()
 
     def debug_fast_cells(self, pyr: Pyramid, frame: int, ncellsize: int, fast_th: int):
-        """Stage F1 only: list per cell of (x, y, response) candidates (cell-local, scan order)."""
+        """Stage F1 only: list per cell of (x, y, response) candidates (cell-local, scan order).  The per-cell capacity
+        the hook reports is left in self.last_fast_cell_cap."""
         ncell = (pyr.h // ncellsize) * (pyr.w // ncellsize)
-        cand = np.zeros((ncell, 128), np.uint32)
+        cap_in = self.fast_cell_capacity(ncellsize)
+        cand = np.zeros((ncell, max(cap_in, 1)), np.uint32)
         cn = np.zeros(ncell, np.int32)
         cap = C.c_int()
         self.ctx.check(self.ctx.lib.ov2_debug_fast_cells(self.ctx.h, pyr.h_, frame, ncellsize, int(fast_th),
-                                                         cand.ctypes.data, cn.ctypes.data, 128, C.byref(cap)))
+                                                         cand.ctypes.data, cn.ctypes.data, cap_in, C.byref(cap)))
+        self.last_fast_cell_cap = cap.value
         flat = cand.reshape(-1)[:ncell * cap.value].reshape(ncell, cap.value)
         return [[(int(v & 255), int((v >> 8) & 255), float(v >> 16)) for v in flat[c, :cn[c]]] for c in range(ncell)]
+
+    def fast_cell_capacity(self, ncellsize: int) -> int:
+        """ov2_fast_cell_capacity: the most FAST candidates a cell of this size can hold (0 for an unsupported size)."""
+        return int(self.ctx.lib.ov2_fast_cell_capacity(int(ncellsize)))
 
     DESC_ORB_FALLBACK, DESC_BRIEF32 = 0, 1
 

@@ -45,8 +45,6 @@ extern "C" void ov2_destroy(ov2_ctx* ctx) {
     if (ctx->ba_stop) cudaFreeHost(ctx->ba_stop);
     if (ctx->ba_ws) cudaFreeHost(ctx->ba_ws);   // pinned staging block of the BA path
     if (ctx->desc_table) cudaFree(ctx->desc_table);
-    if (ctx->cap_flag_dev) cudaFree(ctx->cap_flag_dev);
-    if (ctx->cap_flag_host) cudaFreeHost(ctx->cap_flag_host);
     if (ctx->pe0) { cudaEventDestroy(ctx->pe0); cudaEventDestroy(ctx->pe1); }
     if (ctx->sync_ev) cudaEventDestroy(ctx->sync_ev);
     if (ctx->upload_ev) cudaEventDestroy(ctx->upload_ev);
@@ -227,30 +225,6 @@ ov2_status ov2_end(ov2_ctx* ctx) {
     return ov2_wait_stream(ctx);
 }
 
-ov2_status ov2_cap_flag_get(ov2_ctx* ctx, int** dev) {
-    if (!ctx->cap_flag_dev) {
-        OV2_CUDA(ctx, cudaMalloc(&ctx->cap_flag_dev, sizeof(int)));
-        OV2_CUDA(ctx, cudaMemset(ctx->cap_flag_dev, 0, sizeof(int)));
-        OV2_CUDA(ctx, cudaHostAlloc(&ctx->cap_flag_host, sizeof(int), cudaHostAllocDefault));
-        *ctx->cap_flag_host = 0;
-    }
-    *dev = ctx->cap_flag_dev;
-    return OV2_OK;
-}
-
-ov2_status ov2_cap_flag_mirror(ov2_ctx* ctx) {
-    if (!ctx->cap_flag_dev) return OV2_OK;
-    OV2_CUDA(ctx, cudaMemcpyAsync(ctx->cap_flag_host, ctx->cap_flag_dev, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    return OV2_OK;
-}
-
-ov2_status ov2_cap_flag_check(ov2_ctx* ctx, const char* who) {
-    if (!ctx->cap_flag_host || *ctx->cap_flag_host == 0) return OV2_OK;
-    *ctx->cap_flag_host = 0;
-    OV2_CUDA(ctx, cudaMemsetAsync(ctx->cap_flag_dev, 0, sizeof(int), ctx->stream));
-    return ov2_fail(ctx, OV2_ERR_CAPACITY, who);
-}
-
 extern "C" ov2_status ov2_batch_begin(ov2_ctx* ctx) {
     if (!ctx) return OV2_ERR_INVALID;
     if (ctx->batch) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_batch_begin: batch already open");
@@ -280,9 +254,7 @@ extern "C" ov2_status ov2_batch_end(ov2_ctx* ctx) {
     ctx->batch = false;
     ov2_status fst = ov2_batch_flush_outputs(ctx);
     if (fst != OV2_OK) return fst;
-    fst = ov2_wait_stream(ctx);
-    if (fst != OV2_OK) return fst;
-    return ov2_cap_flag_check(ctx, "ov2_batch_end: a detector cell exceeded its candidate capacity in this batch");
+    return ov2_wait_stream(ctx);
 }
 
 // ------------------------------------------------------------------------ pyramid storage

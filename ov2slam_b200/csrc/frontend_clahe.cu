@@ -271,7 +271,10 @@ extern "C" ov2_status ov2_clahe(ov2_ctx* ctx, const uint8_t* src, uint8_t* dst, 
     const void* d = nullptr;
     void* o = nullptr;
     if ((st = ov2_stage_in(ctx, src, bytes, &d)) != OV2_OK) return st;
-    if ((st = ov2_stage_out(ctx, dst, bytes, &o)) != OV2_OK) return st;
+    // a host dst is copied back over the whole span: when rows or frames leave gaps (a ROI of a wider image), stage its
+    // current bytes first so the gaps come back unchanged
+    const bool gaps = row_stride != (size_t)width || (count > 1 && frame_stride != row_stride * (size_t)height);
+    if ((st = ov2_stage_out(ctx, dst, bytes, &o, gaps)) != OV2_OK) return st;
     if ((st = clahe_device(ctx, (const uint8_t*)d, (int)row_stride, (long long)frame_stride, (uint8_t*)o, (int)row_stride,
                            (long long)frame_stride, width, height, count, clip_limit, tiles_x, tiles_y)) != OV2_OK)
         return st;

@@ -38,6 +38,12 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int MAX_CELL = 128;
 constexpr int MAX_RADIUS = MAX_CELL / 4;
 
+// Largest number of candidates a cell of size cs can hold.  A candidate lies in the interior [3, cs - 3)^2 at cell-local
+// x % 4 in {2, 3} and is a strict 3x3 maximum.  The nk = (cs - 6) / 4 + 1 column groups {4k + 2, 4k + 3} that meet the
+// interior hold at most one per row (the two columns are neighbours) and none in two adjacent rows (diagonal neighbours),
+// so at most ceil((cs - 6) / 2) each.  A dot lattice with one dot per group every second row reaches the bound.
+__host__ __device__ constexpr int fast_cell_cap(int cs) { return ((cs - 6) / 4 + 1) * ((cs - 5) / 2); }
+
 // FAST ring, clockwise from 12 o'clock (SURVEY.md A.1)
 __host__ __device__ constexpr int ring_dx(int k) {
     constexpr int dx[16] = {0, 1, 2, 3, 3, 3, 2, 1, 0, -1, -2, -3, -3, -3, -2, -1};
@@ -51,7 +57,6 @@ struct FastArgs {
     const int32_t* th;          // [count] threshold per frame
     uint32_t* cand;             // [count][ncells][cap]  (resp << 16) | (ky << 8) | kx
     int32_t* cand_n;            // [count][ncells]
-    int32_t* overflow;          // set to 1 if a cell had more than cap candidates
 };
 
 // Shared-memory layout of fast_cells_kernel (bytes), shared by the kernel and its launch.
@@ -267,21 +272,27 @@ __global__ void fast_cells_kernel(FastArgs A, const __grid_constant__ CUtensorMa
                 const int p = n + __popc(m0 & below) + __popc(m1 & below);
                 const unsigned t = base + lane, yy = nk > 1 ? __umulhi(t, rnk) : t, kk = t - yy * nk;
                 const uint32_t yx = ((yy + 3u) << 8) | (4u * kk + 2u);
-                if (s0 && p < A.cap) out[p] = ((s0 - 1u) << 16) | yx;
-                if (s1 && p + (s0 != 0u) < A.cap) out[p + (s0 != 0u)] = ((s1 - 1u) << 16) | (yx + 1u);
+                // n never exceeds fast_cell_cap(cs), so every candidate has a slot
+                if (s0) out[p] = ((s0 - 1u) << 16) | yx;
+                if (s1) out[p + (s0 != 0u)] = ((s1 - 1u) << 16) | (yx + 1u);
             }
             n += __popc(m0) + __popc(m1);
         }
-        if (lane == 0) {
-            if (n > A.cap) { atomicExch(A.overflow, 1); n = A.cap; }
-            *out_n = n;
-        }
+        if (lane == 0) *out_n = n;
     }
 }
 
 // ---------------------------------------------------------------------------------- F2
+// Sort keys are (response << 16) | candidate index (stdsort_emul.h).
+constexpr int SKEY_SHIFT = 16;
+constexpr int SKEY_IDX = (1 << SKEY_SHIFT) - 1;
+// fast_sweep_wave_kernel holds up to WAVE_REG_CAND candidates of a cell in registers (four per lane) and their sort keys in
+// shared memory; a cell with more candidates reads them from the list and sorts in a global area (SweepArgs::skey_g).
+constexpr int WAVE_REG_CAND = 128;
+
 struct SweepArgs {
     int w, h, cs, nwc, nhc, cap, radius, max_per_frame;
+    int* skey_g;                     // wave kernel: [count][warps][cap] sort keys of cells with > WAVE_REG_CAND candidates
     int hw[MAX_RADIUS + 1];          // cv::circle half-widths per |dy|
     const int32_t* kp_off;           // [count+1] or NULL
     const float2* kps;               // existing keypoints
@@ -364,7 +375,7 @@ __global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
             unsigned m = __ballot_sync(FULL, ok);
             if (ok) {
                 int pos = ns + __popc(m & ((1u << lane) - 1));
-                skey[pos] = (int)((cd >> 16) << 8) | j;   // (response << 8) | candidate index
+                skey[pos] = (int)((cd >> 16) << SKEY_SHIFT) | j;   // (response << 16) | candidate index
                 vmax = max(vmax, (int)(cd >> 16));
             }
             ns += __popc(m);
@@ -376,7 +387,7 @@ __global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
         int nmax = 0, firstmax = 0x7fffffff;
         for (int base = 0; base < ns; base += 32) {
             int j = base + lane;
-            bool is = j < ns && (skey[j] >> 8) == vmax;
+            bool is = j < ns && (skey[j] >> SKEY_SHIFT) == vmax;
             unsigned m = __ballot_sync(FULL, is);
             if (m && firstmax == 0x7fffffff) firstmax = base + __ffs(m) - 1;
             nmax += __popc(m);
@@ -384,11 +395,11 @@ __global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
         int win_j;
         if (nmax == 1 || ns <= 16) {
             // unique maximum, or libstdc++ falls straight to (stable) insertion sort
-            win_j = skey[firstmax] & 255;
+            win_j = skey[firstmax] & SKEY_IDX;
         } else {
             if (lane == 0) ov2sort::sort_desc(skey, ns);
             __syncwarp();
-            win_j = skey[0] & 255;
+            win_j = skey[0] & SKEY_IDX;
         }
         __syncwarp();
         if (vmax >= 20) {   // vkps.at(0).response >= 20
@@ -430,10 +441,12 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
     const int wpr = (A.w + 31) >> 5, ncells = A.nwc * A.nhc;
     uint32_t* bm = sm;                                                        // h * wpr words, bit = 1: mask is 0.0f there
     int2* det = reinterpret_cast<int2*>(sm + (((size_t)A.h * wpr + 1) & ~(size_t)1));   // per cell, x < 0: none
-    int* skey_all = reinterpret_cast<int*>(det + ncells);                    // [nwarps][cap] sort keys
-    volatile int* progress = reinterpret_cast<volatile int*>(skey_all + (size_t)nwarps * A.cap);   // [nhc]
+    const int nskey = min(A.cap, WAVE_REG_CAND);
+    int* skey_all = reinterpret_cast<int*>(det + ncells);                    // [nwarps][nskey] sort keys
+    volatile int* progress = reinterpret_cast<volatile int*>(skey_all + (size_t)nwarps * nskey);   // [nhc]
     uint8_t* occ = reinterpret_cast<uint8_t*>(const_cast<int*>(progress) + A.nhc);       // (nhc+1)*(nwc+1)
-    int* skey = skey_all + (size_t)warp * A.cap;
+    int* skey_sm = skey_all + (size_t)warp * nskey;
+    int* skey_big = A.skey_g ? A.skey_g + ((size_t)fr * nwarps + warp) * A.cap : nullptr;
     for (int i = tid; i < A.h * wpr; i += nthreads) bm[i] = 0;
     for (int i = tid; i < ncells; i += nthreads) det[i] = make_int2(-1, -1);
     for (int i = tid; i < A.nhc; i += nthreads) progress[i] = 0;
@@ -466,12 +479,13 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
             const bool search = !occ[r * (A.nwc + 1) + c] && (x0 + A.cs < A.w - 1 && y0 + A.cs < A.h - 1);
             // the cell's candidates do not depend on any other cell: fetch them before waiting for the neighbours
             const int n = search ? cand_n[cell] : 0;
-            uint32_t cdv[4] = {0u, 0u, 0u, 0u};                                // cap <= 128: four candidates per lane
+            const uint32_t* ccand = cand + (size_t)cell * A.cap;
+            uint32_t cdv[4] = {0u, 0u, 0u, 0u};                                // the first WAVE_REG_CAND: four per lane
             if (n > 0) {
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                     const int j = 32 * q + lane;
-                    if (j < n) cdv[q] = __ldg(cand + (size_t)cell * A.cap + j);
+                    if (j < n) cdv[q] = __ldg(ccand + j);
                 }
             }
             if (r > 0) {
@@ -480,14 +494,12 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
                 __threadfence_block();
             }
             if (n > 0) {
-                // mask filter + ordered compaction of survivors into skey
+                // mask filter + ordered compaction of survivors into skey (shared memory, or the global area for big cells)
+                const bool big = n > WAVE_REG_CAND;                            // uniform
+                int* skey = big ? skey_big : skey_sm;
                 int ns = 0, vmax = -1;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int j = 32 * q + lane;
-                    if (32 * q >= n) break;                                    // uniform
+                auto filter = [&](uint32_t cd, int j) {
                     bool ok = false;
-                    const uint32_t cd = cdv[q];
                     if (j < n) {
                         const int kx = cd & 255, ky = (cd >> 8) & 255;
                         const int mx = x0 + (kx >> 2), my = y0 + ky;
@@ -496,10 +508,19 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
                     const unsigned m = __ballot_sync(FULL, ok);
                     if (ok) {
                         const int pos = ns + __popc(m & ((1u << lane) - 1));
-                        skey[pos] = (int)((cd >> 16) << 8) | j;                // (response << 8) | candidate index
+                        skey[pos] = (int)((cd >> 16) << SKEY_SHIFT) | j;       // (response << 16) | candidate index
                         vmax = max(vmax, (int)(cd >> 16));
                     }
                     ns += __popc(m);
+                };
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    if (32 * q >= n) break;                                    // uniform
+                    filter(cdv[q], 32 * q + lane);
+                }
+                for (int base = WAVE_REG_CAND; base < n; base += 32) {         // big cells only
+                    const int j = base + lane;
+                    filter(j < n ? __ldg(ccand + j) : 0u, j);
                 }
                 if (ns > 0) {
                     vmax = __reduce_max_sync(FULL, vmax);
@@ -507,24 +528,24 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
                     int nmax = 0, firstmax = 0x7fffffff;
                     for (int base = 0; base < ns; base += 32) {
                         const int j = base + lane;
-                        const bool is = j < ns && (skey[j] >> 8) == vmax;
+                        const bool is = j < ns && (skey[j] >> SKEY_SHIFT) == vmax;
                         const unsigned m = __ballot_sync(FULL, is);
                         if (m && firstmax == 0x7fffffff) firstmax = base + __ffs(m) - 1;
                         nmax += __popc(m);
                     }
                     int win_j;
                     if (nmax == 1 || ns <= 16) {
-                        win_j = skey[firstmax] & 255;                          // unique maximum / libstdc++'s insertion-sort range
+                        win_j = skey[firstmax] & SKEY_IDX;                     // unique maximum / libstdc++'s insertion-sort range
                     } else {
                         if (lane == 0) ov2sort::sort_desc(skey, ns);
                         __syncwarp();
-                        win_j = skey[0] & 255;
+                        win_j = skey[0] & SKEY_IDX;
                     }
                     __syncwarp();
                     if (vmax >= 20) {                                          // vkps.at(0).response >= 20
                         const int wq = win_j >> 5;                              // uniform
                         const uint32_t mine = wq == 0 ? cdv[0] : (wq == 1 ? cdv[1] : (wq == 2 ? cdv[2] : cdv[3]));
-                        const uint32_t cd = __shfl_sync(FULL, mine, win_j & 31);
+                        const uint32_t cd = win_j < WAVE_REG_CAND ? __shfl_sync(FULL, mine, win_j & 31) : __ldg(ccand + win_j);
                         const int px = x0 + (int)(cd & 255), py = y0 + (int)((cd >> 8) & 255);
                         if (lane == 0) det[cell] = make_int2(px, py);
                         for (int rI = lane; rI < nrows; rI += 32) {
@@ -766,12 +787,24 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     const int nwc = W / cellsize, nhc = H / cellsize, ncells = nwc * nhc;
     if (ncells == 0 || max_per_frame < ncells)
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_grid_fast: max_per_frame < number of cells");
+    const int cap = fast_cell_cap(cellsize);
+    // sweep: the wavefront kernel (one warp per cell row) unless its shared memory (mask bitmap, per-cell detections, per-warp
+    // sort keys, row progress, occupancy; the carve-up at the top of fast_sweep_wave_kernel) is over 200 KB or
+    // OV2_FAST_SWEEP=seq; else one warp per frame, which needs the bitmap, cap sort keys and the occupancy
+    const size_t wpr = (size_t)(W + 31) / 32;
+    const int nw = nhc < FSWEEP_MAX_WARPS ? nhc : FSWEEP_MAX_WARPS;
+    const int nskey = cap < WAVE_REG_CAND ? cap : WAVE_REG_CAND;
+    size_t wsmem = ((((size_t)H * wpr + 1) & ~(size_t)1)) * 4 + (size_t)nwc * nhc * 8 + (size_t)nw * nskey * 4 + (size_t)nhc * 4 +
+                   (size_t)(nhc + 1) * (nwc + 1);
+    wsmem = (wsmem + 15) & ~(size_t)15;
+    size_t smem = (size_t)H * wpr * 4 + (size_t)cap * 4 + (size_t)(nhc + 1) * (nwc + 1);
+    smem = (smem + 15) & ~(size_t)15;
+    const char* fs = getenv("OV2_FAST_SWEEP");
+    const bool wave = wsmem <= 200 * 1024 && !(fs && fs[0] == 's');
+    if (!wave && smem > 227 * 1024)
+        return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_grid_fast: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-    const int in_w = cellsize - 6;
-    int cap = ((in_w + 1) / 2) * ((in_w + 1) / 2);
-    if (cap > 128) cap = 128;
-    if (cap < 4) cap = 4;
 
     const void* d = nullptr;
     void* o = nullptr;
@@ -812,51 +845,39 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     d_int = (int2*)o;
     uint32_t* d_cand = nullptr;
     int32_t* d_candn = nullptr;
-    int32_t* d_ovf = nullptr;
     if ((st = ov2_scratch(ctx, sizeof(uint32_t) * (size_t)count * ncells * cap, &o)) != OV2_OK) return st;
     d_cand = (uint32_t*)o;
     if ((st = ov2_scratch(ctx, sizeof(int32_t) * (size_t)count * ncells, &o)) != OV2_OK) return st;
     d_candn = (int32_t*)o;
-    {   // sticky, context-owned flag (reported by this call when it synchronises, else by ov2_batch_end / ov2_frontend_step)
-        int* f = nullptr;
-        if ((st = ov2_cap_flag_get(ctx, &f)) != OV2_OK) return st;
-        d_ovf = (int32_t*)f;
+    int* d_skey = nullptr;      // sort keys of the wave kernel's cells with more candidates than it keeps in registers
+    if (wave && cap > WAVE_REG_CAND) {
+        if ((st = ov2_scratch(ctx, sizeof(int) * (size_t)count * nw * cap, &o)) != OV2_OK) return st;
+        d_skey = (int*)o;
     }
 
     FastArgs FA;
     FA.img = pyr->l0; FA.w = W; FA.h = H; FA.pitch = (int)pyr->l0_pitch; FA.fstride = (long long)pyr->l0_fstride;
     FA.first = first; FA.cs = cellsize; FA.nwc = nwc; FA.nhc = nhc; FA.cap = cap;
-    FA.th = d_th; FA.cand = d_cand; FA.cand_n = d_candn; FA.overflow = d_ovf;
+    FA.th = d_th; FA.cand = d_cand; FA.cand_n = d_candn;
     if ((st = launch_fast_cells(ctx, pyr, FA, count)) != OV2_OK) return st;
     SweepArgs SA;
     SA.w = W; SA.h = H; SA.cs = cellsize; SA.nwc = nwc; SA.nhc = nhc; SA.cap = cap;
     SA.radius = cellsize / 4; SA.max_per_frame = max_per_frame;
+    SA.skey_g = d_skey;
     circle_halfwidths(SA.radius, SA.hw);
     SA.kp_off = d_off; SA.kps = d_kps; SA.cand = d_cand; SA.cand_n = d_candn; SA.th = d_th;
     SA.out_int = d_int; SA.out_n = d_cnt;
-    {
-        size_t wpr = (size_t)(W + 31) / 32;
-        // wavefront sweep (one warp per cell row) unless the bitmap + per-warp sort keys do not fit, cap > 128 or OV2_FAST_SWEEP=seq
-        const int nw = nhc < FSWEEP_MAX_WARPS ? nhc : FSWEEP_MAX_WARPS;
-        size_t wsmem = ((((size_t)H * wpr + 1) & ~(size_t)1)) * 4 + (size_t)nwc * nhc * 8 + (size_t)nw * cap * 4 + (size_t)nhc * 4 +
-                       (size_t)(nhc + 1) * (nwc + 1);
-        wsmem = (wsmem + 15) & ~(size_t)15;
-        const char* fs = getenv("OV2_FAST_SWEEP");
-        if (cap <= 128 && wsmem <= 200 * 1024 && !(fs && fs[0] == 's')) {
-            static size_t wave_attr[16] = {0};
-            if (wsmem > 48 * 1024 && wsmem > wave_attr[ctx->device & 15]) {
-                OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-                wave_attr[ctx->device & 15] = wsmem;
-            }
-            OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_wave_kernel<<<count, nw * 32, wsmem, ctx->stream>>>(SA));
-        } else {
-        size_t smem = (size_t)H * wpr * 4 + (size_t)cap * 4 + (size_t)(nhc + 1) * (nwc + 1);
-        smem = (smem + 15) & ~(size_t)15;
-        if (smem > 227 * 1024) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_grid_fast: image too large for the shared-memory mask bitmap");
+    if (wave) {
+        static size_t wave_attr[16] = {0};
+        if (wsmem > 48 * 1024 && wsmem > wave_attr[ctx->device & 15]) {
+            OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
+            wave_attr[ctx->device & 15] = wsmem;
+        }
+        OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_wave_kernel<<<count, nw * 32, wsmem, ctx->stream>>>(SA));
+    } else {
         if (smem > 48 * 1024)
             OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_kernel<<<count, 32, smem, ctx->stream>>>(SA));
-        }
     }
     SubpixArgs PA;
     PA.img = pyr->l0; PA.w = W; PA.h = H; PA.pitch = (int)pyr->l0_pitch; PA.fstride = (long long)pyr->l0_fstride;
@@ -871,15 +892,11 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
         }
     }
     OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
-    // capacity overflow is an error, never a silent truncation: the flag's D2H mirror is enqueued behind the kernels (it is
-    // captured into the composite step's CUDA graph too); a call that synchronises reports it here, a call that only
-    // enqueues (batch mode, device outputs) leaves it to the next synchronising call of this context
-    const bool host_out = !ctx->pending.empty() && !ctx->batch;
-    if ((st = ov2_cap_flag_mirror(ctx)) != OV2_OK) return st;
-    st = ov2_end(ctx);
-    if (st != OV2_OK) return st;
-    if (host_out) return ov2_cap_flag_check(ctx, "ov2_grid_fast: per-cell candidate capacity exceeded");
-    return OV2_OK;
+    return ov2_end(ctx);
+}
+
+extern "C" int ov2_fast_cell_capacity(int cellsize) {
+    return cellsize < 8 || cellsize > MAX_CELL ? 0 : fast_cell_cap(cellsize);
 }
 
 // Test hook: the per-cell FAST candidate lists of one frame (stage F1 only), so the tests can
@@ -891,10 +908,7 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_debug_fast_cells: bad arguments");
     const int W = pyr->w[0], H = pyr->h[0];
     const int nwc = W / cellsize, nhc = H / cellsize, ncells = nwc * nhc;
-    const int in_w = cellsize - 6;
-    int cap = ((in_w + 1) / 2) * ((in_w + 1) / 2);
-    if (cap > 128) cap = 128;
-    if (cap < 4) cap = 4;
+    const int cap = fast_cell_cap(cellsize);
     if (cap_out) *cap_out = cap;
     if (cap_in < cap) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_debug_fast_cells: cap_in too small");
     ov2_status st = ov2_begin(ctx);
@@ -911,9 +925,6 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
     FA.cand = (uint32_t*)o;
     if ((st = ov2_stage_out(ctx, cand_n_out, sizeof(int32_t) * (size_t)ncells, &o)) != OV2_OK) return st;
     FA.cand_n = (int32_t*)o;
-    if ((st = ov2_scratch(ctx, sizeof(int32_t), &o)) != OV2_OK) return st;
-    FA.overflow = (int32_t*)o;
-    OV2_CUDA(ctx, cudaMemsetAsync(FA.overflow, 0, sizeof(int32_t), ctx->stream));
     if ((st = launch_fast_cells(ctx, pyr, FA, 1)) != OV2_OK) return st;
     return ov2_end(ctx);
 }

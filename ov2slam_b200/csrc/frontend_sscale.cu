@@ -333,6 +333,13 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
         if (ov2_is_device_ptr(roi_xywh)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_detect_single_scale: roi must be a host pointer");
         for (int i = 0; i < 4; ++i) roi[i] = roi_xywh[i];
     }
+    // ss_sweep_kernel's shared memory: mask bitmap, two detections per cell, row progress, occupancy
+    const size_t wpr = (size_t)(W + 31) / 32;
+    size_t sweep_smem = (((size_t)H * wpr + 1) & ~(size_t)1) * 4 + (size_t)ncells * sizeof(int2) * 2 + (size_t)nhc * sizeof(int) +
+                        (size_t)(nhc + 1) * (nwc + 1);
+    sweep_smem = (sweep_smem + 15) & ~(size_t)15;
+    if (sweep_smem > 227 * 1024)
+        return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_detect_single_scale: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
     const void* d = nullptr;
@@ -388,16 +395,10 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
     SA.roi_x = roi[0]; SA.roi_y = roi[1]; SA.roi_w = roi[2]; SA.roi_h = roi[3];
     SA.kp_off = d_off; SA.kps = d_kps; SA.resp = d_resp; SA.cellmax = d_cellmax; SA.quality = d_q; SA.out_int = d_int; SA.out_n = d_cnt;
     {
-        const size_t wpr = (size_t)(W + 31) / 32;
-        size_t smem = (((size_t)H * wpr + 1) & ~(size_t)1) * 4 + (size_t)ncells * sizeof(int2) * 2 + (size_t)nhc * sizeof(int) +
-                      (size_t)(nhc + 1) * (nwc + 1);
-        smem = (smem + 15) & ~(size_t)15;
-        if (smem > 227 * 1024)
-            return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_detect_single_scale: image too large for the shared-memory mask bitmap");
-        if (smem > 48 * 1024)
-            OV2_CUDA(ctx, cudaFuncSetAttribute(ss_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (sweep_smem > 48 * 1024)
+            OV2_CUDA(ctx, cudaFuncSetAttribute(ss_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sweep_smem));
         const int nw = nhc < SWEEP_MAX_WARPS ? nhc : SWEEP_MAX_WARPS;       // one warp per cell row (wavefront)
-        OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, smem, ctx->stream>>>(SA));
+        OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, sweep_smem, ctx->stream>>>(SA));
     }
     if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, do_subpix)) != OV2_OK) return st;
     return ov2_end(ctx);

@@ -148,6 +148,5 @@ extern "C" ov2_status ov2_frontend_step(ov2_ctx* ctx, ov2_pyr* prev, ov2_pyr* cu
         token.drop();
         if (ce != cudaSuccess) return ov2_fail(ctx, OV2_ERR_CUDA, "cudaEventSynchronize(upload)", ce);
     }
-    if ((st = ov2_wait_stream(ctx)) != OV2_OK) return st;
-    return ov2_cap_flag_check(ctx, "ov2_frontend_step: a detector cell exceeded its candidate capacity");
+    return ov2_wait_stream(ctx);
 }

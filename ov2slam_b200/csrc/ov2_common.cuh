@@ -39,11 +39,6 @@ struct ov2_ctx {
     // persistent small device blocks (tables)
     void* ba_ws = nullptr; size_t ba_ws_cap = 0;
     int desc_mode = 0;            // OV2_DESC_* (ov2_describe_config)
-    // sticky "a detector cell had more candidates than its capacity" flag: device word + pinned host mirror, so that calls
-    // that only enqueue (batch mode, device outputs, the graph-replayed composite step) still report OV2_ERR_CAPACITY at the
-    // next synchronising call instead of truncating silently
-    int* cap_flag_dev = nullptr;
-    int* cap_flag_host = nullptr;
     int8_t* desc_table = nullptr; // device copy of the BRIEF-32 test pairs [256][4]
     double* ba_hscal = nullptr;   // pinned: per-iteration scalar readbacks of the LM controller (legacy path)
     int* ba_stop = nullptr;       // mapped pinned int: stop request polled by the persistent solve kernel
@@ -128,9 +123,6 @@ ov2_status ov2_stage_in(ov2_ctx* ctx, const void* p, size_t bytes, const void** 
 ov2_status ov2_stage_out(ov2_ctx* ctx, void* p, size_t bytes, void** dev, bool copy_in = false);
 ov2_status ov2_end(ov2_ctx* ctx);                                 // D2H of pending outputs + sync if any
 ov2_status ov2_wait_stream(ov2_ctx* ctx);                         // sleep-wait for the context's stream
-ov2_status ov2_cap_flag_get(ov2_ctx* ctx, int** dev);             // lazily allocated sticky capacity flag (device word)
-ov2_status ov2_cap_flag_mirror(ov2_ctx* ctx);                     // enqueue its D2H copy into the pinned mirror
-ov2_status ov2_cap_flag_check(ov2_ctx* ctx, const char* who);     // after a sync: OV2_ERR_CAPACITY (and reset) if it was raised
 ov2_status ov2_batch_flush_outputs(ov2_ctx* ctx);                 // batch mode: enqueue the D2H copies (no wait)
 
 // pyramid build in two halves (frontend_step.cu orders the uploads of concurrent contexts)

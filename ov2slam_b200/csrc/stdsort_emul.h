@@ -6,7 +6,8 @@
 // keypoints share the maximal response the winner is decided by this exact sequence of
 // comparisons and swaps - which is what must be reproduced for bit-exact keypoints.
 //
-// Keys are (response, original index) pairs packed in one int: key = (response << 8) | index,
+// Keys are (response, original index) pairs packed in one int: key = (response << 16) | index
+// (response <= 254, index < 65536: a cell holds at most a few thousand candidates),
 // compared on the response part only.  Compiles for host (unit-tested against the real
 // std::sort in tests/test_stdsort_emul.py) and device (used by the grid-FAST sweep).
 #pragma once
@@ -20,7 +21,7 @@
 namespace ov2sort {
 
 // comp(a, b) == compare_response(a, b): strictly greater response
-OV2_HD bool gt(int a, int b) { return (a >> 8) > (b >> 8); }
+OV2_HD bool gt(int a, int b) { return (a >> 16) > (b >> 16); }
 OV2_HD void swp(int* v, int i, int j) { int t = v[i]; v[i] = v[j]; v[j] = t; }
 
 OV2_HD void move_median_to_first(int* v, int result, int a, int b, int c) {
@@ -116,8 +117,8 @@ OV2_HD void unguarded_insertion_sort(int* v, int first, int last) {
     }
 }
 
-// In-place std::sort of v[0..n) (n <= 256 here; the explicit stack replaces the recursion of
-// __introsort_loop, which recurses on the right part and iterates on the left).
+// In-place std::sort of v[0..n) (the explicit stack replaces the recursion of __introsort_loop,
+// which recurses on the right part and iterates on the left; it holds at most 2 log2(n) ranges).
 OV2_HD void sort_desc(int* v, int n) {
     if (n < 2) return;
     int lg = 0;

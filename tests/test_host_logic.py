@@ -11,9 +11,11 @@ import pytest
 ROOT = Path(__file__).resolve().parent.parent
 
 
-def test_stdsort_emulation_matches_libstdcxx(tmp_path):
+def test_stdsort_emulation_matches_libstdcxx_16bit_index(tmp_path):
     """ov2slam_b200/csrc/stdsort_emul.h compiled for the host vs the real std::sort (and
-    std::partial_sort for the heapsort fallback) on tie-heavy inputs."""
+    std::partial_sort for the heapsort fallback) on tie-heavy inputs.  Keys are (response << 16) | index; every fourth
+    input is up to 2 100 long, past the 1 891 candidates a 128-pixel FAST cell can hold, so indices above 255 and the
+    deep introsort / heapsort paths are pinned too."""
     src = tmp_path / "t.cpp"
     src.write_text(r'''
 #include "%s/ov2slam_b200/csrc/stdsort_emul.h"
@@ -24,19 +26,21 @@ def test_stdsort_emulation_matches_libstdcxx(tmp_path):
 struct Kp { float r; int idx; };
 static bool cmp(Kp a, Kp b) { return a.r > b.r; }
 int main() {
-  std::mt19937 rng(7); long bad = 0, badh = 0;
+  std::mt19937 rng(7); long bad = 0, badh = 0, nlong = 0;
   for (int it = 0; it < 60000; ++it) {
-    int n = 1 + rng() %% 200, nv = 1 + rng() %% (it %% 3 ? 6 : 40), pat = rng() %% 3;
+    int n = 1 + rng() %% (it %% 4 ? 200 : 2100), nv = 1 + rng() %% (it %% 3 ? 6 : 40), pat = rng() %% 3;
+    nlong += n > 1891;
     std::vector<Kp> v(n); std::vector<int> k(n);
-    for (int i = 0; i < n; ++i) { int r = 20 + (pat == 1 ? i %% nv : pat == 2 ? (n - i) / (1 + (int)(rng() %% 3)) : (int)(rng() %% nv));
-      v[i] = {(float)r, i}; k[i] = (r << 8) | i; }
+    for (int i = 0; i < n; ++i) { int r = pat == 1 ? i %% nv : pat == 2 ? (n - i) / (1 + (int)(rng() %% 3)) : (int)(rng() %% nv);
+      r = 20 + r %% 235;                                   // responses 20 .. 254, as FAST gives
+      v[i] = {(float)r, i}; k[i] = (r << 16) | i; }
     std::vector<Kp> w = v; std::vector<int> k2 = k;
     std::sort(v.begin(), v.end(), cmp); ov2sort::sort_desc(k.data(), n);
-    for (int i = 0; i < n; ++i) if ((k[i] & 255) != v[i].idx) { bad++; break; }
+    for (int i = 0; i < n; ++i) if ((k[i] & 0xFFFF) != v[i].idx) { bad++; break; }
     std::partial_sort(w.begin(), w.end(), w.end(), cmp); ov2sort::heap_sort(k2.data(), 0, n);
-    for (int i = 0; i < n; ++i) if ((k2[i] & 255) != w[i].idx) { badh++; break; }
+    for (int i = 0; i < n; ++i) if ((k2[i] & 0xFFFF) != w[i].idx) { badh++; break; }
   }
-  printf("%%ld %%ld\n", bad, badh); return (bad || badh) ? 1 : 0;
+  printf("%%ld %%ld %%ld\n", bad, badh, nlong); return (bad || badh || nlong < 1000) ? 1 : 0;
 }''' % ROOT)
     exe = tmp_path / "t"
     subprocess.check_call(["g++", "-O2", "-o", str(exe), str(src)])
