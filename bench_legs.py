@@ -421,7 +421,8 @@ def ba_bytes_per_iteration(nobs: int, npts: int) -> float:
 
 def c5_leg(torch, api, dist, ctx, rank, world, args, peaks, ncu_traffic=None):
     """1 GPU: ov2_localba_solve on the C5 window (host buffers in/out).  N GPUs: landmarks (with their observations)
-    split N ways, reduced camera system summed over NVLink every LM iteration (ov2_localba_solve_sharded)."""
+    split N ways, reduced camera system summed over NVLink peer memory inside the solve kernel every LM iteration
+    (ov2_localba_solve_p2p)."""
     from ov2slam_b200 import synth
     ncam, npts, nobs = C5 if not args.c5_small else (20, 3000, 18000)
     pb = synth.make_ba_problem(5, ncam, npts, nobs)

@@ -365,8 +365,8 @@ typedef struct {
 
 /* outlier_out (optional): [nobs] bytes, bit0 = flagged after solve #1, bit1 = after solve #2.
  * The whole two-stage solve (both Ceres solves, every LM iteration, both outlier scans) is ONE kernel launch with the
- * trust-region controller on the device (csrc/ba_lm.cu); OV2_BA_LEGACY=1 selects the round-1 path (one launch per phase,
- * controller on the host) as a cross-check.  At most 64 optimised and 256 total keyframes per window.
+ * trust-region controller on the device (csrc/ba_lm.cu).  At most 64 optimised keyframes per window (OV2_ERR_CAPACITY
+ * beyond); no limit on the total keyframe count (constant keyframes included).
  * Residency of a window's arrays is decided on `pose`: host poses = every array of the window (and outlier_out) is host
  * memory, the reference's flow; device poses = each array is inspected and may be either. */
 OV2_API ov2_status ov2_localba_solve(ov2_ctx* ctx, const ov2_ba_problem* pb, const ov2_ba_opts* opts,
@@ -392,7 +392,9 @@ OV2_API ov2_status ov2_localba_request_stop(ov2_ctx* ctx, int stop);
  * the ranks' partial reduced camera systems [cost, rhs, F'r, column norms, S] straight out of peer memory over NVLink
  * (rank order, so every rank holds bit-identical sums, solves the same system and takes the same decisions): no NCCL call
  * and no host round trip between iterations.  Poses come back identical on all ranks, inverse depths / flags / outlier
- * counts are the shard's own. */
+ * counts are the shard's own.  A window of more than 256 keyframes (constant ones included) is refused with
+ * OV2_ERR_CAPACITY when world > 1; every rank refuses it on the host before anything is launched, so no rank waits for a
+ * peer that never started.  With world == 1 the window is solved as ov2_localba_solve would. */
 typedef struct ov2_ba_comm ov2_ba_comm;
 OV2_API ov2_status ov2_ba_comm_create(ov2_ctx* ctx, int rank, int world, ov2_ba_comm** out);       /* world <= 8 */
 OV2_API ov2_status ov2_ba_comm_handle(ov2_ba_comm* comm, void* handle_out, size_t handle_bytes);    /* >= 64 bytes */
@@ -401,21 +403,6 @@ OV2_API ov2_status ov2_ba_comm_connect_local(ov2_ba_comm* comm, ov2_ba_comm* con
 OV2_API void       ov2_ba_comm_destroy(ov2_ba_comm* comm);
 OV2_API ov2_status ov2_localba_solve_p2p(ov2_ctx* ctx, ov2_ba_comm* comm, const ov2_ba_problem* pb, const ov2_ba_opts* opts,
                                  ov2_ba_result* res, uint8_t* outlier_out);
-
-/* Multi-GPU localBA, callback variant (round 1; the collective is whatever the caller wires in, e.g. ncclAllReduce):
- * landmarks (with all their observations) are
- * partitioned over ranks, every rank holds all keyframe poses.  `pb` describes THIS rank's shard
- * (ncam / pose / pose_const identical on all ranks; npts / nobs local, may be 0 observations).
- * Per LM iteration the partial reduced camera system [cost, rhs, F'r, column norms, S] is summed
- * over ranks by ONE call of `allreduce` (the caller wires it to ncclAllReduce / torch.distributed
- * over NVLink), followed by a 4-double collective for the candidate cost and model decrease; all
- * ranks then solve the same reduced system and take identical LM decisions (no broadcast).
- * allreduce(user, device_buf, count, cuda_stream): in-place SUM of `count` doubles on the given
- * stream (or synchronously); returns 0 on success.  Result counts (outliers) are per shard. */
-typedef int (*ov2_allreduce_fn)(void* user, double* device_buf, size_t count, void* cuda_stream);
-OV2_API ov2_status ov2_localba_solve_sharded(ov2_ctx* ctx, const ov2_ba_problem* pb, const ov2_ba_opts* opts,
-                                     ov2_ba_result* res, uint8_t* outlier_out, ov2_allreduce_fn allreduce,
-                                     void* user, int rank);
 
 #ifdef __cplusplus
 }

@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_sharded", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -83,9 +83,6 @@ class BaResult(C.Structure):
     _fields_ = [("iters_robust", C.c_int), ("iters_refine", C.c_int), ("initial_cost", C.c_double),
                 ("final_cost", C.c_double), ("n_outliers_first", C.c_int), ("n_outliers_second", C.c_int),
                 ("termination", C.c_int)]
-
-
-ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p)
 
 
 def lib_path() -> Path:
@@ -143,8 +140,6 @@ def load():
     lib.ov2_match_to_map.argtypes = [vp, C.POINTER(MatchProblem), vp, vp, vp, vp]
     lib.ov2_frontend_step.argtypes = [vp, vp, vp, C.POINTER(FrontendStepArgs)]
     lib.ov2_localba_solve.argtypes = [vp, C.POINTER(BaProblem), C.POINTER(BaOpts), C.POINTER(BaResult), vp]
-    lib.ov2_localba_solve_sharded.argtypes = [vp, C.POINTER(BaProblem), C.POINTER(BaOpts), C.POINTER(BaResult), vp,
-                                              ALLREDUCE_FN, vp, i32]
     lib.ov2_localba_solve_batch.argtypes = [vp, i32, C.POINTER(BaProblem), C.POINTER(BaOpts), C.POINTER(BaResult), vp]
     lib.ov2_localba_request_stop.argtypes = [vp, i32]
     lib.ov2_ba_comm_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
@@ -769,72 +764,18 @@ def partition_ba_problem(pb: dict, world: int):
     return shards
 
 
-class _CudaView:
-    """Zero-copy view of raw device memory for torch.as_tensor (CUDA array interface v2)."""
-
-    def __init__(self, ptr: int, count: int):
-        self.__cuda_array_interface__ = {"shape": (count,), "typestr": "<f8", "data": (ptr, False), "version": 2}
-
-
-def make_torch_allreduce(dist, torch, group=None):
-    """ov2_allreduce_fn that sums the buffer over the process group with torch.distributed
-    (NCCL over NVLink for device buffers; gloo for the CPU tests, where `buf` is host memory)."""
-    def _fn(user, buf, count, stream):
-        try:
-            if torch.cuda.is_available() and dist.get_backend(group) == "nccl":
-                t = torch.as_tensor(_CudaView(buf, count), device="cuda")
-                s = torch.cuda.ExternalStream(stream) if stream else torch.cuda.current_stream()
-                with torch.cuda.stream(s):
-                    dist.all_reduce(t, group=group)
-            else:
-                a = np.ctypeslib.as_array(C.cast(buf, C.POINTER(C.c_double)), shape=(count,))
-                t = torch.from_numpy(a)
-                dist.all_reduce(t, group=group)
-            return 0
-        except Exception as e:  # never let an exception cross the C boundary
-            print("[ov2b200] allreduce callback failed:", e, flush=True)
-            return 1
-    return ALLREDUCE_FN(_fn)
-
-
-def local_ba_sharded(ctx: Context, shard: dict, allreduce_cb, rank: int, **opts):
-    """ov2_localba_solve_sharded on this rank's shard; poses come back identical on every rank,
-    inverse depths / flags are the shard's own."""
-    o = dict(DEFAULT_BA_OPTS)
-    o.update(opts)
-    bo = BaOpts(**o)
-    keep = {k: np.ascontiguousarray(shard[k]) for k in
-            ("K", "pose", "pose_const", "lm_anchor_cam", "lm_anchor_px", "lm_invdepth", "obs_cam", "obs_lm", "obs_px")}
-    p = BaProblem(len(keep["pose"]), len(keep["lm_invdepth"]), len(keep["obs_cam"]),
-                  *[keep[k].ctypes.data for k in ("K", "pose", "pose_const", "lm_anchor_cam", "lm_anchor_px", "lm_invdepth",
-                                                  "obs_cam", "obs_lm", "obs_px")], *_stereo_ptrs(shard, keep))
-    res = BaResult()
-    flags = np.zeros(max(len(keep["obs_cam"]), 1), np.uint8)
-    ctx.check(ctx.lib.ov2_localba_solve_sharded(ctx.h, C.byref(p), C.byref(bo), C.byref(res), flags.ctypes.data,
-                                                allreduce_cb, None, int(rank)))
-    shard["pose"][...] = keep["pose"]
-    shard["lm_invdepth"][...] = keep["lm_invdepth"]
-    return {f: getattr(res, f) for f, _ in BaResult._fields_}, flags[:len(keep["obs_cam"])]
-
-
 class ShardedOptimizer:
-    """Multi-GPU Optimizer::localBA (BASELINE.json configs[4]): this rank's landmark shard, poses replicated.
-    mode "p2p" (default): the per-iteration sum of the reduced camera system happens inside the solve kernel over peer
-    memory (ov2_localba_solve_p2p); mode "callback": round-1 path, ncclAllReduce through torch.distributed per iteration."""
+    """Multi-GPU Optimizer::localBA (BASELINE.json configs[4]): this rank's landmark shard, poses replicated; the
+    per-iteration sum of the reduced camera system happens inside the solve kernel over peer memory
+    (ov2_localba_solve_p2p)."""
 
-    def __init__(self, ctx: Context, dist, torch, rank: int, world: int, group=None, mode: str = "p2p"):
-        self.ctx, self.rank, self.world, self.mode = ctx, rank, world, mode
-        if mode == "p2p":
-            self.comm = BaComm(ctx, rank, world)
-            self.comm.connect_torch(dist, torch, group)
-        else:
-            self._cb = make_torch_allreduce(dist, torch, group)
+    def __init__(self, ctx: Context, dist, torch, rank: int, world: int, group=None):
+        self.ctx, self.rank, self.world = ctx, rank, world
+        self.comm = BaComm(ctx, rank, world)
+        self.comm.connect_torch(dist, torch, group)
 
     def local_ba(self, shard: dict, **opts):
-        if self.mode == "p2p":
-            return self.comm.local_ba(shard, **opts)
-        return local_ba_sharded(self.ctx, shard, self._cb, self.rank, **opts)
+        return self.comm.local_ba(shard, **opts)
 
     def describe(self) -> str:
-        return ("in-kernel sum of the partial reduced systems over NVLink peer memory (CUDA IPC), one persistent kernel per solve"
-                if self.mode == "p2p" else "ncclAllReduce through the ov2_allreduce_fn callback (torch.distributed), host LM controller")
+        return "in-kernel sum of the partial reduced systems over NVLink peer memory (CUDA IPC), one persistent kernel per solve"

@@ -31,7 +31,6 @@ SOURCES = {
     "frontend_sad.cu": ["-fmad=false"],
     "frontend_remap.cu": [],
     "frontend_step.cu": [],
-    "ba_solver.cu": [],
     "ba_lm.cu": [],
     "ba_comm.cu": [],
     "pnp_solver.cu": [],

@@ -8,13 +8,9 @@
 // iteration and every rank solves the identical system (identical decisions, no broadcast).
 #include "ba_lm.cuh"
 
-#include <stdlib.h>
 #include <string.h>
 
 using namespace balm;
-
-ov2_status ov2_localba_solve_legacy(ov2_ctx* ctx, const ov2_ba_problem* pb, const ov2_ba_opts* opts, ov2_ba_result* res,
-                                    uint8_t* outlier_out);
 
 struct ov2_ba_comm {
     ov2_ctx* ctx = nullptr;
@@ -55,8 +51,6 @@ static const int* stop_flag_dev(ov2_ctx* ctx) {
 extern "C" ov2_status ov2_localba_solve(ov2_ctx* ctx, const ov2_ba_problem* pb, const ov2_ba_opts* opts,
                                         ov2_ba_result* res, uint8_t* outlier_out) {
     if (!ctx || !pb || !opts || !res) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_localba_solve: bad arguments");
-    const char* e = getenv("OV2_BA_LEGACY");
-    if ((e && atoi(e) != 0) || pb->ncam > MAX_CAMS) return ov2_localba_solve_legacy(ctx, pb, opts, res, outlier_out);
     memset(res, 0, sizeof(*res));
     if (pb->nobs == 0) return OV2_OK;
     uint8_t* outs[1] = {outlier_out};

@@ -8,15 +8,15 @@
 // (src/ceres_parametrization.cpp:361-712) with SE3LeftParameterization (se3left_parametrization.hpp:41-60).
 //
 // Design: a solve is launch/sync-latency bound (C3: 0.66 MB per LM iteration, all of it L2 resident), so
-// the whole two-stage solve - both Ceres solves, both outlier scans, every LM iteration - is ONE cooperative
+// the whole two-stage solve - both Ceres solves, both outlier scans, every LM iteration - is ONE kernel
 // launch.  A "group" of G CTAs works on one window; the phases of an LM iteration are separated by a group
 // barrier (monotonic counter in global memory, release/acquire), not by kernel boundaries:
 //
-//   A  residual blocks + analytic Jacobians at x (thread per observation, keyframe rotations staged in shared
-//      memory), cost                                                       [only when x changed]
+//   A  residual blocks + analytic Jacobians at x (thread per observation, keyframe rotations staged in the CTA's
+//      keyframe table), cost                                                       [only when x changed]
 //   B  Schur elimination, one warp per landmark, fp64 RED into the reduced camera system
-//   B2 fold of the privatised accumulation copies (multi-GPU: the partial systems of all ranks are summed here
-//      straight out of peer memory over NVLink - no NCCL call, no host round trip)
+//   B2 multi-GPU only: the partial systems of all ranks are summed straight out of peer memory over NVLink (no NCCL
+//      call, no host round trip)
 //   C  reduced camera system: LM damping + solve (n <= 96: Gauss-Jordan in CTA 0's shared memory; larger: blocked
 //      Cholesky, sequential part on CTA 0, FP64 tensor-core trailing update spread over the group), gradient
 //      projection by the last CTA
@@ -177,7 +177,7 @@ struct GroupBar {
 };
 
 // ------------------------------------------------------------------ keyframe staging
-// Rwc (9) + twc (3) of every keyframe of the window in shared memory: one normalisation + quaternion-to-rotation
+// Rwc (9) + twc (3) of every keyframe of the window in the CTA's keyframe table: one normalisation + quaternion-to-rotation
 // per keyframe and CTA instead of two per residual block.
 __device__ __forceinline__ void stage_cams(const Prob& P, const double* __restrict__ pose, double* s_cam) {
     for (int c = threadIdx.x; c < P.ncam; c += blockDim.x) {
@@ -292,28 +292,14 @@ __device__ __forceinline__ void red_add_f64(double* p, double v) {
 // over the landmark's observations in registers and leave the warp once.
 constexpr int SCH = 8;   // observations staged per chunk (C3: 4 per landmark, C5: 7.5)
 
-// CTA-local lock for the shared-memory accumulation mode: lane 0 spins on a shared-memory CAS, the warp follows.
-__device__ __forceinline__ void warp_lock(int* lock, int lane) {
-    if (!lock) return;                       // per-warp private block: nothing to serialise
-    if (lane == 0)
-        while (atomicCAS(lock, 0, 1) != 0) __nanosleep(20);
-    __syncwarp();
-    __threadfence_block();
-}
-__device__ __forceinline__ void warp_unlock(int* lock, int lane) {
-    if (!lock) return;
-    __threadfence_block();
-    __syncwarp();
-    if (lane == 0) atomicExch(lock, 0);
-}
-
-// SM = false: contributions leave the warp as fp64 RED into the (privatised) global accumulation block.  The phase is
-// bound by the rate at which an SM retires fp64 REDs (it scales with 1/SMs, not with warps per SM), ~900 REDs per landmark.  SM = true (reduced systems that fit shared memory, n <= ~100): the CTA keeps ONE
-// copy of [rhs | F'r | column norms | S] in shared memory, warps commit under a CTA-local lock with plain
-// read-modify-writes (shared-memory fp64 atomics are CAS loops, slower than RED) and the CTA flushes the non-zeros once.
+// SM = false: contributions leave the warp as fp64 RED into the global accumulation block.  The phase is bound by the
+// rate at which an SM retires fp64 REDs (it scales with 1/SMs, not with warps per SM), ~900 REDs per landmark.  SM = true
+// (reduced systems that fit shared memory): `acc` is the warp's own copy of [rhs | F'r | column norms | S] in shared
+// memory, updated with plain read-modify-writes (shared-memory fp64 atomics are CAS loops, slower than RED); the CTA sums
+// its warps' copies and flushes the non-zeros once.
 template <bool SM>
 __device__ __forceinline__ void schur_landmark(const Prob& P, const int* __restrict__ s_slot, double* s_etf, int* s_eslot, double* sJ, int* smeta,
-                                               int l, int lane, double radius, int first_iter, double* acc, int n, double& gmax_lm, int* lock) {
+                                               int l, int lane, double radius, int first_iter, double* acc, int n, double& gmax_lm) {
 #define ACC(ptr, v) do { if (SM) *(ptr) += (v); else red_add_f64((ptr), (v)); } while (0)
     const int p0 = P.lm_ptr[l], p1 = P.lm_ptr[l + 1];
     double* const cRhs = acc; double* const cG = acc + n; double* const cCn = acc + 2 * n; double* const cS = acc + 3 * n;
@@ -376,7 +362,6 @@ __device__ __forceinline__ void schur_landmark(const Prob& P, const int* __restr
             smeta[lane] = !act ? -3 : (ty == 2 ? -2 : s_slot[cam]);   // -3: inactive, -2: e-block-only row (schur_eliminator_impl.h:196-217)
         }
         __syncwarp();
-        if (SM) warp_lock(lock, lane);
     for (int q = 0; q < cnt; ++q) {
         const int so = smeta[q];
         if (so < -1) continue;
@@ -436,9 +421,7 @@ __device__ __forceinline__ void schur_landmark(const Prob& P, const int* __restr
         }
         __syncwarp();
     }
-        if (SM) warp_unlock(lock, lane);
     }
-    if (SM) warp_lock(lock, lane);
     if (sa >= 0) {
         if (e0a <= e0b) ACC(cS + (size_t)(6 * sa + e0a) * n + 6 * sa + e0b, aFF0);
         if (e1 < 36 && e1a <= e1b) ACC(cS + (size_t)(6 * sa + e1a) * n + 6 * sa + e1b, aFF1);
@@ -491,7 +474,6 @@ __device__ __forceinline__ void schur_landmark(const Prob& P, const int* __restr
         const int i = e / 6, a = e - 6 * i;
         ACC(cRhs + 6 * s_eslot[i] + a, -s_etf[6 * i + a] * ge * inv_ete);
     }
-    if (SM) warp_unlock(lock, lane);
     __syncwarp();
 #undef ACC
 }
@@ -802,78 +784,6 @@ __device__ __forceinline__ void gj_pivots(double* sA, int n, int PIT, int* s_fai
     }
 }
 
-// Two pivots per barrier (n <= 48).  The 48-pivot loop above is a latency chain: barrier -> pivot read -> reciprocal ->
-// row factor -> update -> store, ~0.5 us per pivot, 24 us of a 75 us LM iteration of a single C3 window.  Eliminating
-// columns j and j+1 in one step halves the barriers and overlaps the second reciprocal with the first update's loads:
-//   a = A[j][j], b = A[j][j+1], c = A[j+1][j], d = A[j+1][j+1];   m = c / a;   d' = d - m b   (the SAME second pivot the
-//   scalar loop meets);   row j+1 := row j+1 - m row j;   row j := row j - (b / d') row j+1;   every other row r:
-//   f0 = A[r][j] / a,  f1 = (A[r][j+1] - f0 b) / d',  row r -= f0 row j(old) + f1 row j+1(new).
-// Rows j and j+1 are rewritten in their own step, so the step's readers take them from a double-buffered copy (pbuf) that
-// the rows' owners filled at the end of the previous step.
-template <int QMAX>
-__device__ __forceinline__ void gj_pivots2(double* sA, int n, int PIT, double* pbuf, int* s_fail) {
-    const int tid = threadIdx.x, nt = blockDim.x;
-    const int sub = tid & 3, r0 = tid >> 2, rows_per_pass = nt >> 2;
-    for (int e = tid; e < 2 * PIT; e += nt) pbuf[e] = sA[e];        // rows 0 and 1 -> parity 0
-    __syncthreads();
-    for (int j = 0; j < n; j += 2) {
-        const int par = (j >> 1) & 1;
-        const double* P0 = pbuf + (size_t)(2 * par) * PIT;
-        const double* P1 = P0 + PIT;
-        double* N0 = pbuf + (size_t)(2 * (par ^ 1)) * PIT;
-        double* N1 = N0 + PIT;
-        const double a = P0[j], b = P0[j + 1], c = P1[j], d = P1[j + 1];
-        if (!(a > 0.0) || !isfinite(a)) { if (tid == 0) *s_fail = 1; break; }   // uniform: every thread reads the same pivots
-        double ip0;
-        asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(ip0) : "d"(a));
-        ip0 = fma(ip0, fma(-a, ip0, 1.0), ip0);
-        ip0 = fma(ip0, fma(-a, ip0, 1.0), ip0);
-        const double m = c * ip0;
-        const double d2 = d - m * b;
-        if (!(d2 > 0.0) || !isfinite(d2)) { if (tid == 0) *s_fail = 1; break; }
-        double ip1;
-        asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(ip1) : "d"(d2));
-        ip1 = fma(ip1, fma(-d2, ip1, 1.0), ip1);
-        ip1 = fma(ip1, fma(-d2, ip1, 1.0), ip1);
-        const double g = b * ip1;
-        const int c0 = j + 2 + sub;
-        const int nq = (n - j + 2 - sub) >> 2;              // columns c = c0 + 4 q <= n
-        double p0[QMAX], p1[QMAX];
-#pragma unroll
-        for (int q = 0; q < QMAX; ++q) {
-            p0[q] = q < nq ? P0[c0 + 4 * q] : 0.0;
-            p1[q] = q < nq ? P1[c0 + 4 * q] - m * p0[q] : 0.0;
-        }
-        for (int r = r0; r < n; r += rows_per_pass) {
-            double* rowr = sA + r * PIT;
-            double v[QMAX];
-            if (r == j) {
-#pragma unroll
-                for (int q = 0; q < QMAX; ++q) v[q] = p0[q] - g * p1[q];
-            } else if (r == j + 1) {
-#pragma unroll
-                for (int q = 0; q < QMAX; ++q) v[q] = p1[q];
-                if (sub == 0) rowr[j + 1] = d2;              // the diagonal holds the second pivot (z = A[i][n] / A[i][i])
-            } else {
-                const double f0 = rowr[j] * ip0;
-                const double f1 = (rowr[j + 1] - f0 * b) * ip1;
-#pragma unroll
-                for (int q = 0; q < QMAX; ++q) v[q] = q < nq ? rowr[c0 + 4 * q] : 0.0;
-#pragma unroll
-                for (int q = 0; q < QMAX; ++q) v[q] -= f0 * p0[q] + f1 * p1[q];
-            }
-            double* nxt = r == j + 2 ? N0 : (r == j + 3 ? N1 : nullptr);
-#pragma unroll
-            for (int q = 0; q < QMAX; ++q)
-                if (q < nq) {
-                    rowr[c0 + 4 * q] = v[q];
-                    if (nxt) nxt[c0 + 4 * q] = v[q];
-                }
-        }
-        __syncthreads();
-    }
-}
-
 __device__ void reduced_solve_small(const Prob& P, double* T, int n, double radius, int first_iter, double* sA, double* scal) {
     const int tid = threadIdx.x, nt = blockDim.x;
     const int PIT = n + 2;
@@ -901,8 +811,7 @@ __device__ void reduced_solve_small(const Prob& P, double* T, int n, double radi
     }
     __syncthreads();
     TRS(12);
-    if (n <= 48 && P.gj2) gj_pivots2<13>(sA, n, PIT, sA + (size_t)n * PIT, &s_fail);   // two pivots per barrier
-    else if (n <= 48) gj_pivots<13>(sA, n, PIT, &s_fail);    // (n + 1 + 3) / 4 columns per thread
+    if (n <= 48) gj_pivots<13>(sA, n, PIT, &s_fail);         // (n + 1 + 3) / 4 columns per thread
     else if (n <= 64) gj_pivots<17>(sA, n, PIT, &s_fail);
     else gj_pivots<25>(sA, n, PIT, &s_fail);
     __syncthreads();
@@ -1260,7 +1169,7 @@ struct SolveOut { int iterations; double initial_cost, final_cost; int terminati
 __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restrict__ probs, int nprob, int G, Peers X) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ lmctl::State S;
-    __shared__ int s_action, s_ncv, s_any, s_refine, s_trivial, s_lock;
+    __shared__ int s_action, s_ncv, s_any, s_refine, s_trivial;
     __shared__ double s_red[WARPS][4];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int group = blockIdx.x / G, bid = blockIdx.x - group * G, ngroups = gridDim.x / G;
@@ -1279,9 +1188,10 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
         const bool tracing = P.trace != nullptr && bid == 0 && tid == 0;
         if (tracing) tr_last = global_ns();
 #define TR(k) do { if (tracing) { const unsigned long long t_ = global_ns(); tr_acc[k] += t_ - tr_last; tr_last = t_; } } while (0)
-        // shared memory carve-up
-        double* s_cam = reinterpret_cast<double*>(smem_raw);                       // [ncam][12]
-        int* s_slot = reinterpret_cast<int*>(s_cam + 12 * (size_t)P.ncam);         // [ncam]
+        // keyframe table [ncam][12] + [ncam] slots: in shared memory, or (windows too large for it) this CTA's copy in
+        // global memory; either way only this CTA reads and writes it
+        double* s_cam = P.cam_tab ? P.cam_tab + (size_t)bid * P.cam_tab_stride : reinterpret_cast<double*>(smem_raw);
+        int* s_slot = reinterpret_cast<int*>(s_cam + 12 * (size_t)P.ncam);
         double* s_work = reinterpret_cast<double*>(smem_raw + P.smem_work_off);    // Schur scratch / solve area (union)
         const int etf_stride = 6 * (P.ncv_max + 1);
         double* s_etf = s_work + (size_t)warp * etf_stride;
@@ -1319,7 +1229,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                 if (s_slot[c]) cam_used[c] = 1;
             for (int i = gtid; i < 7 * P.ncam; i += gthreads) c_pose[i] = x_pose[i];
             for (int i = gtid; i < P.npts; i += gthreads) c_invd[i] = x_invd[i];
-            for (size_t i = gtid; i < (size_t)P.ncopy * blk; i += gthreads) P.acc[i] = 0.0;
+            for (size_t i = gtid; i < blk; i += gthreads) P.acc[i] = 0.0;
             for (int i = gtid; i < 2 * SC_COUNT; i += gthreads) P.scal[i] = 0.0;
             TR(stage == 0 ? 0 : 10);
             bar.sync();
@@ -1356,7 +1266,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
             if (!s_any) { if (stage == 0) break; else continue; }   // no residual blocks (on any rank)
             if (bid == 0)
                 for (int c = tid; c < P.ncam; c += THREADS) P.cam_slot[c] = s_slot[c];
-            double* T = (P.ncopy > 1 || X.world > 1) ? P.total : P.acc;      // the system the solve reads
+            double* T = X.world > 1 ? P.total : P.acc;                       // the system the solve reads
             TR(0);
             // ---- LM iterations
             for (;;) {
@@ -1384,7 +1294,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                 }
                 bar.sync();
                 TR(1);
-                // ---- B: Schur elimination into this CTA's accumulation copy (global, RED) or shared-memory block (lock)
+                // ---- B: Schur elimination into the accumulation block
                 if (P.schur_smem == 3) {
                     // owner mode (n <= 96): pair-sorted Gram blocks + dense landmark rows, no per-observation reductions
 #define OV2_OWNER(NT_) do { if (P.sg == 4) schur_owner_phase<NT_, 4>(P, s_slot, s_work, n, radius, first_iter, bid, G, scal); \
@@ -1402,7 +1312,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     for (int e = lane; e < live_s; e += 32) mine[e] = 0.0;
                     __syncwarp();
                     double gmax_lm = 0.0;
-                    for (int l = gwarp; l < P.npts; l += gwarps) schur_landmark<true>(P, s_slot, s_etf, s_eslot, sJ, smeta, l, lane, radius, first_iter, mine, n, gmax_lm, nullptr);
+                    for (int l = gwarp; l < P.npts; l += gwarps) schur_landmark<true>(P, s_slot, s_etf, s_eslot, sJ, smeta, l, lane, radius, first_iter, mine, n, gmax_lm);
                     if (lane == 0 && gmax_lm > 0.0) atomic_max_pos(scal + SC_GMAX_LM, gmax_lm);
                     __syncthreads();
                     const double* all = s_work + P.smem_sacc_off;
@@ -1412,37 +1322,18 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                         for (int w_ = 0; w_ < WARPS; ++w_) v += all[(size_t)w_ * live_s + e];
                         if (v != 0.0) red_add_f64(P.acc + e, v);
                     }
-                } else if (P.schur_smem) {
-                    double* sS = s_work + P.smem_sacc_off;
-                    const int live_s = 3 * n + n * n;
-                    for (int e = tid; e < live_s; e += THREADS) sS[e] = 0.0;
-                    if (tid == 0) s_lock = 0;
-                    __syncthreads();
-                    double gmax_lm = 0.0;
-                    for (int l = gwarp; l < P.npts; l += gwarps) schur_landmark<true>(P, s_slot, s_etf, s_eslot, sJ, smeta, l, lane, radius, first_iter, sS, n, gmax_lm, &s_lock);
-                    if (lane == 0 && gmax_lm > 0.0) atomic_max_pos(scal + SC_GMAX_LM, gmax_lm);
-                    __syncthreads();
-                    for (int e = tid; e < live_s; e += THREADS) {
-                        const double v = sS[e];
-                        if (v != 0.0) red_add_f64(P.acc + e, v);
-                    }
                 } else {
-                    double* acc = P.acc + (size_t)(bid % P.ncopy) * blk;
                     double gmax_lm = 0.0;
-                    for (int l = gwarp; l < P.npts; l += gwarps) schur_landmark<false>(P, s_slot, s_etf, s_eslot, sJ, smeta, l, lane, radius, first_iter, acc, n, gmax_lm, nullptr);
+                    for (int l = gwarp; l < P.npts; l += gwarps) schur_landmark<false>(P, s_slot, s_etf, s_eslot, sJ, smeta, l, lane, radius, first_iter, P.acc, n, gmax_lm);
                     if (lane == 0 && gmax_lm > 0.0) atomic_max_pos(scal + SC_GMAX_LM, gmax_lm);
                 }
                 bar.sync();
                 TR(2);
-                // ---- B2: fold the copies; multi-GPU: sum the ranks' partial systems out of peer memory
+                // ---- B2: multi-GPU: sum the ranks' partial systems out of peer memory
                 const int live = 3 * n + n * n;
                 if (X.world > 1) {
                     double* mine = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(X.base[X.rank]) + XB_PARTIAL) + (size_t)par * (SC_COUNT + blk);
-                    for (int e = gtid; e < live; e += gthreads) {
-                        double a = P.acc[e];
-                        for (int k = 1; k < P.ncopy; ++k) a += P.acc[e + (size_t)k * blk];
-                        mine[SC_COUNT + e] = a;
-                    }
+                    for (int e = gtid; e < live; e += gthreads) mine[SC_COUNT + e] = P.acc[e];
                     if (gtid < SC_COUNT) mine[gtid] = scal[gtid];
                     bar.sync();
                     if (bid == 0 && tid == 0) xsync(X, xepoch, P.bar + 1);
@@ -1464,17 +1355,10 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                         scal[SC_GMAX_LM] = g;
                     }
                     bar.sync();
-                } else if (P.ncopy > 1) {
-                    for (int e = gtid; e < live; e += gthreads) {
-                        double a = P.acc[e];
-                        for (int k = 1; k < P.ncopy; ++k) a += P.acc[e + (size_t)k * blk];
-                        T[e] = a;
-                    }
-                    bar.sync();
                 }
                 TR(3);
                 // ---- C: reduced camera system (CTA 0); gradient projection |x - Plus(x, -g)|_inf (last CTA); the other
-                //      CTAs clear the accumulation copies for the next iteration (T is separate whenever ncopy > 1)
+                //      CTAs clear the accumulation block for the next iteration once the solve has read it
                 const bool group_solve = P.solve_blocked && n > 0;
                 if (bid == 0 && !group_solve && n > 0) reduced_solve_small(P, T, n, radius, first_iter, s_work, scal);
                 if (bid == G - 1 && x_is_new && n > 0) {
@@ -1542,8 +1426,8 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                         for (int w_ = 0; w_ < WARPS; ++w_) a += s_red[w_][tid];
                         if (a != 0.0) red_add_f64(scal + SC_CAND_COST + tid, a);
                     }
-                    // clear for the next iteration: accumulation copies and the other parity's scalars
-                    for (size_t i = gtid; i < (size_t)P.ncopy * blk; i += gthreads) P.acc[i] = 0.0;
+                    // clear for the next iteration: accumulation block and the other parity's scalars
+                    for (size_t i = gtid; i < blk; i += gthreads) P.acc[i] = 0.0;
                     double* oscal = P.scal + (par ^ 1) * SC_COUNT;
                     if (gtid < SC_COUNT) oscal[gtid] = 0.0;
                 }
@@ -1693,10 +1577,11 @@ struct HostPlan {
     size_t off_pp, off_pch; int pch_cap, sg;   // owner mode: pair-sorted permutation, chunk table (capacity), lanes per landmark
     // device-only work areas (offsets into the work block)
     size_t w_pose1, w_invd1, w_active, w_flags, w_camused, w_camslot, w_Jr, w_Ja, w_Jo, w_Jl, w_chi2, w_dpos, w_sclm, w_ete, w_ge,
-           w_acc, w_total, w_scal, w_z, w_panel, w_sccam, w_counts, w_bar, w_result, w_trace, work_bytes, zero_off, zero_bytes;
+           w_acc, w_total, w_scal, w_z, w_panel, w_sccam, w_counts, w_bar, w_result, w_trace, w_camtab, work_bytes, zero_off, zero_bytes;
     size_t out_result, out_flags, act_rel;   // offsets inside the batch's output region / 'active' region (set up by balm_solve)
-    int ncv_max, n_max, ncopy, solve_blocked, schur_smem;
-    size_t blk, smem_work_off, smem_bytes, smem_sacc_off;
+    int ncv_max, n_max, solve_blocked, schur_smem;
+    bool cam_tab_global;                     // keyframe table in the work block (one copy per CTA), not in shared memory
+    size_t blk, tab_bytes, smem_work_off, smem_bytes, smem_sacc_off;
 };
 
 size_t take(size_t& off, size_t bytes, size_t align = 256) {
@@ -1710,21 +1595,15 @@ size_t take(size_t& off, size_t bytes, size_t align = 256) {
 
 // Plans one window: offsets of its inputs inside the upload block and of its work areas inside the work block.
 static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world, size_t& st_off, size_t& in_off, size_t& work_off,
-                              size_t& zero_off, size_t& out_off, size_t& act_off, HostPlan& H, int ncopy_cap, bool single_window) {
+                              size_t& zero_off, size_t& out_off, size_t& act_off, HostPlan& H, bool single_window) {
     const int ncam = pb->ncam, npts = pb->npts, nobs = pb->nobs;
     int ncv = 0;
     for (int c = 0; c < ncam; ++c) ncv += pb->pose_const[c] ? 0 : 1;
     if (ncv > MAX_VAR_CAMS) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: more than 64 optimised keyframes");
-    if (ncam > MAX_CAMS) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: more than 256 keyframes in the window");
+    if (world > 1 && ncam > MAX_CAMS) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve_p2p: more than 256 keyframes in a multi-GPU window");
     H.ncv_max = ncv; H.n_max = 6 * ncv;
     H.blk = 3 * (size_t)H.n_max + (size_t)H.n_max * H.n_max;
     if (H.blk == 0) H.blk = 1;
-    // ONE accumulation block: privatised copies (round 1 used up to 8) do not pay - the phase is bound by the
-    // rate at which an SM retires fp64 REDs, not by same-address contention
-    // - and a single copy needs no fold phase.  OV2_BA_NCOPY = 2..8 brings the copies back for experiments.
-    (void)ncopy_cap;
-    H.ncopy = 1;
-    if (getenv("OV2_BA_NCOPY")) { int e = atoi(getenv("OV2_BA_NCOPY")); if (e >= 1 && e <= 8 && (size_t)e * H.blk <= (size_t)(3 * MAX_N + MAX_N * MAX_N)) H.ncopy = e; }
     H.solve_blocked = H.n_max > 96 ? 1 : 0;
     // states (pose, inverse depth) of all windows sit together at the head of the block: they are what comes back
     H.off_pose = take(st_off, sizeof(double) * 7 * ncam, 16);
@@ -1773,54 +1652,52 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     H.w_dpos = take(work_off, no);
     H.w_ete = take(work_off, sizeof(double) * np);
     H.w_ge = take(work_off, sizeof(double) * np);
-    H.w_acc = take(work_off, sizeof(double) * (size_t)H.ncopy * H.blk);
+    H.w_acc = take(work_off, sizeof(double) * H.blk);
     H.w_total = take(work_off, sizeof(double) * H.blk);
     H.w_scal = take(work_off, sizeof(double) * 2 * SC_COUNT);
     H.w_z = take(work_off, sizeof(double) * MAX_N);
     H.w_panel = take(work_off, sizeof(double) * CH_NB * (size_t)(MAX_N + 24));
-    // dynamic shared memory: [keyframes 12 doubles each][slots][union: Schur scratch | solve area]
+    // dynamic shared memory: [keyframe table: 12 doubles + 1 slot each][union: Schur scratch | solve area]
     size_t s = sizeof(double) * 12 * (size_t)ncam + sizeof(int) * (size_t)ncam;
     s = (s + 15) & ~(size_t)15;
+    H.tab_bytes = s;
     H.smem_work_off = s;
     size_t schur = (size_t)WARPS * 6 * (size_t)(ncv + 1) * sizeof(double) + ((((size_t)WARPS * (ncv + 1) + 1) >> 1) << 3) +
                    (size_t)WARPS * 28 * SCH * sizeof(double) + (size_t)WARPS * SCH * sizeof(int) + 16;
     schur = (schur + 15) & ~(size_t)15;
     const size_t solve = H.solve_blocked ? (size_t)CH_NB * (size_t)((((size_t)H.n_max + 15) & ~(size_t)15) + 8) * sizeof(double)
-                                         : (size_t)(H.n_max + 4) * (size_t)(H.n_max + 2) * sizeof(double);   // + 4 rows: pivot-row double buffer of gj_pivots2
+                                         : (size_t)H.n_max * (size_t)(H.n_max + 2) * sizeof(double);
     // shared-memory accumulation of the reduced system (behind the Schur scratch) when the whole block fits next to it
     // with two CTAs per SM still possible
     H.smem_sacc_off = schur / sizeof(double);
     H.schur_smem = 0;
-    // (opt-in, OV2_BA_SCHUR_SMEM=1: slower than the RED path - the lock serialises the eight warps of a CTA for the whole
-    //  commit.  Kept because it is tested and documents the negative result.)
     const char* ssm = getenv("OV2_BA_SCHUR_SMEM");
-    if (H.n_max > 0 && s + schur + H.blk * sizeof(double) <= 100 * 1024 && ssm && atoi(ssm) == 1) {
-        H.schur_smem = 1;
-        H.ncopy = 1;
-        schur += H.blk * sizeof(double);
-    } else if (H.n_max > 0 && s + schur + (size_t)WARPS * H.blk * sizeof(double) <= 190 * 1024 && !(ssm && atoi(ssm) == 0) &&
+    if (H.n_max > 0 && s + schur + (size_t)WARPS * H.blk * sizeof(double) <= 190 * 1024 && !(ssm && atoi(ssm) == 0) &&
                (single_window || (ssm && atoi(ssm) == 2))) {
         // mode 2 (default for a single window when it fits: reduced systems up to n = 54): one private block per warp, one
         // CTA per SM.  Batches keep the RED path: there two CTAs per SM (different windows overlapping their latency-bound
         // phases) are worth more than the faster accumulation - measured 5.1 k vs 4.1 k solves/s on the C3 batch.
         H.schur_smem = 2;
-        H.ncopy = 1;
         schur += (size_t)WARPS * H.blk * sizeof(double);
     }
     // mode 3 (default up to n = 96, single windows and batches): owner mode, see schur_owner_phase
     // Single windows spread over many CTAs stay on mode 2 when it fits (measured C3: 119 us vs 236 us per solve in the
     // Schur phase at 148 CTAs - there the phase is latency, not RED bound); batches (1-2 CTAs per window) take mode 3.
-    if (H.n_max > 0 && H.n_max <= 96 && ((ssm && atoi(ssm) == 3) || (!ssm && !(single_window && H.schur_smem == 2)))) {
+    // Its host-side pair sort counts over all ncam^2 keyframe pairs, so it is limited to windows of <= MAX_CAMS keyframes.
+    if (H.n_max > 0 && H.n_max <= 96 && ncam <= MAX_CAMS && ((ssm && atoi(ssm) == 3) || (!ssm && !(single_window && H.schur_smem == 2)))) {
         const size_t R = (size_t)WARPS * (32 / H.sg);
         size_t tile = (R * (size_t)owner_tile_pitch(H.n_max) + 2 * R) * sizeof(double);
         const size_t stage = (size_t)WARPS * PCH * 26 * sizeof(double);
         if (tile < stage) tile = stage;
         H.schur_smem = 3;
-        H.ncopy = 1;
         schur = (tile + 15) & ~(size_t)15;
     }
-    H.smem_bytes = s + (schur > solve ? schur : solve) + 16;
-    (void)world;
+    // a keyframe table that does not fit next to the work area moves to the work block (balm_solve sizes it, one copy
+    // per CTA of the group: every CTA writes its own candidate poses into it); the kernel code is the same either way
+    const size_t work = (schur > solve ? schur : solve) + 16;
+    H.cam_tab_global = s + work > SMEM_BUDGET;
+    if (H.cam_tab_global) H.smem_work_off = 0;
+    H.smem_bytes = H.cam_tab_global ? work : s + work;
     return OV2_OK;
 }
 
@@ -1869,12 +1746,10 @@ static void fill_prob(const ov2_ba_problem* pb, const ov2_ba_opts* opts, const H
     P.z = (double*)(dwork + H.w_z); P.sc_cam = (double*)(dwork + H.w_sccam); P.panel = (double*)(dwork + H.w_panel);
     P.counts = (double*)(dwork + H.w_counts); P.bar = (unsigned*)(dwork + H.w_bar); P.result = (Result*)(dwork + H.w_result);
     P.trace = getenv("OV2_BA_TRACE") ? (unsigned long long*)(dwork + H.w_trace) : nullptr;
-    P.ncv_max = H.ncv_max; P.ncopy = H.ncopy; P.blk = H.blk; P.solve_blocked = H.solve_blocked;
+    P.ncv_max = H.ncv_max; P.blk = H.blk; P.solve_blocked = H.solve_blocked;
     P.sg = H.sg;   // lanes per landmark in the per-landmark phases
-    // two-pivot Gauss-Jordan steps for n <= 48: opt-in (OV2_BA_GJ2=1).  Slower than one pivot per barrier: the longer
-    // dependent chain of a step (two reciprocals + the second pivot's elimination) and 26 more live registers cost more
-    // than the 24 saved barriers.  Kept: tested, documents the result.
-    P.gj2 = getenv("OV2_BA_GJ2") ? atoi(getenv("OV2_BA_GJ2")) : 0;
+    P.cam_tab = H.cam_tab_global ? (double*)(dwork + H.w_camtab) : nullptr;
+    P.cam_tab_stride = H.tab_bytes / sizeof(double);
     P.schur_smem = H.schur_smem; P.smem_sacc_off = (int)H.smem_sacc_off;
     P.pair_perm = (const int32_t*)(din + H.off_pp); P.pair_chunk = (const int2*)(din + H.off_pch); P.npchunk = 0;
     P.smem_work_off = (int)H.smem_work_off;
@@ -1933,14 +1808,45 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         hp[k].Trl = (const double*)pull(pb.Trl, 56);
         if (pull_err != cudaSuccess) return ov2_fail(ctx, OV2_ERR_CUDA, "ov2_localba_solve: staging a device-resident window", pull_err);
         if (pb.obs_type && (!pb.Kr || !pb.Trl)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_localba_solve: obs_type given without Kr / Trl");
-        if ((st = plan_window(ctx, &hp[k], world, st_off, in_off, work_off, zero_off, out_off, act_off, plans[k], 8, nprob == 1)) != OV2_OK) return st;
+        if ((st = plan_window(ctx, &hp[k], world, st_off, in_off, work_off, zero_off, out_off, act_off, plans[k], nprob == 1)) != OV2_OK) return st;
         if (plans[k].smem_bytes > smem_max) smem_max = plans[k].smem_bytes;
         const int wk = (pb.nobs + THREADS - 1) / THREADS;
         const int wl = (pb.npts + WARPS - 1) / WARPS;                  // a landmark per warp and phase (single window: every SM helps)
         const int w = wk > wl ? wk : wl;
         if (w > gmax_work) gmax_work = w;
     }
-    if (smem_max > 200 * 1024) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: window needs more than 200 KB of shared memory");
+    if (smem_max > SMEM_BUDGET) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: window needs more than 200 KB of shared memory");
+    // ---- launch geometry: G CTAs per window, all groups co-resident
+    {
+        // raised only when a window needs more than any before (a function-attribute change while another stream runs the
+        // kernel may serialise with it)
+        // (check + set + record under one lock: two host threads with their own contexts may make their first solves concurrently)
+        static size_t attr_smem[16] = {0};
+        static std::mutex attr_mu;
+        std::lock_guard<std::mutex> attr_lock(attr_mu);
+        const int dv = ctx->device & 15;
+        if (smem_max > attr_smem[dv]) {
+            OV2_CUDA(ctx, cudaFuncSetAttribute(ba_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+            attr_smem[dv] = smem_max;
+        }
+    }
+    int per_sm = 0;
+    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_lm_kernel, THREADS, smem_max));
+    if (per_sm < 1) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: kernel does not fit an SM");
+    const int resident = per_sm * ctx->sm_count;
+    int G = gmax_work < 1 ? 1 : gmax_work;
+    // one wave of work per phase at most; more CTAs only add barrier latency
+    int gcap = nprob == 1 ? resident : (resident / nprob < 1 ? 1 : resident / nprob);
+    if (nprob > 1 && gcap > 16) gcap = 16;
+    if (G > gcap) G = gcap;
+    if (getenv("OV2_BA_CTAS")) { int e = atoi(getenv("OV2_BA_CTAS")); if (e >= 1 && e <= gcap) G = e; }
+    if (world > 1 && G < 2) G = 2;
+    int ngroups = nprob < resident / G ? nprob : resident / G;
+    if (ngroups < 1) ngroups = 1;
+    int grid = ngroups * G;
+    // keyframe tables that live in the work block: one per CTA of the window's group
+    for (int k = 0; k < nprob; ++k)
+        if (plans[k].cam_tab_global) plans[k].w_camtab = take(work_off, (size_t)G * plans[k].tab_bytes);
     // ---- pack the inputs into one pinned block: ONE H2D copy for the whole batch.  Layout: [states | everything else]
     const size_t st_bytes = (st_off + 255) & ~(size_t)255;
     for (int k = 0; k < nprob; ++k) {
@@ -2059,54 +1965,18 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     else OV2_CUDA(ctx, cudaMemcpyAsync(dprobs, parr.data(), sizeof(Prob) * (size_t)nprob, cudaMemcpyHostToDevice, s));   // parr outlives the sync below
     OV2_CUDA(ctx, cudaMemsetAsync(dwork + zbase, 0, zbytes + obytes, s));   // zero region + output region of every window
     OV2_CUDA(ctx, cudaMemsetAsync(dwork + abase, 1, abytes, s));            // every observation starts active
-    // ---- launch geometry: G CTAs per window, all groups co-resident (cooperative launch)
-    {
-        // raised only when a window needs more than any before (a function-attribute change while another stream runs the
-        // kernel may serialise with it)
-        // (check + set + record under one lock: two host threads with their own contexts may make their first solves concurrently)
-        static size_t attr_smem[16] = {0};
-        static std::mutex attr_mu;
-        std::lock_guard<std::mutex> attr_lock(attr_mu);
-        const int dv = ctx->device & 15;
-        if (smem_max > attr_smem[dv]) {
-            OV2_CUDA(ctx, cudaFuncSetAttribute(ba_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-            attr_smem[dv] = smem_max;
-        }
-    }
-    int per_sm = 0;
-    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_lm_kernel, THREADS, smem_max));
-    if (per_sm < 1) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: kernel does not fit an SM");
-    const int resident = per_sm * ctx->sm_count;
-    int G = gmax_work < 1 ? 1 : gmax_work;
-    // one wave of work per phase at most; more CTAs only add barrier latency
-    int gcap = nprob == 1 ? resident : (resident / nprob < 1 ? 1 : resident / nprob);
-    if (nprob > 1 && gcap > 16) gcap = 16;
-    if (G > gcap) G = gcap;
-    if (getenv("OV2_BA_CTAS")) { int e = atoi(getenv("OV2_BA_CTAS")); if (e >= 1 && e <= gcap) G = e; }
-    if (world > 1 && G < 2) G = 2;
-    int ngroups = nprob < resident / G ? nprob : resident / G;
-    if (ngroups < 1) ngroups = 1;
-    int grid = ngroups * G;
     Peers X;
     memset(&X, 0, sizeof(X));
     X.world = 1;
     if (peers) X = *peers;
     const Prob* dp = dprobs;
-    void* kargs[] = {(void*)&dp, (void*)&nprob, (void*)&G, (void*)&X};
     if (ctx->profiling) ov2_prof_begin(ctx);
-    // grid <= resident capacity, so on a GPU this process owns every CTA starts at once whichever launch API is used.  The
-    // plain launch is the default: cooperative launches were measured to start their CTAs one after the other (~4 us each)
-    // and are not run concurrently with another cooperative kernel (ranks sharing one GPU in the tests); OV2_BA_COOP=1
-    // selects cudaLaunchCooperativeKernel (co-residency guaranteed by the driver).  A CTA that never arrives trips the
-    // barrier timeout instead of hanging the device.
-    const char* coop = getenv("OV2_BA_COOP");
-    cudaError_t le;
-    if (coop && atoi(coop) != 0) {
-        le = cudaLaunchCooperativeKernel((const void*)ba_lm_kernel, dim3(grid), dim3(THREADS), kargs, smem_max, s);
-    } else {
-        ba_lm_kernel<<<grid, THREADS, smem_max, s>>>(dp, nprob, G, X);
-        le = cudaGetLastError();
-    }
+    // grid <= resident capacity, so on a GPU this process owns every CTA starts at once.  A plain launch: cooperative
+    // launches were measured to start their CTAs one after the other (~4 us each) and are not run concurrently with
+    // another cooperative kernel (ranks sharing one GPU in the tests).  A CTA that never arrives trips the barrier timeout
+    // instead of hanging the device.
+    ba_lm_kernel<<<grid, THREADS, smem_max, s>>>(dp, nprob, G, X);
+    const cudaError_t le = cudaGetLastError();
     ctx->launches++;
     if (le != cudaSuccess) return ov2_fail(ctx, OV2_ERR_CUDA, "ba_lm_kernel launch", le);
     if (ctx->profiling) ov2_prof_end(ctx, "ba_lm_kernel");
@@ -2131,7 +2001,8 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         cudaMemcpy(tr, dwork + plans[0].w_trace, sizeof(tr), cudaMemcpyDeviceToHost);
         static const char* names[16] = {"setup0", "A:eval", "B:schur", "B2:fold", "C:solve", "C:wait", "D:backsub", "E:ctl", "scan", "wb", "setup1", "bar0",
                                         "chol:P1", "chol:bar", "chol:P2", "chol:back|ownerB1"};
-        fprintf(stderr, "[ba trace] G=%d grid=%d smem=%zu ncopy=%d smemS=%d |", G, grid, smem_max, plans[0].ncopy, plans[0].schur_smem);
+        fprintf(stderr, "[ba trace] G=%d grid=%d smem=%zu smemS=%d camtab=%s |", G, grid, smem_max, plans[0].schur_smem,
+                plans[0].cam_tab_global ? "global" : "shared");
         for (int k = 0; k < 16; ++k) fprintf(stderr, " %s %.1fus", names[k], tr[k] / 1e3);
         fprintf(stderr, "\n");
     }

@@ -10,7 +10,8 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int THREADS = 256, WARPS = THREADS / 32;
 constexpr int MAX_VAR_CAMS = 64;            // optimised keyframes per window
 constexpr int MAX_N = 6 * MAX_VAR_CAMS;     // reduced camera system
-constexpr int MAX_CAMS = 256;               // keyframes per window (optimised + constant)
+constexpr int MAX_CAMS = 256;               // keyframes per multi-GPU window (XB_CAMUSED) and per owner-mode window
+constexpr size_t SMEM_BUDGET = 200 * 1024;  // dynamic shared memory of the solve kernel (H100: 227 KB per CTA, less static)
 constexpr int CH_NB = 32;                   // block size of the blocked Cholesky
 constexpr double SOPHUS_EPS = 1e-10;
 constexpr int MAX_RANKS = 8;
@@ -38,20 +39,21 @@ struct Prob {
     uint8_t* active; uint8_t* flags; uint8_t* cam_used; int32_t* cam_slot;
     double *Jr, *Ja, *Jo, *Jl, *chi2; uint8_t* dpos;
     double *sc_lm, *ete, *ge;
-    double* acc;                       // [ncopy][blk]: rhs | F'r | column norms | S
-    double* total;                     // [blk]: folded / all-rank system
+    double* acc;                       // [blk]: rhs | F'r | column norms | S
+    double* total;                     // [blk]: all-rank system (multi-GPU)
     double* scal;                      // [2][SC_COUNT]
     double *z, *sc_cam, *counts;
     double* panel;                     // [CH_NB][n + 24]: row panel of the blocked Cholesky (read by every CTA of the group)
     unsigned* bar;                     // [0] group barrier counter, [1] abort flag
     Result* result;
     unsigned long long* trace;         // optional [16] per-phase nanoseconds (OV2_BA_TRACE=1), NULL otherwise
-    int ncv_max, ncopy, solve_blocked, smem_work_off, schur_smem, smem_sacc_off;
+    double* cam_tab;                   // NULL: keyframe table in shared memory; else [G][cam_tab_stride] in global memory
+    size_t cam_tab_stride;             // doubles per CTA: [ncam][12] Rwc | twc, then [ncam] int slots
+    int ncv_max, solve_blocked, smem_work_off, schur_smem, smem_sacc_off;
     int sg;                            // lanes per landmark in the per-landmark phases (4, 8 or 32)
     const int32_t* pair_perm;          // [nobs] observation indices sorted by (anchor keyframe, observing keyframe)   (owner mode)
     const int2* pair_chunk;            // [npchunk] (begin, end) into pair_perm, <= PCH observations of ONE pair each
     int npchunk;
-    int gj2;                           // reduced solve n <= 48: two pivots per barrier
     size_t blk;
 };
 

@@ -41,7 +41,6 @@ extern "C" void ov2_destroy(ov2_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     for (auto& ch : ctx->chunks) cudaFree(ch.p);
-    if (ctx->ba_hscal) cudaFreeHost(ctx->ba_hscal);
     if (ctx->ba_stop) cudaFreeHost(ctx->ba_stop);
     if (ctx->ba_ws) cudaFreeHost(ctx->ba_ws);   // pinned staging block of the BA path
     if (ctx->desc_table) cudaFree(ctx->desc_table);

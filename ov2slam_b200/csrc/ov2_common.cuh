@@ -40,7 +40,6 @@ struct ov2_ctx {
     void* ba_ws = nullptr; size_t ba_ws_cap = 0;
     int desc_mode = 0;            // OV2_DESC_* (ov2_describe_config)
     int8_t* desc_table = nullptr; // device copy of the BRIEF-32 test pairs [256][4]
-    double* ba_hscal = nullptr;   // pinned: per-iteration scalar readbacks of the LM controller (legacy path)
     int* ba_stop = nullptr;       // mapped pinned int: stop request polled by the persistent solve kernel
     // optional per-kernel CUDA-event timing (ov2_profile_enable): serialises launches
     bool profiling = false;

@@ -1,5 +1,5 @@
 """Wall time and per-kernel CUDA-event times of one localBA configuration.
-    python scripts/ba_profile.py NCAM NPTS NOBS [reps]      (OV2_BA_SOLVER=0/1/4 forces a reduced-solve path)"""
+    python scripts/ba_profile.py NCAM NPTS NOBS [reps]"""
 import json, os, sys, time
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np
@@ -20,8 +20,7 @@ ctx.profile(True)
 for p in [clone(pb0) for _ in range(reps)]:
     opt.local_ba(p)
 rep = ctx.profile_report(); ctx.profile(False)
-print(json.dumps({"config": f"{ncam} KF x {npts} pts x {nobs} obs", "solver": os.environ.get("OV2_BA_SOLVER", "default"),
-                  "wall_ms_per_solve": 1e3 * wall, "lm_iterations": res["iters_robust"] + res["iters_refine"],
+print(json.dumps({"config": f"{ncam} KF x {npts} pts x {nobs} obs", "wall_ms_per_solve": 1e3 * wall, "lm_iterations": res["iters_robust"] + res["iters_refine"],
                   "final_cost": res["final_cost"],
                   "kernel_ms_per_solve": {k: round(v[0] / reps, 4) for k, v in rep.items()},
                   "launches_per_solve": {k: v[1] / reps for k, v in rep.items()}}))

@@ -1,5 +1,5 @@
-"""C3 / C5 solve rate of the persistent local-BA kernel vs the number of CTAs per window (OV2_BA_CTAS) and the number of
-privatised accumulation copies (OV2_BA_NCOPY), single solves and batches.  Prints one JSON line per configuration."""
+"""C3 / C5 solve rate of the persistent local-BA kernel vs the number of CTAs per window (OV2_BA_CTAS), single solves and
+batches.  Prints one JSON line per configuration."""
 import json
 import os
 import sys
@@ -30,26 +30,17 @@ def rate(pb, reps):
 c3 = synth.make_ba_problem(3, 10, 2000, 8000)
 c5 = synth.make_ba_problem(5, 50, 20000, 150000)
 for name, pb, reps, ctas_list in (("C3", c3, 40, ["1", "4", "8", "16", "32", "64", "96", "148", None]), ("C5", c5, 5, ["32", "74", "148", None])):
-    for ncopy in (None, "1"):
-        for ctas in ctas_list:
-            for k, v in (("OV2_BA_CTAS", ctas), ("OV2_BA_NCOPY", ncopy)):
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
-            try:
-                v, r = rate(pb, reps)
-                print(json.dumps({"window": name, "ctas": ctas, "ncopy": ncopy, "solves_per_s": round(v, 1), "ms": round(1e3 / v, 4),
-                                  "iters": [r["iters_robust"], r["iters_refine"]], "final_cost": r["final_cost"]}), flush=True)
-            except Exception as e:
-                print(json.dumps({"window": name, "ctas": ctas, "ncopy": ncopy, "error": str(e)[:200]}), flush=True)
-os.environ.pop("OV2_BA_CTAS", None)
-os.environ.pop("OV2_BA_NCOPY", None)
-os.environ["OV2_BA_LEGACY"] = "1"
-for name, pb, reps in (("C3", c3, 40), ("C5", c5, 5)):
-    v, r = rate(pb, reps)
-    print(json.dumps({"window": name, "legacy": True, "solves_per_s": round(v, 1), "ms": round(1e3 / v, 4)}), flush=True)
-os.environ.pop("OV2_BA_LEGACY", None)
+    for ctas in ctas_list:
+        if ctas is None:
+            os.environ.pop("OV2_BA_CTAS", None)
+        else:
+            os.environ["OV2_BA_CTAS"] = ctas
+        try:
+            v, r = rate(pb, reps)
+            print(json.dumps({"window": name, "ctas": ctas, "solves_per_s": round(v, 1), "ms": round(1e3 / v, 4),
+                              "iters": [r["iters_robust"], r["iters_refine"]], "final_cost": r["final_cost"]}), flush=True)
+        except Exception as e:
+            print(json.dumps({"window": name, "ctas": ctas, "error": str(e)[:200]}), flush=True)
 base = [synth.make_ba_problem(100 + i, 10, 2000, 8000) for i in range(8)]
 for K in (16, 64, 128, 256):
     for ctas in ("1", "2", "4", "8", None):

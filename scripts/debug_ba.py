@@ -13,6 +13,5 @@ for keep_types in ((0, 1), (0, 2), (0,), (0, 1, 2)):
     log = []
     r = B.local_ba(ref, log=log, max_iters_robust=1, apply_l2_after_robust=False)
     gpu = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in pb.items()}
-    os.environ["OV2_BA_DEBUG"] = "1"
     g, flags = api.Optimizer(ctx).local_ba(gpu, max_iters_robust=1, apply_l2_after_robust=0)
     print(keep_types, 'ref cand %.8f mcc %.8f' % (log[0]['cand_cost'], log[0]['mcc']), 'pose diff', np.abs(gpu['pose'] - ref['pose']).max(), 'invd', np.abs(gpu['lm_invdepth'] - ref['lm_invdepth']).max())

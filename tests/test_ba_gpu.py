@@ -100,29 +100,13 @@ def test_localba_refine_loss_override(ctx):
     _check(ctx, pb, refine_trivial_loss=True)
 
 
-@pytest.mark.parametrize("ncam,npts,nobs,solver", [
-    (16, 1200, 7000, None), (16, 1200, 7000, "4"),
-    (16, 1200, 7000, "5"), (10, 2000, 8000, "5"),
-    (22, 1500, 9000, None), (22, 1500, 9000, "1"), (22, 1500, 9000, "0"),
-    (50, 4000, 30000, None), (50, 4000, 30000, "0")])
-def test_localba_all_reduced_solver_paths(ctx, monkeypatch, ncam, npts, nobs, solver):
-    """(solver None: the persistent kernel's own choice - shared-memory Gauss-Jordan for n <= 96, blocked Cholesky beyond;
-    a solver id selects the round-1 path, OV2_BA_LEGACY=1, and its reduced-solve modes.)
-    Reduced camera systems of 84, 120 and 288 unknowns through every solver path: register
-    Gauss-Jordan (default for n <= 96), blocked Cholesky with the FP64 tensor-core trailing update
-    (default beyond; forced with OV2_BA_SOLVER=4), unblocked Cholesky in shared memory (=1) and in
-    global/L2 (=0), the one-warp shared-memory Gauss-Jordan candidate (=5, n <= 96), each against the C restatement of the oracle (oracle/ba_ref_c.c, itself pinned to
-    oracle/ba_ref.py)."""
-    if solver is None:
-        monkeypatch.delenv("OV2_BA_SOLVER", raising=False)
-        monkeypatch.delenv("OV2_BA_LEGACY", raising=False)
-    else:
-        monkeypatch.setenv("OV2_BA_SOLVER", solver)
-        monkeypatch.setenv("OV2_BA_LEGACY", "1")
-    from oracle import ba_ref_c
-    pb = synth.make_ba_problem(70 + ncam, ncam, npts, nobs)
+def _check_oracle(ctx, pb, oracle=None):
+    """Against the C restatement of the oracle (oracle/ba_ref_c.c, itself pinned to oracle/ba_ref.py; mono windows only) or
+    the given oracle module: same LM decisions, cost 1e-8, states 1e-6, flags equal up to threshold-borderline observations."""
+    if oracle is None:
+        from oracle import ba_ref_c as oracle
     ref = _clone(pb)
-    r = ba_ref_c.local_ba(ref)
+    r = oracle.local_ba(ref)
     gpu = _clone(pb)
     g, flags = api.Optimizer(ctx).local_ba(gpu)
     assert (g["iters_robust"], g["iters_refine"]) == (r["iters_robust"], r["iters_refine"])
@@ -130,6 +114,36 @@ def test_localba_all_reduced_solver_paths(ctx, monkeypatch, ncam, npts, nobs, so
     assert np.abs(gpu["pose"] - ref["pose"]).max() <= 1e-6
     assert np.abs(gpu["lm_invdepth"] - ref["lm_invdepth"]).max() <= 1e-6
     assert (flags != r["flags"]).sum() <= 2
+
+
+@pytest.mark.parametrize("ncam,npts,nobs", [(16, 1200, 7000), (22, 1500, 9000), (50, 4000, 30000)])
+def test_localba_all_reduced_solver_paths(ctx, ncam, npts, nobs):
+    """Reduced camera systems of 84, 120 and 288 unknowns: shared-memory Gauss-Jordan for n <= 96, blocked Cholesky with
+    the FP64 tensor-core trailing update beyond."""
+    _check_oracle(ctx, synth.make_ba_problem(70 + ncam, ncam, npts, nobs))
+
+
+def _keyframe_table_in_shared_memory(ncam, ncv):
+    """plan_window (csrc/ba_lm.cu) for n > 96: the keyframe table (12 doubles + 1 int per keyframe) stays in shared memory
+    when it fits next to the larger of the Schur scratch and the blocked-Cholesky solve area in 200 KB."""
+    warps, sch, ch_nb, n = 8, 8, 32, 6 * ncv
+    assert n > 96
+    tab = (100 * ncam + 15) & ~15
+    schur = (warps * 6 * (ncv + 1) * 8 + (((warps * (ncv + 1) + 1) >> 1) << 3) + warps * 28 * sch * 8 + warps * sch * 4 + 16 + 15) & ~15
+    solve = ch_nb * (((n + 15) & ~15) + 8) * 8
+    return tab + max(schur, solve) + 16 <= 200 * 1024
+
+
+@pytest.mark.parametrize("seed,ncam,npts,stereo,shared", [(81, 300, 1200, False, True), (84, 2000, 5000, False, False),
+                                                          (83, 1200, 3000, True, False)])
+def test_localba_windows_beyond_256_keyframes(ctx, seed, ncam, npts, stereo, shared):
+    """Windows of more than 256 keyframes, the last 64 optimised (Optimizer::fullBA / looseBA put a whole map or keyframe
+    range in one window; the oldest keyframes are held constant): the keyframe table stays in shared memory up to about a
+    thousand keyframes and moves to one copy per CTA in global memory beyond.  Stereo is checked against the numpy oracle."""
+    assert _keyframe_table_in_shared_memory(ncam, 64) == shared
+    pb = synth.make_ba_problem(seed, ncam, npts, 2 * npts, nconst=ncam - 64, stereo=stereo)
+    assert len(np.unique(np.concatenate([pb["obs_cam"], pb["lm_anchor_cam"]]))) == ncam   # every keyframe observes something
+    _check_oracle(ctx, pb, B if stereo else None)       # the C restatement has no stereo residual blocks
 
 
 def test_localba_c5_size_150k_observations(ctx):
@@ -178,11 +192,6 @@ def test_localba_persistent_kernel_group_sizes(ctx, monkeypatch, ctas):
         monkeypatch.setenv("OV2_BA_CTAS", ctas)
     _check(ctx, synth.make_ba_problem(3, 10, 2000, 8000))
     _check(ctx, synth.make_ba_problem(41, 8, 400, 1600, stereo=True))
-
-
-def test_localba_legacy_path_still_matches(ctx, monkeypatch):
-    monkeypatch.setenv("OV2_BA_LEGACY", "1")
-    _check(ctx, synth.make_ba_problem(3, 10, 2000, 8000))
 
 
 def test_localba_batch_equals_single_solves(ctx):
@@ -245,14 +254,12 @@ def test_localba_bal_structure_fixture(ctx):
     assert (flags != r["flags"]).sum() <= 3
 
 
-@pytest.mark.parametrize("env", [{"OV2_BA_SCHUR_SMEM": "1"}, {"OV2_BA_NCOPY": "4"}, {"OV2_BA_COOP": "1"}, {"OV2_BA_GJ2": "1"},
-                                 {"OV2_BA_SCHUR_SMEM": "3"}, {"OV2_BA_SCHUR_SMEM": "0"}, {"OV2_BA_SCHUR_SMEM": "3", "OV2_BA_SG": "8"},
-                                 {"OV2_BA_SG": "32"}])
+@pytest.mark.parametrize("env", [{"OV2_BA_SCHUR_SMEM": "3"}, {"OV2_BA_SCHUR_SMEM": "0"}, {"OV2_BA_SCHUR_SMEM": "3", "OV2_BA_SG": "8"},
+                                 {"OV2_BA_SG": "32"}], ids=["owner", "red", "owner-sg8", "sg32"])
 def test_localba_optional_kernel_modes(ctx, monkeypatch, env):
-    """The opt-in variants of the persistent kernel stay correct: shared-memory Schur accumulation under a CTA lock, privatised
-    accumulation copies + fold phase, cooperative launch, two-pivot Gauss-Jordan steps, and - forced on a SINGLE window - the
-    owner-mode Schur phase that batches use by default (pair-sorted Gram blocks + DMMA landmark rows), the plain RED path, and
-    the other sub-group widths of the per-landmark phases."""
+    """Paths of the persistent kernel that other windows take by default, forced on a SINGLE window: the owner-mode Schur
+    phase that batches use (pair-sorted Gram blocks + DMMA landmark rows), the plain RED path, and the other sub-group widths
+    of the per-landmark phases."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
     _check(ctx, synth.make_ba_problem(3, 10, 2000, 8000))

@@ -1,10 +1,9 @@
-"""Multi-GPU localBA (SURVEY.md 8e): landmark partitioning + one sum-allreduce of the reduced
-camera system per LM iteration.
+"""Multi-GPU localBA (SURVEY.md 8e): landmark partitioning + an in-kernel sum of the reduced camera
+system over peer memory every LM iteration.
 
-CPU: the partition is a partition, and the allreduce callback sums across a 2-process gloo group.
-GPU (one device): two shards run concurrently on two contexts with a loop-back "fake NCCL"
-allreduce (thread barrier + sum) and must reproduce the unsharded solve."""
-import os
+CPU: the partition is a partition.
+GPU (one device): the ranks' shards run concurrently on contexts of one process and must reproduce
+the unsharded solve; windows the exchange buffer cannot hold are refused before any launch."""
 import threading
 
 import numpy as np
@@ -27,107 +26,6 @@ def test_partition_is_a_balanced_partition():
             assert np.array_equal(lms[sh["obs_lm"]], pb["obs_lm"][obs])     # remap is consistent
             assert np.array_equal(sh["obs_px"], pb["obs_px"][obs])
             assert np.array_equal(sh["pose"], pb["pose"])
-
-
-def _gloo_worker(rank, world, port, q):
-    import ctypes as C
-    import torch
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from ov2slam_b200 import api as A
-    A.load()
-    cb = A.make_torch_allreduce(dist, torch)
-    buf = np.arange(10, dtype=np.float64) * (rank + 1)
-    rc = cb(None, buf.ctypes.data, 10, None)
-    dist.barrier()
-    dist.destroy_process_group()
-    q.put((rank, rc, buf.tolist()))
-
-
-def test_allreduce_callback_sums_over_gloo_group():
-    import multiprocessing as mp
-    from ov2slam_b200 import build
-    build.build()                                           # before the workers start: on a fresh checkout both would compile it at once
-    ctxmp = mp.get_context("spawn")
-    q = ctxmp.Queue()
-    port = 29500 + os.getpid() % 2000
-    ps = [ctxmp.Process(target=_gloo_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in ps:
-        p.start()
-    out = [q.get(timeout=120) for _ in ps]
-    for p in ps:
-        p.join(timeout=60)
-    for rank, rc, buf in out:
-        assert rc == 0
-        assert buf == (np.arange(10) * 3.0).tolist()       # 1x + 2x summed on both ranks
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("world,empty", [(2, False), (3, False), (3, True)])
-def test_sharded_solve_matches_unsharded(ctx, world, empty):
-    """The round-1 callback path (ov2_localba_solve_sharded).  With `empty` the last rank owns no landmark and no observation:
-    it must still take part in every all-reduce (ADVICE r1: zero-block launches made it return early and hang the others)."""
-    import ctypes as C
-    import torch
-    pb = synth.make_ba_problem(31, 12, 1500, 9000)
-    ref = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in pb.items()}
-    rres, rflags = api.Optimizer(ctx).local_ba(ref)
-    shards = api.partition_ba_problem(pb, world - 1 if empty else world)
-    if empty:
-        e = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in shards[0][0].items()}
-        for k in ("lm_anchor_cam", "lm_anchor_px", "lm_invdepth", "obs_cam", "obs_lm", "obs_px"):
-            e[k] = e[k][:0].copy()
-        shards.append((e, np.zeros(0, np.int64), np.zeros(0, np.int64)))
-    ctxs = [api.Context(0) for _ in range(world)]
-    barrier = threading.Barrier(world)
-    slots = [None] * world
-    total = [None]
-
-    def make_cb(rank):
-        def fn(user, buf, count, stream):
-            t = torch.as_tensor(api._CudaView(buf, count), device="cuda")
-            torch.cuda.synchronize()
-            slots[rank] = t
-            barrier.wait()
-            if rank == 0:
-                total[0] = torch.stack([s.clone() for s in slots]).sum(0)
-            barrier.wait()
-            t.copy_(total[0])
-            torch.cuda.synchronize()
-            barrier.wait()
-            return 0
-        return api.ALLREDUCE_FN(fn)
-
-    results = [None] * world
-    errs = []
-
-    def run(rank):
-        try:
-            results[rank] = api.local_ba_sharded(ctxs[rank], shards[rank][0], make_cb(rank), rank)
-        except Exception as e:  # pragma: no cover
-            errs.append(e)
-            barrier.abort()
-
-    ths = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-    for t in ths:
-        t.start()
-    for t in ths:
-        t.join(timeout=120)
-    assert not errs, errs
-    invd = np.zeros(len(pb["lm_invdepth"]))
-    flags = np.zeros(len(pb["obs_cam"]), np.uint8)
-    for r, (sh, lms, obs) in enumerate(shards):
-        res, fl = results[r]
-        assert res["iters_robust"] == rres["iters_robust"] and res["iters_refine"] == rres["iters_refine"]
-        assert abs(res["final_cost"] - rres["final_cost"]) <= 1e-9 * max(1.0, rres["final_cost"])
-        assert np.abs(sh["pose"] - ref["pose"]).max() <= 1e-7
-        invd[lms] = sh["lm_invdepth"]
-        flags[obs] = fl
-    assert np.abs(invd - ref["lm_invdepth"]).max() <= 1e-7
-    assert (flags != rflags).sum() <= 2
-    for c in ctxs:
-        c.close()
 
 
 @pytest.mark.gpu
@@ -185,6 +83,37 @@ def test_p2p_sharded_solve_matches_unsharded(ctx, monkeypatch, world, empty):
             flags[obs] = fl
         assert np.abs(invd - ref["lm_invdepth"]).max() <= 1e-7
         assert (flags != rflags).sum() <= 2
+    for c in comms:
+        c.close()
+    for c in ctxs:
+        c.close()
+
+
+@pytest.mark.gpu
+def test_p2p_refuses_windows_beyond_256_keyframes_before_launch(ctx):
+    """The exchange buffer holds 256 keyframes: with world > 1 every rank must refuse a larger window on the host, so no rank
+    launches a kernel that would wait in a rank barrier for a peer that never started."""
+    pb = synth.make_ba_problem(84, 300, 1200, 2400, nconst=236)
+    shards = api.partition_ba_problem(pb, 2)
+    ctxs = [api.Context(0) for _ in range(2)]
+    comms = [api.BaComm(ctxs[r], r, 2) for r in range(2)]
+    api.BaComm.connect_local(comms)
+    launches = [c.launch_count() for c in ctxs]
+    errs = [None, None]
+
+    def run(rank):
+        try:
+            comms[rank].local_ba(shards[rank][0])
+        except api.Ov2Error as ex:
+            errs[rank] = ex
+
+    ths = [threading.Thread(target=run, args=(r,)) for r in range(2)]
+    for t in ths:
+        t.start()
+    for t in ths:
+        t.join(timeout=120)
+    assert all(isinstance(e, api.Ov2Error) for e in errs), errs
+    assert [c.launch_count() for c in ctxs] == launches
     for c in comms:
         c.close()
     for c in ctxs:

@@ -322,48 +322,6 @@ extern "C" int pnp_host(int n, const double* unpx, const double* wpts, const dou
             assert np.abs(est - est_r).max() <= 1e-9, (case, np.abs(est - est_r).max())
 
 
-def test_warp_gauss_jordan_lane_code_solves_spd_systems(tmp_path):
-    """ov2slam_b200/csrc/ge_warp.cuh (the one-warp reduced-camera solve, OV2_BA_SOLVER=5) run lane by lane on
-    the host vs numpy.linalg.solve on damped SPD systems of every window size up to 96 unknowns, plus the
-    failure report on a non-positive pivot."""
-    import numpy as np
-    src = tmp_path / "g.cpp"
-    src.write_text(r'''
-#include "%s/ov2slam_b200/csrc/ge_warp.cuh"
-extern "C" int ge_host(int n, double* A, double* x) {      // A: n x pitch(n) augmented, row-major
-    const int P = gewarp::pitch(n);
-    for (int j = 0; j < n; ++j) {
-        bool ok = true;
-        for (int lane = 0; lane < 32; ++lane) ok = gewarp::step(lane, A, n, P, j) && ok;
-        if (!ok) return 0;
-    }
-    for (int lane = 0; lane < 32; ++lane) gewarp::finish(lane, A, n, P, x);
-    return 1;
-}
-extern "C" int ge_pitch(int n) { return gewarp::pitch(n); }''' % ROOT)
-    so = tmp_path / "libg.so"
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", str(so), str(src)])
-    lib = ctypes.CDLL(str(so))
-    lib.ge_host.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
-    rng = np.random.default_rng(4)
-    for n in (6, 12, 31, 32, 33, 48, 63, 64, 90, 96):
-        J = rng.standard_normal((3 * n, n))
-        S = J.T @ J + np.diag(rng.uniform(1e-4, 1e-2, n))       # Schur complement + LM damping: SPD
-        b = rng.standard_normal(n)
-        P = lib.ge_pitch(n)
-        assert P % 2 == 1 and P >= n + 1
-        A = np.zeros((n, P))
-        A[:, :n] = S
-        A[:, n] = b
-        x = np.zeros(n)
-        assert lib.ge_host(n, A.ctypes.data, x.ctypes.data) == 1
-        ref = np.linalg.solve(S, b)
-        assert np.abs(x - ref).max() <= 1e-9 * max(1.0, np.abs(ref).max()), n
-    A = np.zeros((4, lib.ge_pitch(4)))
-    A[:4, :4] = np.diag([1.0, -1.0, 1.0, 1.0])
-    assert lib.ge_host(4, A.ctypes.data, np.zeros(4).ctypes.data) == 0
-
-
 def test_device_lm_controller_replays_the_oracle_decisions(tmp_path):
     """csrc/ba_lm_ctl.cuh (the trust-region controller every CTA of the persistent solve kernel replays on the device)
     compiled for the host and driven with the per-iteration scalars of the oracle (oracle/ba_ref.py): same iteration
