@@ -6,11 +6,14 @@
 //   drop keypoints whose rounded centre is closer than 31 px to the border,
 //   smooth the image with a float32 separable 7-tap Gaussian (sigma 2) and round to u8,
 //   256 intensity comparisons on the ORB pattern around c = cvRound(pt)   (SURVEY.md A.5).
-// Instead of smoothing the whole image (2 x W x H bytes of traffic per frame) each warp smooths
-// only the 26x26 window the pattern touches, from a 32x32 raw window, in shared memory, with
-// exactly OpenCV's float operation order (rows: sequential FMA chain; columns: symmetric pairs +
-// FMA; pinned bit-exact by oracle/image_ref.py::smooth7_ref against cv2).  Keypoints are >= 31 px
-// from the border, so the 32x32 window never needs the REFLECT_101 border.
+// For sparse keypoint sets, instead of smoothing the whole image (2 x W x H bytes of traffic per
+// frame) each warp smooths only the 26x26 window the pattern touches, from a 32x32 raw window, in
+// shared memory, with exactly OpenCV's float operation order (rows: sequential FMA chain; columns:
+// symmetric pairs + FMA; pinned bit-exact by oracle/image_ref.py::smooth7_ref against cv2).
+// Keypoints are >= 31 px from the border, so the 32x32 window never needs the REFLECT_101 border.
+// Dense fixed-stride sets, whose windows would smooth every reachable pixel several times over (C2's
+// 1024 keypoints per 640x480 frame: 2.6 times), take the dense path instead: one smoothing pass per
+// frame into a scratch plane, then a gather per keypoint (ov2_describe picks by density).
 //
 // The descriptor is DATA-driven (ov2_describe_config): mode OV2_DESC_ORB_FALLBACK is the above; mode
 // OV2_DESC_BRIEF32 is the reference's DEFAULT build (CMakeLists.txt:12 WITH_OPENCV_CONTRIB,
@@ -38,6 +41,63 @@ struct DescArgs {
     uint8_t* desc; uint8_t* valid;
 };
 
+// The two passes of the 7-tap smoothing, shared by the per-window and the dense kernels so that both
+// produce the same bytes.  Row: output at the centre tap x3, sequential FMA chain exactly as OpenCV's
+// float row filter evaluates it.
+__device__ __forceinline__ float smooth_row7(float x0, float x1, float x2, float x3, float x4, float x5, float x6,
+                                             float k0, float k1, float k2, float k3) {
+    float acc = x0 * k0;
+    acc = __fmaf_rn(x1, k1, acc);
+    acc = __fmaf_rn(x2, k2, acc);
+    acc = __fmaf_rn(x3, k3, acc);
+    acc = __fmaf_rn(x4, k2, acc);
+    acc = __fmaf_rn(x5, k1, acc);
+    acc = __fmaf_rn(x6, k0, acc);
+    return acc;
+}
+
+// Column: output at the centre tap y3, symmetric pairs + FMA as OpenCV's float column filter, then
+// saturate_cast<uchar> (round half to even, clamp).  The clamp comes first, which gives the same integer
+// because rint is monotone and 0, 255 are integers; adding 1.5 * 2^23 then rounds to an integer in the low
+// mantissa bits (exact below 2^22), so the conversion stays on the FP32 pipe.  Returns the value in bits 0..7.
+__device__ __forceinline__ unsigned smooth_col7(float y0, float y1, float y2, float y3, float y4, float y5, float y6,
+                                                float k0, float k1, float k2, float k3) {
+    float acc = y3 * k3;
+    acc = __fmaf_rn(y2 + y4, k2, acc);
+    acc = __fmaf_rn(y1 + y5, k1, acc);
+    acc = __fmaf_rn(y0 + y6, k0, acc);
+    acc = fminf(fmaxf(acc, 0.f), 255.f);
+    return __float_as_uint(acc + 12582912.f) & 255u;
+}
+
+// ORB-fallback border rule, KeyPointsFilter::runByImageBorder(kps, size, 31) on the rounded point; x < 0
+// marks an empty slot.  Writes the zero descriptor and valid = 0 for a dropped point.
+__device__ __forceinline__ bool orb_drop(const DescArgs& A, int i, float2 pt, int cx, int cy, int lane) {
+    if (pt.x < 0.f || cx < 31 || cy < 31 || cx >= A.w - 31 || cy >= A.h - 31) {
+        A.desc[(size_t)i * 32 + lane] = 0;
+        if (lane == 0) A.valid[i] = 0;
+        return true;
+    }
+    return false;
+}
+
+// 8 tests per lane -> descriptor byte `lane`; at(dx, dy) reads the smoothed pixel at offset (dx, dy) from the
+// rounded centre
+template <class At>
+__device__ __forceinline__ unsigned orb_byte(int lane, At at) {
+    const int4 pa = __ldg(reinterpret_cast<const int4*>(&g_pat[lane * 8][0]));
+    const int4 pb = __ldg(reinterpret_cast<const int4*>(&g_pat[lane * 8 + 4][0]));
+    const int pw[8] = {pa.x, pa.y, pa.z, pa.w, pb.x, pb.y, pb.z, pb.w};
+    unsigned byte = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int t0 = (int)(signed char)(pw[k] & 255), t1 = (int)(signed char)((pw[k] >> 8) & 255);
+        const int t2 = (int)(signed char)((pw[k] >> 16) & 255), t3 = (int)(signed char)((pw[k] >> 24) & 255);
+        byte |= (unsigned)(at(t0, t1) < at(t2, t3)) << k;
+    }
+    return byte;
+}
+
 __global__ void __launch_bounds__(WARPS * 32) describe_kernel(DescArgs A) {
     __shared__ float sraw[WARPS][32 * 33];   // 32x32 raw window as float (+1 pad: conflict-free rows); row-filtered IN PLACE
     __shared__ uint8_t ssm[WARPS][26 * 28];  // 26 x 26 smoothed (+2 pad)
@@ -47,12 +107,7 @@ __global__ void __launch_bounds__(WARPS * 32) describe_kernel(DescArgs A) {
     const float2 pt = A.pts[i];
     const int cx = __float2int_rn(pt.x), cy = __float2int_rn(pt.y);
     uint8_t* dout = A.desc + (size_t)i * 32;
-    // KeyPointsFilter::runByImageBorder(kps, size, 31) tests the rounded point; x < 0 marks an empty slot
-    if (pt.x < 0.f || cx < 31 || cy < 31 || cx >= A.w - 31 || cy >= A.h - 31) {
-        dout[lane] = 0;
-        if (lane == 0) A.valid[i] = 0;
-        return;
-    }
+    if (orb_drop(A, i, pt, cx, cy, lane)) return;
     const int frame = A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame;
     const uint8_t* img = A.img + A.fstride * frame + (size_t)(cy - 16) * A.pitch + (cx - 16);
     float* raw = sraw[warp];
@@ -63,59 +118,131 @@ __global__ void __launch_bounds__(WARPS * 32) describe_kernel(DescArgs A) {
     for (int r = 0; r < 32; ++r) raw[r * 33 + lane] = (float)__ldg(img + (size_t)r * A.pitch + lane);
     __syncwarp();
     const float k0 = c_gk[0], k1 = c_gk[1], k2 = c_gk[2], k3 = c_gk[3];
-    // row filter, lane = row: output col c (0..25) <-> image col cx-13+c, taps raw cols c..c+6,
-    // sequential FMA chain exactly as OpenCV's float row filter evaluates it
+    // row filter, lane = row: output col c (0..25) <-> image col cx-13+c, taps raw cols c..c+6
     {
         const float* p = raw + lane * 33;
         float x0 = p[0], x1 = p[1], x2 = p[2], x3 = p[3], x4 = p[4], x5 = p[5];
 #pragma unroll
         for (int c = 0; c < 26; ++c) {
             const float x6 = p[c + 6];
-            float acc = x0 * k0;
-            acc = __fmaf_rn(x1, k1, acc);
-            acc = __fmaf_rn(x2, k2, acc);
-            acc = __fmaf_rn(x3, k3, acc);
-            acc = __fmaf_rn(x4, k2, acc);
-            acc = __fmaf_rn(x5, k1, acc);
-            acc = __fmaf_rn(x6, k0, acc);
-            row[lane * 33 + c] = acc;
+            row[lane * 33 + c] = smooth_row7(x0, x1, x2, x3, x4, x5, x6, k0, k1, k2, k3);
             x0 = x1; x1 = x2; x2 = x3; x3 = x4; x4 = x5; x5 = x6;
         }
     }
     __syncwarp();
     // column filter, lane = column: output row q (0..25) <-> image row cy-13+q, taps rows q..q+6
-    // (centre q+3), symmetric pairs + FMA as OpenCV's float column filter, rint -> u8
     if (lane < 26) {
         const float* p = row + lane;
         float y0 = p[0], y1 = p[33], y2 = p[2 * 33], y3 = p[3 * 33], y4 = p[4 * 33], y5 = p[5 * 33];
 #pragma unroll
         for (int q = 0; q < 26; ++q) {
             const float y6 = p[(q + 6) * 33];
-            float acc = y3 * k3;
-            acc = __fmaf_rn(y2 + y4, k2, acc);
-            acc = __fmaf_rn(y1 + y5, k1, acc);
-            acc = __fmaf_rn(y0 + y6, k0, acc);
-            int v = __float2int_rn(acc);
-            v = v < 0 ? 0 : (v > 255 ? 255 : v);
-            sm[q * 28 + lane] = (uint8_t)v;
+            sm[q * 28 + lane] = (uint8_t)smooth_col7(y0, y1, y2, y3, y4, y5, y6, k0, k1, k2, k3);
             y0 = y1; y1 = y2; y2 = y3; y3 = y4; y4 = y5; y5 = y6;
         }
     }
     __syncwarp();
-    // 8 tests per lane -> one descriptor byte per lane
-    unsigned byte = 0;
-    const int4 pa = __ldg(reinterpret_cast<const int4*>(&g_pat[lane * 8][0]));
-    const int4 pb = __ldg(reinterpret_cast<const int4*>(&g_pat[lane * 8 + 4][0]));
-    const int pw[8] = {pa.x, pa.y, pa.z, pa.w, pb.x, pb.y, pb.z, pb.w};
+    dout[lane] = (uint8_t)orb_byte(lane, [&](int dx, int dy) { return (int)sm[(dy + 13) * 28 + (dx + 13)]; });
+    if (lane == 0) A.valid[i] = 1;
+}
+
+
+// ---- Dense path for keypoint sets that cover each frame several times over (see ov2_describe): the smoothed
+// image is computed once per frame into a plane, then every keypoint reads its 512 test pixels from it.
+// Plane: same geometry as level 0 (pitch rounded up to 16 bytes), written only where a valid keypoint's pattern
+// can reach (centres >= 31 px from the border, pattern radius 13): rows [18, h - 18) and a column band [16, ...)
+// that covers [18, w - 18) in runs of SMOOTH_COLS.  The filter reaches 3 px, so every tap lies inside the image
+// and no border handling is needed.  Needs w, h >= 63 (the smallest frame with a valid centre).
+constexpr int SMOOTH_COLS = 8;    // output columns per thread (one 8-byte store per row)
+constexpr int SMOOTH_ROWS = 16;   // output rows per thread (SMOOTH_ROWS + 6 row-filtered rows in registers)
+constexpr int SMOOTH_THREADS = 128;
+
+struct SmoothArgs {
+    const uint8_t* img; int pitch; long long fstride;
+    int first_frame, h;
+    int ncs, nrs;                 // column runs and row runs per frame
+    uint8_t* plane; int ppitch; long long pfstride;
+};
+
+__global__ void __launch_bounds__(SMOOTH_THREADS) desc_smooth_kernel(SmoothArgs S) {
+    const int t = blockIdx.x * SMOOTH_THREADS + threadIdx.x;
+    if (t >= S.ncs * S.nrs) return;
+    const int cs = t % S.ncs, rs = t / S.ncs;
+    const int x0 = 16 + SMOOTH_COLS * cs;
+    // the last row run is pulled up to end at h - 18 (overlapping runs write the same bytes); rows read stay in
+    // [15, h - 16)
+    const int y0 = min(18 + SMOOTH_ROWS * rs, S.h - 18 - SMOOTH_ROWS);
+    // taps of output columns x0 .. x0+7 are image columns x0-3 .. x0+10; read the 16 bytes x0-4 .. x0+11 as five
+    // aligned words (the row and the pitch need not be aligned) and funnel-shift them into place.  x0+7 <= w - 12,
+    // so every word lies inside the row.
+    const uint8_t* src = S.img + S.fstride * (S.first_frame + (int)blockIdx.y) + (size_t)(y0 - 3) * S.pitch + (x0 - 4);
+    uint8_t* dst = S.plane + S.pfstride * (int)blockIdx.y + (size_t)y0 * S.ppitch + x0;
+    const float k0 = c_gk[0], k1 = c_gk[1], k2 = c_gk[2], k3 = c_gk[3];
+    auto row_words = [&](int r, unsigned* wd) {
+        const unsigned* wp = reinterpret_cast<const unsigned*>(((uintptr_t)src + (size_t)r * S.pitch) & ~(uintptr_t)3);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int t0 = (int)(signed char)(pw[k] & 255), t1 = (int)(signed char)((pw[k] >> 8) & 255);
-        const int t2 = (int)(signed char)((pw[k] >> 16) & 255), t3 = (int)(signed char)((pw[k] >> 24) & 255);
-        int a = sm[(t1 + 13) * 28 + (t0 + 13)];
-        int b = sm[(t3 + 13) * 28 + (t2 + 13)];
-        byte |= (unsigned)(a < b) << k;
+        for (int k = 0; k < 5; ++k) wd[k] = __ldg(wp + k);
+    };
+    unsigned nxt[5];              // words of the next row, loaded one row ahead of their use
+    row_words(0, nxt);
+    float win[7][SMOOTH_COLS];    // row-filtered rows y-3 .. y+3 of the next output row y
+#pragma unroll
+    for (int r = 0; r < SMOOTH_ROWS + 6; ++r) {
+        const unsigned w0 = nxt[0], w1 = nxt[1], w2 = nxt[2], w3 = nxt[3], w4 = nxt[4];
+        const unsigned s = (unsigned)(((uintptr_t)src + (size_t)r * S.pitch) & 3) * 8;
+        if (r + 1 < SMOOTH_ROWS + 6) row_words(r + 1, nxt);
+        const unsigned b[4] = {__funnelshift_r(w0, w1, s), __funnelshift_r(w1, w2, s), __funnelshift_r(w2, w3, s),
+                               __funnelshift_r(w3, w4, s)};
+        // byte j of b <-> image column x0-4+j; u8 -> float as (2^23 + v) - 2^23 (exact), on the FP32 pipe
+        float f[16];
+#pragma unroll
+        for (int j = 1; j < 15; ++j)
+            f[j] = __uint_as_float(__byte_perm(b[j >> 2], 0x4B000000u, 0x7650 | (j & 3))) - 8388608.f;
+#pragma unroll
+        for (int q = 0; q < 6; ++q)
+#pragma unroll
+            for (int c = 0; c < SMOOTH_COLS; ++c) win[q][c] = win[q + 1][c];
+#pragma unroll
+        for (int c = 0; c < SMOOTH_COLS; ++c)
+            win[6][c] = smooth_row7(f[c + 1], f[c + 2], f[c + 3], f[c + 4], f[c + 5], f[c + 6], f[c + 7], k0, k1, k2, k3);
+        if (r >= 6) {
+            unsigned v[SMOOTH_COLS];
+#pragma unroll
+            for (int c = 0; c < SMOOTH_COLS; ++c)
+                v[c] = smooth_col7(win[0][c], win[1][c], win[2][c], win[3][c], win[4][c], win[5][c], win[6][c], k0, k1, k2, k3);
+            const uint2 o = make_uint2(v[0] | v[1] << 8 | v[2] << 16 | v[3] << 24, v[4] | v[5] << 8 | v[6] << 16 | v[7] << 24);
+            *reinterpret_cast<uint2*>(dst + (size_t)(r - 6) * S.ppitch) = o;
+        }
     }
-    dout[lane] = (uint8_t)byte;
+}
+
+struct DenseArgs {
+    DescArgs d;
+    const uint8_t* plane; int ppitch; long long pfstride;
+};
+
+// One warp per keypoint, lane = descriptor byte.  The 27 x 27 patch the pattern touches is first copied from the
+// plane into shared memory as aligned words (4 rows x 8 words per load), so the 512 scattered byte reads hit
+// shared memory instead of costing one L1 wavefront per distinct line.
+__global__ void __launch_bounds__(WARPS * 32) describe_dense_kernel(DenseArgs D) {
+    __shared__ unsigned spatch[WARPS][27 * 8];   // rows cy-13 .. cy+13, columns xb .. xb+31 (xb = (cx-13) & ~3)
+    const DescArgs& A = D.d;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * WARPS + warp;
+    if (i >= A.n) return;
+    const float2 pt = A.pts[i];
+    const int cx = __float2int_rn(pt.x), cy = __float2int_rn(pt.y);
+    if (orb_drop(A, i, pt, cx, cy, lane)) return;
+    // plane rows are 16-byte aligned, so column alignment is address alignment; xb + 31 <= cx + 18 < pitch
+    const int xb = (cx - 13) & ~3;
+    const uint8_t* base = D.plane + D.pfstride * (i / A.per_frame) + (size_t)(cy - 13) * D.ppitch + xb;
+    unsigned* patch = spatch[warp];
+#pragma unroll
+    for (int r = lane >> 3; r < 27; r += 4)
+        patch[r * 8 + (lane & 7)] = __ldg(reinterpret_cast<const unsigned*>(base + (size_t)r * D.ppitch) + (lane & 7));
+    __syncwarp();
+    const uint8_t* pb = reinterpret_cast<const uint8_t*>(patch) + 13 * 32 + (cx - xb);
+    A.desc[(size_t)i * 32 + lane] = (uint8_t)orb_byte(lane, [&](int dx, int dy) { return (int)pb[dy * 32 + dx]; });
     if (lane == 0) A.valid[i] = 1;
 }
 
@@ -207,6 +334,23 @@ __global__ void __launch_bounds__(WARPS * 32) describe_box_kernel(BoxArgs B) {
 
 bool g_tables_loaded[64] = {false};
 
+// Dense path (smooth each frame once, then gather) when the keypoints' 26 x 26 windows cover the band a valid
+// keypoint can reach, (w - 36) x (h - 36), at least DENSE_COVER times over.  The per-window kernel costs about
+// per_frame * 26^2 smoothed pixels per frame, the dense one (w - 36)(h - 36) pixels plus a plane write and read.
+// Measured with scripts/bench_describe.py (640 x 480, batch 256, H100 SXM 80GB at its 700 W limit, 1980 MHz):
+// per-window / dense ms per call 0.145 / 0.151 at cover 1.29 (512 per frame), 0.212 / 0.175 at cover 1.94 (768),
+// 0.279 / 0.199 at cover 2.58 (1024); the lines cross near cover 1.4.
+constexpr float DENSE_COVER = 1.4f;
+
+// Fixed-stride ORB-fallback calls only (ragged frame_idx calls keep the per-window kernel); OV2_DESC_DENSE=0 / 1
+// forces the per-window / dense path for those calls.
+bool use_dense(const int32_t* frame_idx, int per_frame, int w, int h) {
+    if (frame_idx || w < 63 || h < 63) return false;   // below 63 px no keypoint is valid
+    const char* e = getenv("OV2_DESC_DENSE");
+    if (e && *e) return atoi(e) != 0;
+    return (double)per_frame * 26.0 * 26.0 >= (double)DENSE_COVER * (w - 36) * (h - 36);
+}
+
 }  // namespace
 
 
@@ -271,6 +415,24 @@ extern "C" ov2_status ov2_describe(ov2_ctx* ctx, const ov2_pyr* pyr, int n, cons
         B.d = A;
         B.table = (const signed char*)ctx->desc_table;
         OV2_LAUNCH(ctx, "describe_box_kernel", describe_box_kernel<<<div_up(n, WARPS), WARPS * 32, 0, ctx->stream>>>(B));
+    } else if (use_dense(frame_idx, per_frame, A.w, A.h)) {
+        const int nframes = div_up(n, per_frame);
+        DenseArgs D;
+        D.d = A;
+        D.ppitch = (A.w + 15) & ~15;
+        D.pfstride = (long long)D.ppitch * A.h;
+        void* pl = nullptr;
+        if ((st = ov2_scratch(ctx, (size_t)D.pfstride * nframes, &pl)) != OV2_OK) return st;
+        D.plane = (const uint8_t*)pl;
+        SmoothArgs S;
+        S.img = A.img; S.pitch = A.pitch; S.fstride = A.fstride;
+        S.first_frame = first_frame; S.h = A.h;
+        S.ncs = div_up(A.w - 34, SMOOTH_COLS);
+        S.nrs = div_up(A.h - 36, SMOOTH_ROWS);
+        S.plane = (uint8_t*)pl; S.ppitch = D.ppitch; S.pfstride = D.pfstride;
+        OV2_LAUNCH(ctx, "desc_smooth_kernel",
+                   desc_smooth_kernel<<<dim3(div_up(S.ncs * S.nrs, SMOOTH_THREADS), nframes), SMOOTH_THREADS, 0, ctx->stream>>>(S));
+        OV2_LAUNCH(ctx, "describe_dense_kernel", describe_dense_kernel<<<div_up(n, WARPS), WARPS * 32, 0, ctx->stream>>>(D));
     } else {
         OV2_LAUNCH(ctx, "describe_kernel", describe_kernel<<<div_up(n, WARPS), WARPS * 32, 0, ctx->stream>>>(A));
     }
