@@ -366,7 +366,9 @@ typedef struct {
 /* outlier_out (optional): [nobs] bytes, bit0 = flagged after solve #1, bit1 = after solve #2.
  * The whole two-stage solve (both Ceres solves, every LM iteration, both outlier scans) is ONE kernel launch with the
  * trust-region controller on the device (csrc/ba_lm.cu).  At most 64 optimised keyframes per window (OV2_ERR_CAPACITY
- * beyond); no limit on the total keyframe count (constant keyframes included).
+ * beyond): non-constant keyframes that no residual touches (or only right-camera residuals in their own anchor frame,
+ * obs_type 2) drop out of the problem as in Ceres and do not count, except in a multi-GPU window, where every declared
+ * non-constant keyframe counts.  No limit on the total keyframe count (constant keyframes included).
  * Residency of a window's arrays is decided on `pose`: host poses = every array of the window (and outlier_out) is host
  * memory, the reference's flow; device poses = each array is inspected and may be either. */
 OV2_API ov2_status ov2_localba_solve(ov2_ctx* ctx, const ov2_ba_problem* pb, const ov2_ba_opts* opts,

@@ -1599,6 +1599,22 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     const int ncam = pb->ncam, npts = pb->npts, nobs = pb->nobs;
     int ncv = 0;
     for (int c = 0; c < ncam; ++c) ncv += pb->pose_const[c] ? 0 : 1;
+    if (world == 1 && ncv > 0) {
+        // Optimised keyframes are the non-constant ones some pose-dependent residual touches as observer or anchor
+        // (Program::RemoveFixedBlocks drops the others; the kernel's rule in each stage).  Every residual starts active and
+        // the active set only shrinks, so this count bounds both stages.  A rank of a multi-GPU window sees only its own
+        // shard and keeps the declared count.  The scan stops once every declared keyframe has been seen.
+        std::vector<uint8_t> seen((size_t)ncam, 0);
+        int nused = 0;
+        for (int i = 0; i < nobs && nused < ncv; ++i) {
+            if (pb->obs_type && pb->obs_type[i] == 2) continue;
+            const int l = pb->obs_lm[i];
+            if (l < 0 || l >= npts) continue;                          // refused when the window is packed
+            for (const int c : {pb->obs_cam[i], pb->lm_anchor_cam[l]})
+                if (c >= 0 && c < ncam && !pb->pose_const[c] && !seen[c]) { seen[c] = 1; ++nused; }
+        }
+        ncv = nused;
+    }
     if (ncv > MAX_VAR_CAMS) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve: more than 64 optimised keyframes");
     if (world > 1 && ncam > MAX_CAMS) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_localba_solve_p2p: more than 256 keyframes in a multi-GPU window");
     H.ncv_max = ncv; H.n_max = 6 * ncv;
@@ -1674,7 +1690,8 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     const char* ssm = getenv("OV2_BA_SCHUR_SMEM");
     if (H.n_max > 0 && s + schur + (size_t)WARPS * H.blk * sizeof(double) <= 190 * 1024 && !(ssm && atoi(ssm) == 0) &&
                (single_window || (ssm && atoi(ssm) == 2))) {
-        // mode 2 (default for a single window when it fits: reduced systems up to n = 54): one private block per warp, one
+        // mode 2 (default for a single window when it fits: reduced systems up to n = 48 with at most 195 keyframes in the
+        // window's keyframe table): one private block per warp, one
         // CTA per SM.  Batches keep the RED path: there two CTAs per SM (different windows overlapping their latency-bound
         // phases) are worth more than the faster accumulation - measured 5.1 k vs 4.1 k solves/s on the C3 batch.
         H.schur_smem = 2;
@@ -2001,8 +2018,8 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         cudaMemcpy(tr, dwork + plans[0].w_trace, sizeof(tr), cudaMemcpyDeviceToHost);
         static const char* names[16] = {"setup0", "A:eval", "B:schur", "B2:fold", "C:solve", "C:wait", "D:backsub", "E:ctl", "scan", "wb", "setup1", "bar0",
                                         "chol:P1", "chol:bar", "chol:P2", "chol:back|ownerB1"};
-        fprintf(stderr, "[ba trace] G=%d grid=%d smem=%zu smemS=%d camtab=%s |", G, grid, smem_max, plans[0].schur_smem,
-                plans[0].cam_tab_global ? "global" : "shared");
+        fprintf(stderr, "[ba trace] G=%d grid=%d smem=%zu smemS=%d camtab=%s blocked=%d sg=%d |", G, grid, smem_max,
+                plans[0].schur_smem, plans[0].cam_tab_global ? "global" : "shared", plans[0].solve_blocked, plans[0].sg);
         for (int k = 0; k < 16; ++k) fprintf(stderr, " %s %.1fus", names[k], tr[k] / 1e3);
         fprintf(stderr, "\n");
     }

@@ -172,11 +172,20 @@ def test_unused_and_constant_blocks_drop_out():
     assert res["final_cost"] <= res["summaries"][0]["initial_cost"]
 
 
-@pytest.mark.parametrize("seed,ncam,npts,nobs", [(3, 10, 2000, 8000), (11, 6, 300, 1200), (5, 6, 100, 300)])
-def test_c_port_matches_numpy_oracle(seed, ncam, npts, nobs):
-    """oracle/ba_ref_c.c (the single-threaded CPU baseline bench.py times) == oracle/ba_ref.py."""
+def _c_port_window(name):
+    if name in ("unused_keyframes", "keyframe_leaves_refinement", "landmarks_without_residuals"):
+        import ba_windows
+        return ba_windows.small_shrinking_windows()[name]
+    return synth.make_ba_problem(*[int(v) for v in name.split("-")])
+
+
+@pytest.mark.parametrize("window", ["3-10-2000-8000", "11-6-300-1200", "5-6-100-300",
+                                    "unused_keyframes", "keyframe_leaves_refinement", "landmarks_without_residuals"])
+def test_c_port_matches_numpy_oracle(window):
+    """oracle/ba_ref_c.c (the single-threaded CPU baseline bench.py times) == oracle/ba_ref.py, also on windows whose
+    program is smaller than the declared one (tests/ba_windows.py; the C restatement is mono only)."""
     from oracle import ba_ref_c
-    pb = synth.make_ba_problem(seed, ncam, npts, nobs)
+    pb = _c_port_window(window)
     a = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in pb.items()}
     b = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in pb.items()}
     ra = B.local_ba(a)

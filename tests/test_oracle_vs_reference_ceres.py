@@ -167,6 +167,28 @@ def test_bal_structure_window_equals_real_ceres(lib):
     assert res["n_outliers_first"] > 0
 
 
+@pytest.mark.parametrize("case", ["unused_keyframes", "keyframe_leaves_refinement", "type2_only_keyframe", "landmarks_without_residuals"])
+def test_shrinking_program_equals_real_ceres(lib, case):
+    """Windows whose Ceres program is smaller than the declared one (tests/ba_windows.py): non-constant keyframes no residual
+    touches, a keyframe whose residuals the first scan removes (the refinement has one pose block fewer), a stereo keyframe
+    touched only by anchor-frame right-camera residuals, landmarks without a residual.  The restatement's RemoveFixedBlocks
+    model must match Ceres' own program reduction, and the blocks outside the program keep their values."""
+    import ba_windows as W
+    pb = W.small_shrinking_windows()[case]
+    res, _ = check(lib, f"shrink_{case}", pb)
+    o = W.clone(pb)
+    B.local_ba(o)
+    if case == "unused_keyframes":
+        assert W.used_keyframes(pb).sum() == 4 and np.array_equal(o["pose"][-2:], pb["pose"][-2:])
+    elif case == "keyframe_leaves_refinement":
+        assert W.used_keyframes(pb)[5] and not W.used_keyframes(pb, (res["flags"] & 1) == 0)[5] and res["iters_refine"] > 0
+    elif case == "type2_only_keyframe":
+        assert not W.used_keyframes(pb)[2] and (pb["lm_anchor_cam"] == 2).any() and np.array_equal(o["pose"][2], pb["pose"][2])
+    else:
+        lone = np.setdiff1d(np.arange(len(pb["lm_invdepth"])), pb["obs_lm"])
+        assert len(pb["obs_cam"]) < len(pb["lm_invdepth"]) and np.array_equal(o["lm_invdepth"][lone], pb["lm_invdepth"][lone])
+
+
 @pytest.mark.parametrize("seed,npts,noise,nout", [(1, 300, 0.5, 30), (2, 120, 1.0, 0), (3, 700, 0.3, 100), (4, 40, 0.5, 8)])
 def test_ceres_pnp_equals_real_ceres(lib, seed, npts, noise, nout):
     """oracle/pnp_ref.py::ceres_pnp against MultiViewGeometry::ceresPnP's Ceres calls (multi_view_geometry.cpp:492-588: one pose block,
