@@ -18,8 +18,12 @@ arrays ov2_match_to_map takes (the map walking that produces them is the host sh
   per keypoint               the candidate with the smallest distance, later candidates win ties (:758-772)
 
 The reference iterates an unordered_set of map-point ids; the order of `cand_mp` is used here (and by the kernel).
-Rotations are applied as 3 x 3 matrices (the reference goes through Sophus' quaternion product: last-bit differences in
-the camera-frame point).
+Every double is formed in the kernel's operation order (csrc/match_map.cu, built with -fmad=false): each row of the
+camera-frame point is the left-to-right sum T0*w0 + T1*w1 + T2*w2 + T9 of Python doubles (IEEE, no contraction), the
+norm is sqrt(X*X + Y*Y + Z*Z) left to right, and float steps round through numpy float32.  Division and sqrt are correctly
+rounded on both sides, so the oracle reproduces the kernel bit for bit: every output is compared for equality, and a
+test can put a value exactly on a threshold.  The reference goes through Sophus' quaternion product instead: last-bit
+differences in the camera-frame point against it.
 
 PINNING STATUS: the distortion model is pinned against cv2; the flow against the reference's own Mapper::matchToMap (src/mapper.cpp
 compiled in place with the reference's Frame / MapManager / MapPoint, oracle/ref_build/build_map_ref.py) on maps built from flattened
@@ -62,32 +66,70 @@ def _norm2(dx, dy):
     return math.sqrt(float(dx) * float(dx) + float(dy) * float(dy))
 
 
-def _hamming(a, b):
-    return int(np.unpackbits(np.bitwise_xor(a, b)).sum())
+def camera_point(T, w):
+    """transform() of match_map.cu: T = (row-major R, t) as 12 doubles, each row summed left to right."""
+    T = [float(v) for v in T]
+    w0, w1, w2 = float(w[0]), float(w[1]), float(w[2])
+    return (T[0] * w0 + T[1] * w1 + T[2] * w2 + T[9],
+            T[3] * w0 + T[4] * w1 + T[5] * w2 + T[10],
+            T[6] * w0 + T[7] * w1 + T[8] * w2 + T[11])
+
+
+def view_angle(X, Y, Z):
+    """z / |p| of the camera-frame point, rounded to float (mapper.cpp:634)."""
+    return f32(Z / math.sqrt(X * X + Y * Y + Z * Z))
+
+
+def pixel_distance(px, py, kx, ky):
+    """Distance of the projection to a keypoint: float components, norm in double, rounded to float (mapper.cpp:667)."""
+    return f32(_norm2(f32(f32(px) - f32(kx)), f32(f32(py) - f32(ky))))
+
+
+def coprojection(sc, wpt, lm):
+    """(mean co-projection error as a float, nb): the map point `wpt` projected into every keyframe observing map point `lm`,
+    float accumulation of the double norms (mapper.cpp:698-716).  The mean is None when no keyframe observes `lm`."""
+    kf_T = np.asarray(sc["kf_Tcw"], np.float64).reshape(-1, 12)
+    coproj, nb = f32(0.0), 0
+    for o in range(int(sc["mp_obs_ptr"][lm]), int(sc["mp_obs_ptr"][lm + 1])):
+        qx, qy = project_dist(camera_point(kf_T[int(sc["obs_kf"][o])], wpt), sc["K"], sc.get("dist"))
+        ox, oy = sc["obs_px"][o]
+        coproj = f32(float(coproj) + _norm2(f32(ox - qx), f32(oy - qy)))
+        nb += 1
+    return (f32(coproj / f32(nb)) if nb else None), nb
+
+
+def min_dist(fdistratio):
+    """The starting best / second distance: desc_.cols * fdistratio * 8. with a 32-byte descriptor (mapper.cpp:650)."""
+    return f32(float(f32(32 * f32(fdistratio))) * 8.0)
+
+
+def _desc_ints(desc):
+    return [int.from_bytes(bytes(row), "little") for row in np.asarray(desc, np.uint8).reshape(-1, 32)]
 
 
 def match_to_map(sc: dict):
     """Returns (best_kp int32[ncand], best_dist float32[ncand], kp_match int32[nkps], kp_dist float32[nkps])."""
     K, dist = sc["K"], sc.get("dist")
-    R, t = np.asarray(sc["Tcw"][:9], np.float64).reshape(3, 3), np.asarray(sc["Tcw"][9:], np.float64)
+    Tcw = np.asarray(sc["Tcw"], np.float64).reshape(-1)
     cs, nbw = int(sc["ncellsize"]), int(sc["nbwcells"])
     ncells = len(sc["cell_ptr"]) - 1
     w, h = int(sc["img_w"]), int(sc["img_h"])
-    dmax, ratio, view_th = f32(sc["dmaxpxdist"]), f32(sc["fdistratio"]), f32(sc["view_th"])
-    kf_T = np.asarray(sc["kf_Tcw"], np.float64).reshape(-1, 12)
+    dmax, view_th = f32(sc["dmaxpxdist"]), f32(sc["view_th"])
     ncand = len(sc["cand_mp"])
     best_kp = -np.ones(ncand, np.int32)
     best_dist = np.zeros(ncand, np.float32)
-    mindist = f32(float(f32(32 * ratio)) * 8.0)
-    for ci, mp in enumerate(sc["cand_mp"]):
-        wpt = np.asarray(sc["mp_xyz"][mp], np.float64)
-        campt = R @ wpt + t
-        if campt[2] < 0.1:
+    mindist = min_dist(sc["fdistratio"])
+    desc = _desc_ints(sc["desc"])
+    desc_ptr = [int(v) for v in sc["mp_desc_ptr"]]
+    kfmask = [tuple(int(v) for v in row) for row in np.asarray(sc["mp_kfmask"], np.uint64).reshape(-1, 4)]
+    for ci, mp in enumerate(int(v) for v in sc["cand_mp"]):
+        wpt = sc["mp_xyz"][mp]
+        X, Y, Z = camera_point(Tcw, wpt)
+        if Z < 0.1:
             continue
-        view_angle = f32(campt[2] / math.sqrt(float(campt @ campt)))
-        if abs(view_angle) < view_th:
+        if abs(view_angle(X, Y, Z)) < view_th:
             continue
-        px, py = project_dist(campt, K, dist)
+        px, py = project_dist((X, Y, Z), K, dist)
         if not (px >= 0 and py >= 0 and px < w and py < h):
             continue
         rkp, ckp = int(math.floor(float(f32(py / f32(cs))))), int(math.floor(float(f32(px / f32(cs)))))
@@ -103,30 +145,21 @@ def match_to_map(sc: dict):
                     if lm < 0:
                         continue
                     kx, ky = sc["kp_px"][j]
-                    pxdist = f32(_norm2(f32(px - kx), f32(py - ky)))
-                    if pxdist > dmax:
+                    if pixel_distance(px, py, kx, ky) > dmax:
                         continue
-                    d0, d1 = sc["mp_desc_ptr"][lm], sc["mp_desc_ptr"][lm + 1]
+                    d0, d1 = desc_ptr[lm], desc_ptr[lm + 1]
                     if d1 == d0:
                         continue
-                    if np.any(np.bitwise_and(sc["mp_kfmask"][mp], sc["mp_kfmask"][lm])):
+                    if any(a & b for a, b in zip(kfmask[mp], kfmask[lm])):
                         continue
-                    coproj, nb = f32(0.0), 0
-                    for o in range(sc["mp_obs_ptr"][lm], sc["mp_obs_ptr"][lm + 1]):
-                        T = kf_T[sc["obs_kf"][o]]
-                        cpt = T[:9].reshape(3, 3) @ wpt + T[9:]
-                        qx, qy = project_dist(cpt, K, dist)
-                        ox, oy = sc["obs_px"][o]
-                        coproj = f32(float(coproj) + _norm2(f32(ox - qx), f32(oy - qy)))
-                        nb += 1
-                    if nb > 0 and f32(coproj / f32(nb)) > dmax:
+                    mean, nb = coprojection(sc, wpt, lm)
+                    if nb > 0 and mean > dmax:
                         continue
-                    dd = f32(1000.0)
-                    for a in sc["desc"][sc["mp_desc_ptr"][mp]:sc["mp_desc_ptr"][mp + 1]]:
-                        for b in sc["desc"][d0:d1]:
-                            v = f32(_hamming(a, b))
-                            if v < dd:
-                                dd = v
+                    dd = 1000
+                    for a in desc[desc_ptr[mp]:desc_ptr[mp + 1]]:
+                        for b in desc[d0:d1]:
+                            dd = min(dd, (a ^ b).bit_count())
+                    dd = f32(dd)
                     if dd <= bestdist:
                         secdist, secid = bestdist, bestid
                         bestdist, bestid = dd, int(j)

@@ -301,21 +301,50 @@ def test_mapper_match_shim_flattens_the_map_like_the_scene(tmp_path, distorted):
     assert len(want ^ got) <= max(1, len(want) // 100)
 
 
-@pytest.mark.gpu
-def test_mapper_match_shim_matches_python_binding(ctx, tmp_path):
-    """The same drop-in end to end on the GPU: the (keypoint id -> map-point id) map it returns equals ov2_match_to_map on the scene
-    the map was built from, candidates in the order the shim walked the id set."""
+def _shim_against_the_oracle(tmp_path, sc):
+    """Runs the drop-in twice on the map built from `sc`: once with the recorder to capture the flat problem it hands to
+    ov2_match_to_map, once on the GPU.  Returns the (keypoint lmid, map-point lmid) pairs it returned, the pairs the oracle
+    gives on the recorded problem (named through the recorded map-point table), and the recorded problem."""
+    from oracle import match_ref as M
     exe = build.build_mapper_shim()
-    sc = synth.make_match_scene(9, nkps=1200, ncand=700, nkfs=12, distorted=True)
+    rec = tmp_path / "librec.so"
+    subprocess.check_call(["gcc", "-shared", "-fPIC", "-O1", "-o", str(rec), str(ROOT / "tests" / "helpers" / "match_dump.c")])
     _write_match_scene(tmp_path / "s.bin", sc)
+    env = dict(os.environ, LD_PRELOAD=str(rec), OV2_MATCH_DUMP=str(tmp_path / "d.bin"))
+    out = subprocess.run([str(exe), str(tmp_path / "s.bin"), str(tmp_path / "rd.bin")], capture_output=True, text=True, timeout=120, env=env)
+    assert out.returncode == 0, out.stdout + out.stderr
     out = subprocess.run([str(exe), str(tmp_path / "s.bin"), str(tmp_path / "r.bin")], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
-    order, pairs, _ = _read_match_result(tmp_path / "r.bin")
-    ref = dict(sc, cand_mp=np.asarray(order, np.int32))
-    _, _, kp_match, _ = api.match_to_map(ctx, ref)
-    want = {(int(sc["kp_lm"][j]), int(order[c])) for j, c in enumerate(kp_match) if c >= 0}
+    _, pairs, _ = _read_match_result(tmp_path / "r.bin")
+    dump = _read_match_dump(tmp_path / "d.bin")
+    # the self-test gives map point m the id m, and the shim copies each map point's position as it is: name the recorded
+    # map-point table by position
+    lmid_of_xyz = {row.tobytes(): m for m, row in enumerate(np.asarray(sc["mp_xyz"], np.float64))}
+    assert len(lmid_of_xyz) == len(sc["mp_xyz"])
+    lmid = [lmid_of_xyz[row.tobytes()] for row in dump["mp_xyz"]]
+    _, _, kp_match, _ = M.match_to_map(dump)
+    want = {(lmid[dump["kp_lm"][j]], lmid[dump["cand_mp"][c]]) for j, c in enumerate(kp_match) if c >= 0}
+    return pairs, want, dump
+
+
+@pytest.mark.gpu
+def test_mapper_match_shim_matches_python_binding(ctx, tmp_path):
+    """The same drop-in end to end on the GPU: the (keypoint id -> map-point id) map it returns equals the oracle on the flat
+    problem it hands over (recorded in a first run of the same binary, which walks the same id set the same way)."""
+    sc = synth.make_match_scene(9, nkps=1200, ncand=700, nkfs=12, distorted=True)
+    pairs, want, _ = _shim_against_the_oracle(tmp_path, sc)
     assert len(want) > 100
-    assert len(want ^ pairs) <= max(1, len(want) // 100)
+    assert pairs == want
+
+
+@pytest.mark.gpu
+def test_mapper_match_shim_with_150_keyframes(ctx, tmp_path):
+    """A map of 150 keyframes: the shim's own keyframe numbering fills words 0-2 of the observation masks."""
+    sc = synth.make_match_scene(10, nkps=1200, ncand=700, nkfs=150, distorted=True)
+    pairs, want, dump = _shim_against_the_oracle(tmp_path, sc)
+    assert len(dump["kf_Tcw"]) == 150 and np.all(dump["mp_kfmask"][:, :3].any(axis=0)) and not dump["mp_kfmask"][:, 3].any()
+    assert len(want) > 100
+    assert pairs == want
 
 
 # ---------------------------------------------------------------------------------------------- MapManager::stereoMatching drop-in
