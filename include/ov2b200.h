@@ -214,6 +214,12 @@ OV2_API int ov2_fast_cell_capacity(int cellsize);
 OV2_API ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int frame, int cellsize, int fast_th,
                                 uint32_t* cand_out, int32_t* cand_n_out, int cap_in, int* cap_out);
 
+/* Measurement hook: cornerSubPix alone on count * max_per_frame integer points (x < 0: empty slot) of frames
+ * [first, first + count), as ov2_grid_fast runs it.  out_pts: the refined points; iters_out: iterations run per slot
+ * (1 .. 30; -1 for an empty slot).  Host or device pointers. */
+OV2_API ov2_status ov2_debug_subpix_iters(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame,
+                                  const int32_t* pts_int, float* out_pts, int32_t* iters_out);
+
 /* ------------------------------------------------------------------ ceresPnP (motion-only BA), "next" row 2
  * Replaces MultiViewGeometry::ceresPnP(vunkps, vwpts, vscales, Twc, nmaxiter, chi2th, buse_robust,
  * bapply_l2_after_robust, fx, fy, cx, cy, voutliersidx)

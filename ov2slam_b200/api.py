@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -134,6 +134,7 @@ def load():
     lib.ov2_fast_cell_capacity.argtypes = [i32]
     lib.ov2_fast_cell_capacity.restype = i32
     lib.ov2_debug_fast_cells.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, C.POINTER(i32)]
+    lib.ov2_debug_subpix_iters.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp]
     lib.ov2_describe.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp]
     lib.ov2_describe_config.argtypes = [vp, i32, vp]
     lib.ov2_line_min_sad.argtypes = [vp, vp, vp, i32, i32, vp, i32, i32, vp, i32, i32, vp, vp]
@@ -456,6 +457,11 @@ class FeatureExtractor:
         self.detect_grid_fast(pyr, ncellsize, frame, 1, th, pts, cnt, off, cur if len(cur) else None, ipts)
         self.nfast_th_ = int(th[0])
         return pts[:cnt[0]].copy(), ipts[:cnt[0]].copy()
+
+    def debug_subpix_iters(self, pyr: Pyramid, first: int, count: int, max_per_frame: int, pts_int, out_pts, iters_out):
+        """cornerSubPix alone on integer points (int32 (n, 2), x < 0: empty slot): refined points and iterations per slot."""
+        self.ctx.check(self.ctx.lib.ov2_debug_subpix_iters(self.ctx.h, pyr.h_, first, count, int(max_per_frame),
+                                                           _ptr(pts_int), _ptr(out_pts), _ptr(iters_out)))
 
     def debug_fast_cells(self, pyr: Pyramid, frame: int, ncellsize: int, fast_th: int):
         """Stage F1 only: list per cell of (x, y, response) candidates (cell-local, scan order).  The per-cell capacity

@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
             // unique maximum, or libstdc++ falls straight to (stable) insertion sort
             win_j = skey[firstmax] & SKEY_IDX;
         } else {
-            if (lane == 0) ov2sort::sort_desc(skey, ns);
+            if (lane == 0) ov2sort::sort_desc_front(skey, ns);     // only skey[0] is read
             __syncwarp();
             win_j = skey[0] & SKEY_IDX;
         }
@@ -429,8 +429,8 @@ __global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
 // Wavefront variant: the sequential cell order is the semantics, but a cell only reads mask bits of its own area, and a disc
 // (radius cs / 4) reaches no further than the neighbouring cells - so cell (r, c) needs (r, c-1), (r-1, c-1), (r-1, c) and
 // (r-1, c+1) finished, nothing else.  One warp per cell row, row r trailing row r-1 by two cells (as ss_sweep_kernel does):
-// exactly the sequential result in nwc + 2 nhc cell times instead of nwc * nhc (one warp per frame was 10 % of the C2 step,
-// pure latency).  Detections are kept per cell and put in cell order at the end.
+// exactly the sequential result in nwc + 2 nhc cell times instead of nwc * nhc (pure latency; 0.070 ms, 3.5 % of the C2 step,
+// on an H100 SXM at 700 W).  Detections are kept per cell and put in cell order at the end.
 constexpr int FSWEEP_MAX_WARPS = 16;
 
 __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kernel(SweepArgs A) {
@@ -472,22 +472,35 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
     __syncthreads();
     const uint32_t* cand = A.cand + (size_t)fr * ncells * A.cap;
     const int32_t* cand_n = A.cand_n + (size_t)fr * ncells;
+    // A cell's candidates do not depend on any other cell, and the row's cell-to-cell chain is what the frame waits for: the
+    // count and the first WAVE_REG_CAND candidates of cell c + 2 are requested (five independent loads; the list's slots past
+    // the count are allocated, and dropped below) before cell c is worked on, so no global-memory latency is left in the chain.
+    struct CellFetch { int n; uint32_t v[4]; };
+    auto fetch = [&](int r, int c) {
+        CellFetch f = {0, {0u, 0u, 0u, 0u}};
+        if (c < A.nwc) {
+            const int cell = r * A.nwc + c;
+            f.n = __ldg(cand_n + cell);
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+                if (32 * q + lane < A.cap) f.v[q] = __ldg(cand + (size_t)cell * A.cap + 32 * q + lane);
+        }
+        return f;
+    };
     for (int r = warp; r < A.nhc; r += nwarps) {
+        CellFetch f0 = fetch(r, 0), f1 = fetch(r, 1);
         for (int c = 0; c < A.nwc; ++c) {
+            const CellFetch cur = f0;
+            f0 = f1;
+            f1 = fetch(r, c + 2);
             const int cell = r * A.nwc + c;
             const int x0 = c * A.cs, y0 = r * A.cs;
             const bool search = !occ[r * (A.nwc + 1) + c] && (x0 + A.cs < A.w - 1 && y0 + A.cs < A.h - 1);
-            // the cell's candidates do not depend on any other cell: fetch them before waiting for the neighbours
-            const int n = search ? cand_n[cell] : 0;
+            const int n = search ? cur.n : 0;
             const uint32_t* ccand = cand + (size_t)cell * A.cap;
-            uint32_t cdv[4] = {0u, 0u, 0u, 0u};                                // the first WAVE_REG_CAND: four per lane
-            if (n > 0) {
+            uint32_t cdv[4];                                                   // the first WAVE_REG_CAND: four per lane
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int j = 32 * q + lane;
-                    if (j < n) cdv[q] = __ldg(ccand + j);
-                }
-            }
+            for (int q = 0; q < 4; ++q) cdv[q] = 32 * q + lane < n ? cur.v[q] : 0u;
             if (r > 0) {
                 const int need = min(c + 2, A.nwc);                            // row r-1 has finished cell c+1 (or its last cell)
                 while (progress[r - 1] < need) __nanosleep(40);
@@ -537,7 +550,7 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
                     if (nmax == 1 || ns <= 16) {
                         win_j = skey[firstmax] & SKEY_IDX;                     // unique maximum / libstdc++'s insertion-sort range
                     } else {
-                        if (lane == 0) ov2sort::sort_desc(skey, ns);
+                        if (lane == 0) ov2sort::sort_desc_front(skey, ns);     // only skey[0] is read
                         __syncwarp();
                         win_j = skey[0] & SKEY_IDX;
                     }
@@ -606,13 +619,8 @@ struct SubpixArgs {
     float2* out;
     int do_subpix;
     float mask[49];                // exp(-(i/3)^2) * exp(-(j/3)^2), computed on the host with libm expf
+    int32_t* iters;                // COUNT instantiation only: iterations run per slot (-1: empty slot)
 };
-
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    return v;
-}
 
 // cv::getRectSubPix(8u -> 32f, 9x9) value at patch (i, j); grouping found by probing cv2 4.13
 // (oracle/image_ref.py::_get_rect_subpix_9).
@@ -642,7 +650,13 @@ __device__ __forceinline__ float rect_subpix_px(const uint8_t* img, int pitch, i
     return ((float)s0[cc] * a11 + (float)s0[cc + 1] * a12) + ((float)s1[cc] * a21 + (float)s1[cc + 1] * a22);
 }
 
+// One warp per point.  The 9 x 9 getRectSubPix patch only needs the 10 x 10 pixels at the centre's integer origin (ix, iy),
+// and successive iterations move the centre by a fraction of a pixel: the pixels are staged in shared memory (as floats)
+// when the origin changes and re-interpolated from there otherwise.  Every lane keeps fixed patch and gradient
+// positions, so no division is left in the loop.  Expressions and summation order are those of cv::cornerSubPix.
+template <bool COUNT>
 __global__ void __launch_bounds__(128) subpix_kernel(SubpixArgs A) {
+    __shared__ float sraw[4][100];
     __shared__ float spatch[4][81];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int idx = blockIdx.x * 4 + warp;
@@ -650,42 +664,95 @@ __global__ void __launch_bounds__(128) subpix_kernel(SubpixArgs A) {
     const int2 ip = A.in_int[idx];
     if (ip.x < 0) {
         if (lane == 0) A.out[idx] = make_float2(-1.f, -1.f);
+        if (COUNT && lane == 0) A.iters[idx] = -1;
         return;
     }
     const float2 cT = make_float2((float)ip.x, (float)ip.y);
     if (!A.do_subpix) {
         if (lane == 0) A.out[idx] = cT;
+        if (COUNT && lane == 0) A.iters[idx] = 0;
         return;
     }
     const int fr = idx / A.max_per_frame;
     const uint8_t* img = A.img + A.fstride * (A.first + fr);
     float* sp = spatch[warp];
+    float* raw = sraw[warp];
+    // patch pixels lane, lane + 32, lane + 64 (the last for lanes 0..16): position in the 10-wide staged block
+    const int r0 = lane + lane / 9, r1 = lane + 32 + (lane + 32) / 9, r2 = lane + 64 + (lane + 64) / 9;   // p + p / 9
+    const bool has2 = lane + 64 < 81;
+    // gradient pixels lane and lane + 32 (the second for lanes 0..16)
+    const int gi0 = lane / 7, gj0 = lane % 7;
+    const int gi1 = (lane + 32) / 7, gj1 = (lane + 32) % 7;
+    const bool hasg1 = lane + 32 < 49;
+    const float* q0 = sp + (gi0 + 1) * 9 + (gj0 + 1);
+    const float* q1 = sp + (hasg1 ? (gi1 + 1) * 9 + (gj1 + 1) : 10);
+    const float mf0 = A.mask[lane], mf1 = hasg1 ? A.mask[lane + 32] : 0.f;
+    const float pxf0 = (float)(gj0 - 3), pyf0 = (float)(gi0 - 3), pxf1 = (float)(gj1 - 3), pyf1 = (float)(gi1 - 3);
     float2 cI = cT;
     const double eps = 0.01 * 0.01;
-    int iter = 0;
+    int iter = 0, nrun = 0;
+    int sx = -1, sy = -1;                                       // origin of the staged block (never negative)
     double err = 0.0;
     do {
+        ++nrun;
         const float x = cI.x - 4.f, y = cI.y - 4.f;
         const int ix = __float2int_rd(x), iy = __float2int_rd(y);
         const float a = x - (float)ix, b = y - (float)iy;
         __syncwarp();
-        for (int p = lane; p < 81; p += 32) sp[p] = rect_subpix_px(img, A.pitch, A.w, A.h, ix, iy, a, b, p / 9, p % 9);
+        if (0 <= ix && ix + 9 < A.w && 0 <= iy && iy + 9 < A.h) {
+            if (ix != sx || iy != sy) {
+                const uint8_t* p = img + (size_t)iy * A.pitch + ix;
+                for (int e = lane; e < 100; e += 32) {
+                    const int rr = e / 10;
+                    raw[e] = (float)p[(size_t)rr * A.pitch + (e - rr * 10)];
+                }
+                sx = ix; sy = iy;
+                __syncwarp();
+            }
+            const float a11 = (1.f - a) * (1.f - b), a12 = a * (1.f - b), a21 = (1.f - a) * b, a22 = a * b;
+            sp[lane] = (raw[r0] * a11 + raw[r0 + 1] * a12) + (raw[r0 + 10] * a21 + raw[r0 + 11] * a22);
+            sp[lane + 32] = (raw[r1] * a11 + raw[r1 + 1] * a12) + (raw[r1 + 10] * a21 + raw[r1 + 11] * a22);
+            if (has2) sp[lane + 64] = (raw[r2] * a11 + raw[r2 + 1] * a12) + (raw[r2 + 10] * a21 + raw[r2 + 11] * a22);
+        } else {
+            // within 4 px of a border: getRectSubPix's border rules, pixel by pixel
+            for (int p = lane; p < 81; p += 32) sp[p] = rect_subpix_px(img, A.pitch, A.w, A.h, ix, iy, a, b, p / 9, p % 9);
+        }
         __syncwarp();
         double sa = 0, sb = 0, scc = 0, sbb1 = 0, sbb2 = 0;
-        for (int p = lane; p < 49; p += 32) {
-            int i = p / 7, j = p - i * 7;
-            const float* q = sp + (i + 1) * 9 + (j + 1);
-            double m = (double)A.mask[p];
-            double tgx = (double)(q[1] - q[-1]);
-            double tgy = (double)(q[9] - q[-9]);
-            double gxx = tgx * tgx * m, gxy = tgx * tgy * m, gyy = tgy * tgy * m;
-            double px = (double)(j - 3), py = (double)(i - 3);
+        {
+            const double m0 = (double)mf0, px0 = (double)pxf0, py0 = (double)pyf0;
+            const double tgx = (double)(q0[1] - q0[-1]);
+            const double tgy = (double)(q0[9] - q0[-9]);
+            const double gxx = tgx * tgx * m0, gxy = tgx * tgy * m0, gyy = tgy * tgy * m0;
             sa += gxx; sb += gxy; scc += gyy;
-            sbb1 += gxx * px + gxy * py;
-            sbb2 += gxy * px + gyy * py;
+            sbb1 += gxx * px0 + gxy * py0;
+            sbb2 += gxy * px0 + gyy * py0;
         }
-        sa = warp_sum_d(sa); sb = warp_sum_d(sb); scc = warp_sum_d(scc);
-        sbb1 = warp_sum_d(sbb1); sbb2 = warp_sum_d(sbb2);
+        if (hasg1) {
+            const double m1 = (double)mf1, px1 = (double)pxf1, py1 = (double)pyf1;
+            const double tgx = (double)(q1[1] - q1[-1]);
+            const double tgy = (double)(q1[9] - q1[-9]);
+            const double gxx = tgx * tgx * m1, gxy = tgx * tgy * m1, gyy = tgy * tgy * m1;
+            sa += gxx; sb += gxy; scc += gyy;
+            sbb1 += gxx * px1 + gxy * py1;
+            sbb2 += gxy * px1 + gyy * py1;
+        }
+        // The five warp sums, each the xor butterfly's tree ((x[i] + x[i ^ 16]) + ...: order 16, 8, 4, 2, 1), with the sums
+        // spread over the lanes instead of repeated in all of them: at 16 the lower half-warp goes on with sa and scc, the
+        // upper with sb and sbb1; at 8 lanes with bit 3 clear keep the first of their two, the others the second; at 4 lanes
+        // with bit 2 set take over sbb2.  A lane adds the same two partial sums the butterfly adds there (a + b = b + a), so
+        // every sum has the butterfly's bits with 8 shuffles in place of 25; lanes 0, 16, 8, 24 and 4 hold the results.
+        const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
+        double u = (h16 ? sb : sa) + __shfl_xor_sync(FULL, h16 ? sa : sb, 16);        // sa | sb
+        double v = (h16 ? sbb1 : scc) + __shfl_xor_sync(FULL, h16 ? scc : sbb1, 16);  // scc | sbb1
+        sbb2 += __shfl_xor_sync(FULL, sbb2, 16);
+        u = (h8 ? v : u) + __shfl_xor_sync(FULL, h8 ? u : v, 8);                      // sa | sb | scc | sbb1 by bits 4, 3
+        sbb2 += __shfl_xor_sync(FULL, sbb2, 8);
+        u = (h4 ? sbb2 : u) + __shfl_xor_sync(FULL, h4 ? u : sbb2, 4);
+        u += __shfl_xor_sync(FULL, u, 2);
+        u += __shfl_xor_sync(FULL, u, 1);
+        sa = __shfl_sync(FULL, u, 0); sb = __shfl_sync(FULL, u, 16); scc = __shfl_sync(FULL, u, 8);
+        sbb1 = __shfl_sync(FULL, u, 24); sbb2 = __shfl_sync(FULL, u, 4);
         const double det = sa * scc - sb * sb;
         if (fabs(det) <= 2.220446049250313e-16 * 2.220446049250313e-16) break;
         const double scale = 1.0 / det;
@@ -699,6 +766,19 @@ __global__ void __launch_bounds__(128) subpix_kernel(SubpixArgs A) {
     } while (++iter < 30 && err > eps);
     if (fabsf(cI.x - cT.x) > 3.f || fabsf(cI.y - cT.y) > 3.f) cI = cT;
     if (lane == 0) A.out[idx] = cI;
+    if (COUNT && lane == 0) A.iters[idx] = nrun;
+}
+
+// cornerSubPix's 7 x 7 weights, exactly as OpenCV forms them
+void subpix_mask(float* mask) {
+    for (int i = 0; i < 7; ++i) {
+        float y = (float)(i - 3) / 3;
+        float vy = expf(-y * y);
+        for (int j = 0; j < 7; ++j) {
+            float x = (float)(j - 3) / 3;
+            mask[i * 7 + j] = (float)(vy * expf(-x * x));
+        }
+    }
 }
 
 // OpenCV's filled-circle rasterisation (midpoint algorithm): half-width per |dy|
@@ -883,15 +963,9 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     PA.img = pyr->l0; PA.w = W; PA.h = H; PA.pitch = (int)pyr->l0_pitch; PA.fstride = (long long)pyr->l0_fstride;
     PA.first = first; PA.max_per_frame = max_per_frame; PA.n = count * max_per_frame;
     PA.in_int = d_int; PA.out = d_out; PA.do_subpix = do_subpix;
-    for (int i = 0; i < 7; ++i) {
-        float y = (float)(i - 3) / 3;
-        float vy = expf(-y * y);
-        for (int j = 0; j < 7; ++j) {
-            float x = (float)(j - 3) / 3;
-            PA.mask[i * 7 + j] = (float)(vy * expf(-x * x));
-        }
-    }
-    OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
+    PA.iters = nullptr;
+    subpix_mask(PA.mask);
+    OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<false><<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
     return ov2_end(ctx);
 }
 
@@ -932,19 +1006,38 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
 // Internal (not part of the C ABI): cornerSubPix stage S on integer points produced by another detector
 // (frontend_sscale.cu).  Same launch as inside ov2_grid_fast; slots holding (-1, -1) stay empty.
 ov2_status ov2_subpix_launch(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame, const int2* d_int,
-                             float2* d_out, int do_subpix) {
+                             float2* d_out, int do_subpix, int32_t* d_iters) {
     SubpixArgs PA;
     PA.img = pyr->l0; PA.w = pyr->w[0]; PA.h = pyr->h[0]; PA.pitch = (int)pyr->l0_pitch; PA.fstride = (long long)pyr->l0_fstride;
     PA.first = first; PA.max_per_frame = max_per_frame; PA.n = count * max_per_frame;
     PA.in_int = d_int; PA.out = d_out; PA.do_subpix = do_subpix;
-    for (int i = 0; i < 7; ++i) {
-        float y = (float)(i - 3) / 3;
-        float vy = expf(-y * y);
-        for (int j = 0; j < 7; ++j) {
-            float x = (float)(j - 3) / 3;
-            PA.mask[i * 7 + j] = (float)(vy * expf(-x * x));
-        }
-    }
-    OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
+    PA.iters = d_iters;
+    subpix_mask(PA.mask);
+    if (d_iters)
+        OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<true><<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
+    else
+        OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<false><<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
     return OV2_OK;
+}
+
+// Measurement hook: cornerSubPix on `pts_int` (count * max_per_frame slots, x < 0: empty) as ov2_grid_fast runs it,
+// returning the number of iterations each point took.  A second instantiation of the kernel: the product launch
+// carries no counter.
+extern "C" ov2_status ov2_debug_subpix_iters(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame,
+                                             const int32_t* pts_int, float* out_pts, int32_t* iters_out) {
+    if (!ctx || !pyr || !pyr->l0 || first < 0 || count <= 0 || first + count > pyr->batch || max_per_frame <= 0 || !pts_int ||
+        !out_pts || !iters_out)
+        return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_debug_subpix_iters: bad arguments");
+    ov2_status st = ov2_begin(ctx);
+    if (st != OV2_OK) return st;
+    const size_t n = (size_t)count * max_per_frame;
+    const void* d = nullptr;
+    void* o = nullptr;
+    if ((st = ov2_stage_in(ctx, pts_int, sizeof(int32_t) * 2 * n, &d)) != OV2_OK) return st;
+    const int2* d_int = (const int2*)d;
+    if ((st = ov2_stage_out(ctx, out_pts, sizeof(float) * 2 * n, &o)) != OV2_OK) return st;
+    float2* d_out = (float2*)o;
+    if ((st = ov2_stage_out(ctx, iters_out, sizeof(int32_t) * n, &o)) != OV2_OK) return st;
+    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, 1, (int32_t*)o)) != OV2_OK) return st;
+    return ov2_end(ctx);
 }

@@ -19,7 +19,7 @@
 #include "sscale_math.cuh"
 
 ov2_status ov2_subpix_launch(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame, const int2* d_int,
-                             float2* d_out, int do_subpix);   // frontend_fast.cu
+                             float2* d_out, int do_subpix, int32_t* d_iters);   // frontend_fast.cu
 
 namespace {
 
@@ -400,6 +400,6 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
         const int nw = nhc < SWEEP_MAX_WARPS ? nhc : SWEEP_MAX_WARPS;       // one warp per cell row (wavefront)
         OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, sweep_smem, ctx->stream>>>(SA));
     }
-    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, do_subpix)) != OV2_OK) return st;
+    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, do_subpix, nullptr)) != OV2_OK) return st;
     return ov2_end(ctx);
 }

@@ -150,4 +150,24 @@ OV2_HD void sort_desc(int* v, int n) {
     }
 }
 
+// The element sort_desc(v, n) leaves at v[0], for a caller that reads nothing else (the reference reads only
+// vkps.at(0)).  __introsort_loop's recursion into (cut, last) never touches [first, cut), and every element right of a
+// cut has a response no larger than every element left of it, so the final insertion sort cannot move one of them in
+// front of the leftmost partition: only the leftmost chain of partitions has to be followed, n + n/2 + ... steps
+// instead of the whole sort.  v is left permuted but not sorted.
+OV2_HD int sort_desc_front(int* v, int n) {
+    if (n < 2) return v[0];
+    int lg = 0;
+    for (int t = n; t > 1; t >>= 1) ++lg;
+    int last = n, depth = 2 * lg;
+    while (last > 16) {
+        if (depth == 0) { heap_sort(v, 0, last); break; }
+        --depth;
+        move_median_to_first(v, 0, 1, last / 2, last - 1);
+        last = unguarded_partition(v, 1, last, 0);
+    }
+    insertion_sort(v, 0, last < 16 ? last : 16);
+    return v[0];
+}
+
 }  // namespace ov2sort
