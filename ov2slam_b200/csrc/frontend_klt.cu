@@ -16,13 +16,13 @@
 // the image edge, constant 0 outside the image - exactly the planes buildOpticalFlowPyramid
 // would have materialised), so the tracker reads only the 8-bit pyramid.
 #include <climits>
-#include <cstdio>
 #include "ov2_common.cuh"
 #include "klt_setup.cuh"
 
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
+constexpr int WARPS_PER_CTA = 8;   // one keypoint per warp
 
 struct KltArgs {
     PyrView prev, cur;
@@ -35,42 +35,11 @@ struct KltArgs {
     float2* priors;
     uint8_t* status;
     int max_iter;
-    float eps, ferr, fb_dist;
+    float ferr, fb_dist;
     double eps2;           // epsilon^2 as OpenCV forms it (double)
     float eps_lo, eps_hi;  // float brackets of eps2: outside them the float evaluation of |delta|^2 decides
     int* work_counter;   // persistent launch: warps pull keypoint indices from this counter (null: one warp per index)
-    // three-keypoints-per-warp kernel: keypoints it cannot take (border windows, unaligned levels, huge gradients) are
-    // appended here and tracked by the one-warp-per-keypoint kernel in a second launch
-    int* defer_list;
-    int* defer_count;
-    int from_list;       // 1: fb_klt_kernel takes its keypoint indices from defer_list[0 .. *defer_count)
-    // keypoints bucketed by pyramid depth (klt_bucket_kernel) so that the three keypoints of a warp walk the same number of
-    // levels: bucket[0 .. n) = depth <= 1, bucket[n .. 2n) = deeper; bucket_count[0], [1] = their sizes.  NULL: consecutive indices
-    const int* bucket;
-    const int* bucket_count;
 };
-
-__device__ __forceinline__ int reflect101_safe(int i, int n) {
-    if (n == 1) return 0;
-    while (i < 0 || i >= n) {
-        if (i < 0) i = -i;
-        if (i >= n) i = 2 * (n - 1) - i;
-    }
-    return i;
-}
-
-// dp2a with SIGNED 16-bit halves of a (bilinear weights: iw11 = 16384 - others can round to -1) and
-// UNSIGNED bytes of b (pixels): lo uses bytes 0,1 of b, hi bytes 2,3
-__device__ __forceinline__ int dp2a_lo_su(unsigned a, unsigned b, int c) {
-    int d;
-    asm("dp2a.lo.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ int dp2a_hi_su(unsigned a, unsigned b, int c) {
-    int d;
-    asm("dp2a.hi.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
 
 // exact 64-bit warp sum of per-lane int32 partials via two 32-bit redux ops
 __device__ __forceinline__ long long warp_sum64(int s) {
@@ -83,17 +52,14 @@ __device__ __forceinline__ long long warp_sum64(int s) {
 
 // One calcOpticalFlowPyrLK track for one point (whole warp cooperates).
 // Ipyr = template pyramid, Jpyr = search pyramid.  nxt: in = initial guess, out = result.
-template <int WIN>
 __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
                          int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sP, int* sD, int lane) {
-    constexpr int NPX = WIN * WIN;
-    constexpr int PER_LANE = (NPX + 31) / 32;
-    // window pixel owned by (lane, k).  WIN = 9: lane l < 27 owns the three horizontally adjacent pixels
-    // 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..), so the search-image taps of a lane are 4 consecutive
-    // bytes on two rows (packed fast path below); the integer window sums are order independent.
-    constexpr bool PACK3 = (WIN == 9);
-#define PIX(lane_, k_) (PACK3 ? ((lane_) < 27 ? 3 * (lane_) + (k_) : NPX) : (lane_) + 32 * (k_))
-    constexpr int DW = WIN + 1;  // derivative / search patch width
+    using kltsetup::WIN;
+    using kltsetup::DW;          // search patch width
+    // lane l < 27 owns the three horizontally adjacent window pixels 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..),
+    // so the search-image taps of a lane are 4 consecutive bytes on two rows (packed fast path below); the integer
+    // window sums are order independent.
+    constexpr int PER_LANE = 3;
     const float half = (WIN - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
     bool status = true;
@@ -128,7 +94,6 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         // ---- level set-up (klt_setup.cuh): 12 x 12 neighbourhood -> shared memory (aligned words on the
         //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window + exact
         //      integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2.
-        static_assert(WIN == kltsetup::WIN, "the level set-up is written for the 9 x 9 window");
         __syncwarp();
         const bool tmpl_aligned = ((reinterpret_cast<uintptr_t>(Iimg) | (uintptr_t)Ipitch) & 3) == 0;
         const int off = kltsetup::stage_patch(lane, Iimg, Ipitch, lw, lh, ix, iy, tmpl_aligned, sP);
@@ -148,11 +113,9 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         // every window whose mean |gradient| is below ~3200 of the possible 8160, i.e. anything but a synthetic
         // checkerboard; 8162 * 262000 < 2^31); otherwise the split 64-bit reduction is kept.  Same integers either way.
         int sabs = 0;
-        if (PACK3) {
 #pragma unroll
-            for (int k = 0; k < PER_LANE; ++k) sabs += abs((int)Ixv[k]) + abs((int)Iyv[k]);
-        }
-        const bool b32 = PACK3 && __reduce_add_sync(FULL, sabs) < 262000;
+        for (int k = 0; k < PER_LANE; ++k) sabs += abs((int)Ixv[k]) + abs((int)Iyv[k]);
+        const bool b32 = __reduce_add_sync(FULL, sabs) < 262000;
         // |window sums| <= 81 * 4080^2 = 1.35e9 < 2^31 for the 9 x 9 window: one exact 32-bit redux each
         // (the b sums of the iterations can reach 2.7e9 and keep the split 64-bit reduction)
         float A11 = __int2float_rn(__reduce_add_sync(FULL, sA11)) * FLT_SCALE;
@@ -187,7 +150,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
             iw10 = __float2int_rn((1.f - a) * b * 16384.f);
             iw11 = 16384 - iw00 - iw01 - iw10;
             int sb1 = 0, sb2 = 0;
-            if (PACK3 && (same || (packed_ok && jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh))) {
+            if (same || (packed_ok && jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh)) {
                 // interior, word-aligned level (warp-uniform): the lane's 4 + 4 taps come from two aligned
                 // 32-bit words per row (funnel shift), the 14-bit bilinear weights are applied with
                 // dp2a (u16 x u8 pairs): 4 loads + 6 dp2a per lane instead of 12 byte loads + 12 IMADs.
@@ -202,14 +165,14 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
                         const unsigned t0 = __ldg(w), b0 = __ldg(wb);
                         unsigned t1 = 0, b1w = 0;
                         if (sh) { t1 = __ldg(w + 1); b1w = __ldg(wb + 1); }
-                        top = __funnelshift_r(t0, t1, sh);
-                        bot = __funnelshift_r(b0, b1w, sh);
+                        top = kltsetup::funnel_r(t0, t1, sh);
+                        bot = kltsetup::funnel_r(b0, b1w, sh);
                     }
                     const unsigned W01 = ((unsigned)iw00 & 0xFFFFu) | ((unsigned)iw01 << 16);
                     const unsigned W23 = ((unsigned)iw10 & 0xFFFFu) | ((unsigned)iw11 << 16);
-                    const int j0 = dp2a_lo_su(W01, top, dp2a_lo_su(W23, bot, 256)) >> 9;
-                    const int j1 = dp2a_lo_su(W01, top >> 8, dp2a_lo_su(W23, bot >> 8, 256)) >> 9;
-                    const int j2 = dp2a_hi_su(W01, top, dp2a_hi_su(W23, bot, 256)) >> 9;
+                    const int j0 = kltsetup::dp2a_lo_su16(W01, top, kltsetup::dp2a_lo_su16(W23, bot, 256)) >> 9;
+                    const int j1 = kltsetup::dp2a_lo_su16(W01, top >> 8, kltsetup::dp2a_lo_su16(W23, bot >> 8, 256)) >> 9;
+                    const int j2 = kltsetup::dp2a_hi_su16(W01, top, kltsetup::dp2a_hi_su16(W23, bot, 256)) >> 9;
                     const int d0 = j0 - (int)Iv[0], d1 = j1 - (int)Iv[1], d2 = j2 - (int)Iv[2];
                     sb1 = d0 * (int)Ixv[0] + d1 * (int)Ixv[1] + d2 * (int)Ixv[2];
                     sb2 = d0 * (int)Iyv[0] + d1 * (int)Iyv[1] + d2 * (int)Iyv[2];
@@ -218,13 +181,11 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
                 cjy = jy;
             } else if (jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh) {
                 // interior (warp-uniform): every lane gathers its own 4 taps straight from L1/L2
-                const uint8_t* src = Jimg + (size_t)jy * Jpitch + jx;
+                if (lane < 27) {
+                    const uint8_t* src = Jimg + (size_t)(jy + lane_row) * Jpitch + (jx + lane_col);
 #pragma unroll
-                for (int k = 0; k < PER_LANE; ++k) {
-                    int p = PIX(lane, k);
-                    if (p < NPX) {
-                        int y = p / WIN, x = p - y * WIN;
-                        const uint8_t* q = src + y * Jpitch + x;
+                    for (int k = 0; k < PER_LANE; ++k) {
+                        const uint8_t* q = src + k;
                         int jval = ((int)__ldg(q) * iw00 + (int)__ldg(q + 1) * iw01 + (int)__ldg(q + Jpitch) * iw10 +
                                     (int)__ldg(q + Jpitch + 1) * iw11 + (1 << 8)) >> 9;
                         int diff = jval - (int)Iv[k];
@@ -236,16 +197,15 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
                 __syncwarp();
                 for (int i = lane; i < DW * DW; i += 32) {
                     int r = i / DW, c = i - r * DW;
-                    int y = reflect101_safe(jy + r, lh), x = reflect101_safe(jx + c, lw);
+                    int y = kltsetup::reflect101_any(jy + r, lh), x = kltsetup::reflect101_any(jx + c, lw);
                     sP[i] = __ldg(Jimg + (size_t)y * Jpitch + x);
                 }
                 __syncwarp();
+                if (lane < 27) {
+                    const uint8_t* src = sP + lane_row * DW + lane_col;
 #pragma unroll
-                for (int k = 0; k < PER_LANE; ++k) {
-                    int p = PIX(lane, k);
-                    if (p < NPX) {
-                        int y = p / WIN, x = p - y * WIN;
-                        const uint8_t* q = sP + y * DW + x;
+                    for (int k = 0; k < PER_LANE; ++k) {
+                        const uint8_t* q = src + k;
                         int jval = ((int)q[0] * iw00 + (int)q[1] * iw01 + (int)q[DW] * iw10 + (int)q[DW + 1] * iw11 + (1 << 8)) >> 9;
                         int diff = jval - (int)Iv[k];
                         sb1 += diff * (int)Ixv[k];
@@ -286,11 +246,9 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
     }
     err_out = err;
     return status;
-#undef PIX
 }
 
 // One keypoint, whole warp: forward track, checks, backward track, forward-backward test (feature_tracker.cpp:35-137).
-template <int WIN>
 __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane) {
     const int frame = A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame;
     int maxlevel = A.lvls ? (int)A.lvls[i] : A.lvl_all;
@@ -302,7 +260,7 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     // x < 0 marks an empty slot of a fixed-stride batch (the detectors pad their output with (-1, -1),
     // ov2_describe uses the same rule): status 0, prior untouched, no work
     bool ok = kp.x >= 0.f &&
-              lk_track<WIN>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err, sPw, sDw, lane);
+              lk_track(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err, sPw, sDw, lane);
     // feature_tracker.cpp:79-101
     if (ok && err > A.ferr) ok = false;
     if (ok) {
@@ -313,7 +271,7 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
         // backward: template from the current image at the forward result, search the previous image
         float2 back = kp;
         float err2 = 0.f;
-        bool ok2 = lk_track<WIN>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw, lane);
+        bool ok2 = lk_track(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw, lane);
         if (!ok2) ok = false;
         else {
             float dx = kp.x - back.x, dy = kp.y - back.y;
@@ -328,280 +286,23 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
 }
 
 // Keypoints need very different iteration counts (1 .. 30 per level), so a static warp <-> keypoint
-// assignment leaves SM slots idle while the slowest warp of a CTA finishes.  The persistent variant
-// fills the GPU once (resident CTAs only) and every warp pulls the next keypoint from a global counter.
-template <int WIN, int WARPS_PER_CTA>
+// assignment leaves SM slots idle while the slowest warp of a CTA finishes.  When the grid exceeds the
+// resident CTAs, the launch fills the GPU once and every warp pulls the next keypoint from a global counter.
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A) {
     __shared__ __align__(16) uint8_t sPall[WARPS_PER_CTA][kltsetup::SP_BYTES];
     __shared__ __align__(16) int sDall[WARPS_PER_CTA][kltsetup::SD_INTS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int i = blockIdx.x * WARPS_PER_CTA + warp;;) {
-    if (A.work_counter) {
-        int nxt_i = 0;
-        if (lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
-        i = __shfl_sync(FULL, nxt_i, 0);
-    }
-    if (A.from_list) {
-        if (i >= *A.defer_count) return;
-        i = A.defer_list[i];
-    }
-    if (i >= A.n) return;
-    klt_one<WIN>(A, i, sPall[warp], sDall[warp], lane);
-    if (!A.work_counter) return;
-    __syncwarp();
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Three keypoints per warp.  In fb_klt_kernel every lane of the warp replays the per-keypoint scalar part of an LK
-// iteration (floor, bilinear weights, the two reductions, the 2 x 2 solve, the convergence tests: ~100 of the ~110
-// instructions of an iteration) and of a level set-up for ONE keypoint.  Here a warp carries three keypoints: lanes
-// 10 g .. 10 g + 9 belong to keypoint g, lane r < 9 of a group owns window ROW r (nine pixels, klt_setup.cuh::template_row9 /
-// mismatch_row9: the same integers), lane 9 fetches the tenth search row; the scalar part is computed once per lane for the
-// lane's own keypoint, so one pass of it serves three keypoints.  The three keypoints walk the pyramid levels and the
-// iterations in lock step (a group that has converged idles until the others have).  Only interior, word-aligned windows
-// are handled; a keypoint that meets anything else (border window at any level or iteration, unaligned aliased level 0,
-// gradients too large for the 32-bit reduction) is appended to defer_list and tracked from scratch by fb_klt_kernel
-// afterwards - results are those of fb_klt_kernel by construction.
-__device__ __forceinline__ int group_sum9(int v, int r, int leader) {
-    int t;
-    t = __shfl_down_sync(FULL, v, 8); if (r <= 1) v += t;
-    t = __shfl_down_sync(FULL, v, 4); if (r < 4) v += t;
-    t = __shfl_down_sync(FULL, v, 2); if (r < 2) v += t;
-    t = __shfl_down_sync(FULL, v, 1); if (r < 1) v += t;
-    return __shfl_sync(FULL, v, leader);
-}
-
-// state: 0 = lost (status false), 1 = tracked, 2 = deferred.  `run`: the group holds a keypoint to track in this call.
-__device__ int lk_track3(const PyrView& Ipyr, const PyrView& Jpyr, int frame, bool run, float2 pt, float2& nxt, int maxlevel, int max_iter,
-                         double eps2, float eps_lo, float eps_hi, float& err_out, int lane, int r, int leader) {
-    constexpr int WIN = 9;
-    const float half = (WIN - 1) * 0.5f;
-    const float FLT_SCALE = 1.f / (1 << 20);
-    bool status = true, defer = false;
-    float err = 0.f;
-    const int lmax = __reduce_max_sync(FULL, run ? maxlevel : -1);
-    for (int level = lmax; level >= 0; --level) {
-        bool act = run && !defer && level <= maxlevel;
-        const int lw = Ipyr.w[level], lh = Ipyr.h[level];
-        const uint8_t* Iimg = Ipyr.lvl[level] + Ipyr.fstride[level] * frame;
-        const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
-        const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
-        const bool aligned = ((reinterpret_cast<uintptr_t>(Iimg) | (uintptr_t)Ipitch | reinterpret_cast<uintptr_t>(Jimg) | (uintptr_t)Jpitch) & 3) == 0;
-        const float sc = 1.f / (float)(1 << level);
-        float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
-        float2 nextPt;
-        if (level == maxlevel) nextPt = make_float2(nxt.x * sc, nxt.y * sc);
-        else nextPt = make_float2(nxt.x * 2.f, nxt.y * 2.f);
-        if (act) nxt = nextPt;
-        prevPt.x -= half;
-        prevPt.y -= half;
-        const int ix = __float2int_rd(prevPt.x), iy = __float2int_rd(prevPt.y);
-        if (act && (ix < -WIN || ix >= lw || iy < -WIN || iy >= lh)) {
-            if (level == 0) { status = false; err = 0.f; }
-            act = false;
+        if (A.work_counter) {
+            int nxt_i = 0;
+            if (lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
+            i = __shfl_sync(FULL, nxt_i, 0);
         }
-        if (act && !(aligned && kltsetup::patch_interior(ix, iy, lw, lh))) { defer = true; act = false; }
-        float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
-        int iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
-        int iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
-        int iw10 = __float2int_rn((1.f - a) * b * 16384.f);
-        int iw11 = 16384 - iw00 - iw01 - iw10;
-        // ---- level set-up: window row r of the group's keypoint
-        short Iv[9], Ixv[9], Iyv[9];
-        int sA11 = 0, sA12 = 0, sA22 = 0, sabs = 0;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) { Iv[k] = 0; Ixv[k] = 0; Iyv[k] = 0; }
-        if (act && r < 9) {
-            unsigned nb[4][3];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) kltsetup::load_row12(Iimg + (size_t)(iy - 1 + r + k) * Ipitch, ix - 1, lw, nb[k]);
-            kltsetup::template_row9(nb, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22, sabs);
-        }
-        sA11 = group_sum9(sA11, r, leader);
-        sA12 = group_sum9(sA12, r, leader);
-        sA22 = group_sum9(sA22, r, leader);
-        sabs = group_sum9(sabs, r, leader);
-        const float A11 = __int2float_rn(sA11) * FLT_SCALE, A12 = __int2float_rn(sA12) * FLT_SCALE, A22 = __int2float_rn(sA22) * FLT_SCALE;
-        float D = A11 * A22 - A12 * A12;
-        const float minEig = (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * WIN * WIN);
-        if (act) {
-            err = minEig;
-            if ((double)minEig < 1e-4 || D < 1.1920928955078125e-07f) {
-                if (level == 0) status = false;
-                act = false;
-            }
-        }
-        if (act && sabs >= 262000) { defer = true; act = false; }   // the mismatch sums might not fit 32 bits: leave it to fb_klt_kernel
-        D = 1.f / D;
-        nextPt.x -= half;
-        nextPt.y -= half;
-        float2 prevDelta = make_float2(0.f, 0.f);
-        bool it_on = act;
-        int cjx = INT_MIN, cjy = INT_MIN;
-        unsigned tw[3] = {0u, 0u, 0u}, bw[3] = {0u, 0u, 0u};
-        for (int j = 0; j < max_iter; ++j) {
-            if (!__any_sync(FULL, it_on)) break;
-            const int jx = __float2int_rd(nextPt.x), jy = __float2int_rd(nextPt.y);
-            if (it_on && (jx < -WIN || jx >= lw || jy < -WIN || jy >= lh)) {
-                if (level == 0) status = false;
-                it_on = false;
-            }
-            if (it_on && !(jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh)) { defer = true; it_on = false; }
-            a = nextPt.x - (float)jx;
-            b = nextPt.y - (float)jy;
-            iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
-            iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
-            iw10 = __float2int_rn((1.f - a) * b * 16384.f);
-            iw11 = 16384 - iw00 - iw01 - iw10;
-            // search rows: lane r (0..9) holds row jy + r; the row below comes from the next lane.  Reloaded only when the
-            // window's integer origin moved.
-            const bool reload = it_on && (jx != cjx || jy != cjy);
-            if (reload) {
-                kltsetup::load_row12(Jimg + (size_t)(jy + r) * Jpitch, jx, lw, tw);
-                cjx = jx; cjy = jy;
-            }
-            if (__any_sync(FULL, reload)) {
-                const unsigned n0 = __shfl_down_sync(FULL, tw[0], 1), n1 = __shfl_down_sync(FULL, tw[1], 1), n2 = __shfl_down_sync(FULL, tw[2], 1);
-                if (reload) { bw[0] = n0; bw[1] = n1; bw[2] = n2; }
-            }
-            int sb1 = 0, sb2 = 0;
-            if (it_on && r < 9) kltsetup::mismatch_row9(tw, bw, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sb1, sb2);
-            sb1 = group_sum9(sb1, r, leader);
-            sb2 = group_sum9(sb2, r, leader);
-            if (it_on) {
-                const float b1 = __int2float_rn(sb1) * FLT_SCALE, b2 = __int2float_rn(sb2) * FLT_SCALE;
-                const float2 delta = make_float2((A12 * b2 - A22 * b1) * D, (A12 * b1 - A11 * b2) * D);
-                nextPt.x += delta.x;
-                nextPt.y += delta.y;
-                nxt = make_float2(nextPt.x + half, nextPt.y + half);
-                const float q = delta.x * delta.x + delta.y * delta.y;
-                bool conv;
-                if (q < eps_lo) conv = true;
-                else if (q > eps_hi) conv = false;
-                else conv = (double)delta.x * (double)delta.x + (double)delta.y * (double)delta.y <= eps2;
-                if (conv) it_on = false;
-                else if (j > 0 && fabsf(delta.x + prevDelta.x) <= 0.01f && fabsf(delta.y + prevDelta.y) <= 0.01f) {
-                    nxt.x -= delta.x * 0.5f;
-                    nxt.y -= delta.y * 0.5f;
-                    it_on = false;
-                }
-                prevDelta = delta;
-            }
-        }
-    }
-    err_out = err;
-    return defer ? 2 : (status ? 1 : 0);
-}
-
-// Pre-pass of the three-keypoints-per-warp kernel: split the keypoint indices by pyramid depth (warp-aggregated appends; the
-// order inside a bucket is irrelevant - a keypoint's result does not depend on which keypoints share its warp).
-__global__ void __launch_bounds__(256) klt_bucket_kernel(KltArgs A, int* bucket, int* bucket_count) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
-    const bool valid = i < A.n;
-    int lvl = valid ? (int)A.lvls[i] : 0;
-    if (lvl > A.prev.nlev - 1) lvl = A.prev.nlev - 1;
-    const bool deep = valid && lvl > 1, shallow = valid && !deep;
-    const unsigned md = __ballot_sync(FULL, deep), ms = __ballot_sync(FULL, shallow);
-    int bd = 0, bs = 0;
-    if (lane == 0) {
-        if (md) bd = atomicAdd(bucket_count + 1, __popc(md));
-        if (ms) bs = atomicAdd(bucket_count, __popc(ms));
-    }
-    bd = __shfl_sync(FULL, bd, 0);
-    bs = __shfl_sync(FULL, bs, 0);
-    const unsigned lt = (1u << lane) - 1u;
-    if (deep) bucket[A.n + bd + __popc(md & lt)] = i;
-    if (shallow) bucket[bs + __popc(ms & lt)] = i;
-}
-
-template <int WARPS_PER_CTA>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32) fb_klt3_kernel(KltArgs A) {
-    const int lane = threadIdx.x & 31;
-    const int g = lane / 10, r = lane - 10 * g;
-    const bool member = g < 3;
-    const int leader = 10 * g;                     // lanes 30, 31: leader 30 (a group without a keypoint)
-    int n0 = A.n, n1 = 0;                          // bucket sizes (no buckets: everything in "bucket 0", identity order)
-    if (A.bucket) { n0 = A.bucket_count[0]; n1 = A.bucket_count[1]; }
-    const int ntrip0 = (n0 + 2) / 3, ntrip = ntrip0 + (n1 + 2) / 3;
-    for (;;) {
-        int t = 0;
-        if (lane == 0) t = atomicAdd(A.work_counter, 1);
-        t = __shfl_sync(FULL, t, 0);
-        if (t >= ntrip) return;
-        int i = 0;
-        bool have = false;
-        if (member) {
-            const int e = t < ntrip0 ? 3 * t + g : 3 * (t - ntrip0) + g;      // entry inside the triple's bucket
-            have = e < (t < ntrip0 ? n0 : n1);
-            if (have) i = A.bucket ? A.bucket[(t < ntrip0 ? 0 : A.n) + e] : e;
-        }
-        const int frame = have ? (A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame) : 0;
-        int maxlevel = have ? (A.lvls ? (int)A.lvls[i] : A.lvl_all) : 0;
-        if (maxlevel > A.prev.nlev - 1) maxlevel = A.prev.nlev - 1;  // feature_tracker.cpp:50-52
-        if (maxlevel < 0) maxlevel = 0;
-        const float2 kp = have ? A.kps[i] : make_float2(-1.f, -1.f);
-        float2 fwd = have ? A.priors[i] : make_float2(0.f, 0.f);
-        const bool run = have && kp.x >= 0.f;     // x < 0: empty slot - status 0, prior untouched
-        float err = 0.f;
-        int st = lk_track3(A.prev, A.cur, frame, run, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err, lane, r, leader);
-        bool ok = run && st == 1;
-        bool defer = run && st == 2;
-        // feature_tracker.cpp:79-101
-        if (ok && err > A.ferr) ok = false;
-        if (ok) {
-            const float w0 = (float)A.cur.w[0], h0 = (float)A.cur.h[0];
-            if (!(1.f <= fwd.x && fwd.x < w0 - 1.f && 1.f <= fwd.y && fwd.y < h0 - 1.f)) ok = false;
-        }
-        // backward: template from the current image at the forward result, search the previous image (all groups in lock step)
-        float2 back = kp;
-        float err2 = 0.f;
-        st = lk_track3(A.cur, A.prev, frame, ok, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, lane, r, leader);
-        if (ok) {
-            if (st == 2) { defer = true; ok = false; }
-            else if (st == 0) ok = false;
-            else {
-                const float dx = kp.x - back.x, dy = kp.y - back.y;
-                const double nrm = sqrt((double)dx * (double)dx + (double)dy * (double)dy);
-                if (nrm > (double)A.fb_dist) ok = false;
-            }
-        }
-        if (have && r == 0) {
-            if (defer) {
-                A.defer_list[atomicAdd(A.defer_count, 1)] = i;       // prior untouched: klt_one starts from the same guess
-            } else {
-                if (run) A.priors[i] = fwd;
-                A.status[i] = ok ? 1 : 0;
-            }
-        }
+        if (i >= A.n) return;
+        klt_one(A, i, sPall[warp], sDall[warp], lane);
+        if (!A.work_counter) return;
         __syncwarp();
     }
-}
-// (Draining the deferred list inside the same launch was tried twice - warps leaving when the list is momentarily empty:
-//  the last few warps inherit the whole tail, 33 ms; warps polling a completion counter: thousands of pollers on the cache
-//  line that also holds the work-queue counters, 83 ms.  The second launch below costs one launch gap.)
-
-template <int WPC>
-ov2_status launch_klt(ov2_ctx* ctx, KltArgs& A, bool persistent) {
-    int grid = div_up(A.n, WPC);
-    A.work_counter = nullptr;
-    if (persistent) {
-        int per_sm = 0, dev = 0, sms = 0;
-        OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<9, WPC>, WPC * 32, 0));
-        OV2_CUDA(ctx, cudaGetDevice(&dev));
-        OV2_CUDA(ctx, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        const int resident = per_sm * sms;
-        if (grid > resident) {
-            void* o = nullptr;
-            ov2_status st = ov2_scratch(ctx, sizeof(int), &o);
-            if (st != OV2_OK) return st;
-            A.work_counter = (int*)o;
-            OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
-            grid = resident;
-        }
-    }
-    OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<9, WPC><<<grid, WPC * 32, 0, ctx->stream>>>(A)));
-    return OV2_OK;
 }
 
 // Depth cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), maxlevel) reaches: it stops before a level whose width or
@@ -639,7 +340,6 @@ extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_py
     A.per_frame = per_frame;
     A.lvl_all = nbpyrlvl_all;
     A.max_iter = prm->max_iter;
-    A.eps = prm->eps;
     A.eps2 = (double)prm->eps * (double)prm->eps;
     A.eps_lo = (float)(A.eps2 * (1.0 - 1e-6));
     A.eps_hi = (float)(A.eps2 * (1.0 + 1e-6));
@@ -657,56 +357,16 @@ extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_py
     A.priors = (float2*)o;
     if ((st = ov2_stage_out(ctx, status_out, (size_t)n, &o)) != OV2_OK) return st;
     A.status = (uint8_t*)o;
-    A.defer_list = nullptr; A.defer_count = nullptr; A.from_list = 0; A.bucket = nullptr; A.bucket_count = nullptr;
-    {
-        // three keypoints per warp (OV2_KLT_MODE=3) + the one-warp-per-keypoint kernel for what it defers
-        const char* m = getenv("OV2_KLT_MODE");
-        if (m && atoi(m) == 3 && n >= 96) {
-            void* o2 = nullptr;
-            if ((st = ov2_scratch(ctx, sizeof(int) * ((size_t)n + 4), &o2)) != OV2_OK) return st;
-            int* blk = (int*)o2;                               // [0] triple counter, [1] deferred count, [2] list counter, [4..] list
-            OV2_CUDA(ctx, cudaMemsetAsync(blk, 0, sizeof(int) * 4, ctx->stream));
-            A.work_counter = blk;
-            A.defer_count = blk + 1;
-            A.defer_list = blk + 4;
-            A.bucket = nullptr; A.bucket_count = nullptr;
-            if (A.lvls && !(getenv("OV2_KLT_BUCKET") && atoi(getenv("OV2_KLT_BUCKET")) == 0)) {
-                void* o3 = nullptr;
-                if ((st = ov2_scratch(ctx, sizeof(int) * (2 * (size_t)n + 2), &o3)) != OV2_OK) return st;
-                int* bk = (int*)o3;                            // [0], [1] bucket sizes, [2 ..] the two buckets
-                OV2_CUDA(ctx, cudaMemsetAsync(bk, 0, sizeof(int) * 2, ctx->stream));
-                OV2_LAUNCH(ctx, "klt_bucket_kernel", (klt_bucket_kernel<<<div_up(n, 256), 256, 0, ctx->stream>>>(A, bk + 2, bk)));
-                A.bucket = bk + 2;
-                A.bucket_count = bk;
-            }
-            int per_sm = 0;
-            OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt3_kernel<8>, 256, 0));
-            const int ntrip = (n + 2) / 3;
-            int grid = per_sm * ctx->sm_count;
-            if (grid > div_up(ntrip, 8)) grid = div_up(ntrip, 8);
-            OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt3_kernel<8><<<grid, 256, 0, ctx->stream>>>(A)));
-            KltArgs B = A;
-            B.work_counter = blk + 2;
-            B.from_list = 1;
-            OV2_LAUNCH(ctx, "fb_klt_deferred", (fb_klt_kernel<9, 8><<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(B)));
-            if (getenv("OV2_KLT_DEBUG")) {
-                int nd = 0;
-                cudaMemcpyAsync(&nd, blk + 1, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
-                cudaStreamSynchronize(ctx->stream);
-                fprintf(stderr, "[klt3] %d keypoints, %d deferred (%.1f %%)\n", n, nd, 100.0 * nd / (n > 0 ? n : 1));
-            }
-            return ov2_end(ctx);
-        }
+    int grid = div_up(n, WARPS_PER_CTA), per_sm = 0;
+    A.work_counter = nullptr;
+    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel, WARPS_PER_CTA * 32, 0));
+    const int resident = per_sm * ctx->sm_count;
+    if (grid > resident) {
+        if ((st = ov2_scratch(ctx, sizeof(int), &o)) != OV2_OK) return st;
+        A.work_counter = (int*)o;
+        OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
+        grid = resident;
     }
-    {
-        const char* e = getenv("OV2_KLT_WPC");
-        const int wpc = e ? atoi(e) : 8;
-        const char* pe = getenv("OV2_KLT_PERSIST");
-        const bool persistent = pe ? atoi(pe) != 0 : true;
-        if (wpc == 2) st = launch_klt<2>(ctx, A, persistent);
-        else if (wpc == 4) st = launch_klt<4>(ctx, A, persistent);
-        else st = launch_klt<8>(ctx, A, persistent);
-        if (st != OV2_OK) return st;
-    }
+    OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A)));
     return ov2_end(ctx);
 }

@@ -1,6 +1,7 @@
 // K (level set-up): template patch staging, Scharr derivatives and the int16 template / derivative
 // window of one Lucas-Kanade level, for the 9 x 9 window (all reference configurations,
-// /root/reference/src/feature_tracker.cpp:35-137 via cv::calcOpticalFlowPyrLK).
+// /root/reference/src/feature_tracker.cpp:35-137 via cv::calcOpticalFlowPyrLK), and the reflect-101 /
+// dp2a / funnel-shift helpers that the tracker's iterations (frontend_klt.cu) use as well.
 //
 // Written as plain per-lane functions (no warp intrinsics; the phases are separated by __syncwarp in
 // the kernel) so that tests/test_host_logic.py can compile the SAME code for the host and check it
@@ -137,7 +138,8 @@ KLT_HD void template_rows(int lane, const uint8_t* sP, int off, const int* sD, i
     }
 }
 
-// dp2a: signed 16-bit halves of a times UNSIGNED bytes of b (lo: bytes 0, 1; hi: bytes 2, 3), plus c
+// dp2a: signed 16-bit halves of a (bilinear weights: iw11 = 16384 - others can round to -1) times UNSIGNED bytes of b
+// (pixels; lo: bytes 0, 1; hi: bytes 2, 3), plus c
 KLT_HD int dp2a_lo_su16(unsigned a, unsigned b, int c) {
 #if defined(__CUDA_ARCH__)
     int d;
@@ -216,88 +218,6 @@ KLT_HD void template_direct(int lane, const uint8_t* sP, int off, int iw00, int 
         sA11 += ixval * ixval;
         sA12 += ixval * iyval;
         sA22 += iyval * iyval;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Row-per-lane forms (three keypoints per warp, fb_klt3_kernel): a lane owns window ROW r (9 pixels) of its keypoint.
-// Interior windows only.  Same integers as template_rows() / the packed iteration path, checked on the host
-// (tests/test_host_logic.py).
-
-// 12 bytes of an image row starting at column x (x + 11 < lw guaranteed by patch_interior; the aligned word that holds
-// bytes beyond column lw - 1 is not loaded): w[0..2] = bytes x .. x+11
-KLT_HD void load_row12(const uint8_t* row, int x, int lw, unsigned w[3]) {
-    const int x0 = x & ~3;
-    const unsigned sh = (unsigned)(x & 3) * 8u;
-    const uint32_t* p = reinterpret_cast<const uint32_t*>(row + x0);
-    const unsigned a0 = KLT_LDG32(p), a1 = KLT_LDG32(p + 1), a2 = KLT_LDG32(p + 2);
-    const unsigned a3 = (sh != 0u && x0 + 12 < lw) ? KLT_LDG32(p + 3) : 0u;
-    w[0] = funnel_r(a0, a1, sh);
-    w[1] = funnel_r(a1, a2, sh);
-    w[2] = funnel_r(a2, a3, sh);
-}
-
-// the eleven adjacent byte pairs (c, c+1), c = 0..10, of a 12-byte row as dp2a operands:
-// W[c] = dp2a(W01, top pair c) + dp2a(W23, bottom pair c)
-KLT_HD void interp_row11(const unsigned t[3], const unsigned b[3], unsigned W01, unsigned W23, int W[11]) {
-#pragma unroll
-    for (int q = 0; q < 3; ++q) {
-        const unsigned tw = t[q], bw = b[q];
-        W[4 * q + 0] = dp2a_lo_su16(W01, tw, dp2a_lo_su16(W23, bw, 0));
-        W[4 * q + 1] = dp2a_lo_su16(W01, tw >> 8, dp2a_lo_su16(W23, bw >> 8, 0));
-        W[4 * q + 2] = dp2a_hi_su16(W01, tw, dp2a_hi_su16(W23, bw, 0));
-        if (q < 2) {
-            const unsigned t3 = funnel_r(tw, t[q + 1], 24u), b3 = funnel_r(bw, b[q + 1], 24u);
-            W[4 * q + 3] = dp2a_lo_su16(W01, t3, dp2a_lo_su16(W23, b3, 0));
-        }
-    }
-}
-
-// template row r: nb[k] = the 12-byte neighbourhood rows r + k (k = 0..3; neighbourhood row 0 is image row iy - 1, its
-// byte 0 image column ix - 1).  Outputs the nine I / Ix / Iy of window row r and the row's share of the A sums.
-KLT_HD void template_row9(const unsigned nb[4][3], int iw00, int iw01, int iw10, int iw11, short* Iv, short* Ixv, short* Iyv,
-                          int& sA11, int& sA12, int& sA22, int& sabs) {
-    const unsigned W01 = ((unsigned)iw00 & 0xFFFFu) | ((unsigned)iw01 << 16);
-    const unsigned W23 = ((unsigned)iw10 & 0xFFFFu) | ((unsigned)iw11 << 16);
-    int W0[11], W1[11], W2[11];
-    interp_row11(nb[0], nb[1], W01, W23, W0);
-    interp_row11(nb[1], nb[2], W01, W23, W1);
-    interp_row11(nb[2], nb[3], W01, W23, W2);
-    int vs[11], vd[11];
-#pragma unroll
-    for (int c = 0; c < 11; ++c) {
-        vs[c] = (W0[c] + W2[c]) * 3 + W1[c] * 10;
-        vd[c] = W2[c] - W0[c];
-    }
-    sA11 = 0; sA12 = 0; sA22 = 0; sabs = 0;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-        const int ival = (W1[k + 1] + (1 << 8)) >> 9;
-        const int ixval = (vs[k + 2] - vs[k] + (1 << 13)) >> 14;
-        const int iyval = ((vd[k] + vd[k + 2]) * 3 + vd[k + 1] * 10 + (1 << 13)) >> 14;
-        Iv[k] = (short)ival; Ixv[k] = (short)ixval; Iyv[k] = (short)iyval;
-        sA11 += ixval * ixval;
-        sA12 += ixval * iyval;
-        sA22 += iyval * iyval;
-        sabs += (ixval < 0 ? -ixval : ixval) + (iyval < 0 ? -iyval : iyval);
-    }
-}
-
-// one LK iteration's share of window row r: search rows (jy + r, jy + r + 1) as 12-byte rows starting at column jx
-// (only bytes 0..9 are used)
-KLT_HD void mismatch_row9(const unsigned top[3], const unsigned bot[3], int iw00, int iw01, int iw10, int iw11,
-                          const short* Iv, const short* Ixv, const short* Iyv, int& sb1, int& sb2) {
-    const unsigned W01 = ((unsigned)iw00 & 0xFFFFu) | ((unsigned)iw01 << 16);
-    const unsigned W23 = ((unsigned)iw10 & 0xFFFFu) | ((unsigned)iw11 << 16);
-    int J[11];
-    interp_row11(top, bot, W01, W23, J);
-    sb1 = 0; sb2 = 0;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-        const int jval = (J[k] + (1 << 8)) >> 9;
-        const int diff = jval - (int)Iv[k];
-        sb1 += diff * (int)Ixv[k];
-        sb2 += diff * (int)Iyv[k];
     }
 }
 

@@ -257,14 +257,10 @@ def _klt_inputs(seed, w, h, n_border=60):
     return prev, cur, flow, kps, is3d, pri
 
 
-@pytest.mark.parametrize("mode", ["1", "3"])
 @pytest.mark.parametrize("nbpyrlvl", [0, 1, 3])
-def test_klt_parity(ctx, monkeypatch, nbpyrlvl, mode):
+def test_klt_parity(ctx, nbpyrlvl):
     """fbKltTracking vs the oracle: status flags and tracked positions bit-equal to the exact-integer restatement; against
-    cv2 (when importable) statuses identical, positions within KLT_CV2_TOL and >= 97 % bit-equal (see the constants above).
-    mode 3 = the three-keypoints-per-warp kernel (OV2_KLT_MODE=3) with its deferred border keypoints tracked by the
-    one-warp-per-keypoint kernel: same answers."""
-    monkeypatch.setenv("OV2_KLT_MODE", mode)
+    cv2 (when importable) statuses identical, positions within KLT_CV2_TOL and >= 97 % bit-equal (see the constants above)."""
     w, h = 640, 480
     prev, cur, flow, kps, is3d, pri = _klt_inputs(7, w, h)
     pp = api.Pyramid(ctx, 1, w, h, 3)
@@ -281,11 +277,9 @@ def test_klt_parity(ctx, monkeypatch, nbpyrlvl, mode):
     cp.close()
 
 
-@pytest.mark.parametrize("mode", ["1", "3"])
-def test_klt_mixed_levels_batched(ctx, monkeypatch, mode):
+def test_klt_mixed_levels_batched(ctx):
     """The reference's two calls (nbpyrlvl 1 for 3D-prior keypoints, 3 for the rest,
     visual_front_end.cpp:196,242) fused in one ragged launch over several frames."""
-    monkeypatch.setenv("OV2_KLT_MODE", mode)
     w, h = 640, 480
     nfr = 3
     data = [_klt_inputs(60 + f, w, h, 20) for f in range(nfr)]
@@ -473,12 +467,10 @@ def test_frontend_step_composite_equals_operator_calls(ctx):
     cp.close()
 
 
-@pytest.mark.parametrize("klt_mode", ["1", "3"])
-def test_c4_resolution_1280x720_cell35(ctx, monkeypatch, klt_mode):
+def test_c4_resolution_1280x720_cell35(ctx):
     """BASELINE.json configs[3] geometry: 1280x720, accurate-config cell size 35 (720 cells), CLAHE on
     the tracking image, descriptors on the raw image (map_manager.cpp:301-303): every operator at that
     size against the oracle (the FAST sweep's mask bitmap needs 115 KB of shared memory here)."""
-    monkeypatch.setenv("OV2_KLT_MODE", klt_mode)
     w, h, cs = 1280, 720, 35
     prev, cur, flow = synth.make_pair(500, w, h)
     eq_prev = np.empty_like(prev)

@@ -169,54 +169,6 @@ int main() {
         d11 += t11; d12 += t12; d22 += t22;
       }
       if (A11 != d11 || A12 != d12 || A22 != d22) bad++;
-      // row-per-lane forms (three keypoints per warp): template_row9 from rows read straight from the image must give the
-      // same nine I / Ix / Iy per window row, mismatch_row9 the same b sums as the definition
-      long r11 = 0, r12 = 0, r22 = 0;
-      short Tv[9][9], Tx[9][9], Ty[9][9];
-      for (int r = 0; r < 9; ++r) {
-        unsigned nb[4][3];
-        for (int k = 0; k < 4; ++k) load_row12(img + (size_t)(iy - 1 + r + k) * pitch, ix - 1, lw, nb[k]);
-        int s11, s12, s22, sab;
-        template_row9(nb, iw00, iw01, iw10, iw11, Tv[r], Tx[r], Ty[r], s11, s12, s22, sab);
-        r11 += s11; r12 += s12; r22 += s22;
-        long chk = 0;
-        for (int x = 0; x < 9; ++x) {
-          int iv = (P(r + 1, x + 1) * iw00 + P(r + 1, x + 2) * iw01 + P(r + 2, x + 1) * iw10 + P(r + 2, x + 2) * iw11 + 256) >> 9;
-          int ixv = (dxr[r][x] * iw00 + dxr[r][x + 1] * iw01 + dxr[r + 1][x] * iw10 + dxr[r + 1][x + 1] * iw11 + 8192) >> 14;
-          int iyv = (dyr[r][x] * iw00 + dyr[r][x + 1] * iw01 + dyr[r + 1][x] * iw10 + dyr[r + 1][x + 1] * iw11 + 8192) >> 14;
-          if (Tv[r][x] != (short)iv || Tx[r][x] != (short)ixv || Ty[r][x] != (short)iyv) bad++;
-          chk += (ixv < 0 ? -ixv : ixv) + (iyv < 0 ? -iyv : iyv);
-        }
-        if (chk != sab) bad++;
-      }
-      if (A11 != r11 || A12 != r12 || A22 != r22) bad++;
-      // a search window anywhere inside the same image (the interior condition of the iteration: jx, jy >= 0, + WIN < size)
-      if (lw > WIN + 1 && lh > WIN + 1) {
-        int jx = rng() %% (lw - WIN - 1), jy = rng() %% (lh - WIN - 1);
-        if (jx + 12 <= lw || true) {
-          float ja = (rng() %% 1000) / 1000.f, jb = (rng() %% 1000) / 1000.f;
-          int jw00 = (int)((1.f - ja) * (1.f - jb) * 16384.f + .5f), jw01 = (int)(ja * (1.f - jb) * 16384.f + .5f),
-              jw10 = (int)((1.f - ja) * jb * 16384.f + .5f), jw11 = 16384 - jw00 - jw01 - jw10;
-          long e1 = 0, e2 = 0, g1 = 0, g2 = 0;
-          bool can = jx + 12 <= lw + 3;     // load_row12 reads bytes jx .. jx+11: at most 2 beyond the 10 needed; words past lw are skipped
-          for (int r = 0; r < 9 && can; ++r) {
-            unsigned t[3], b[3];
-            // rows are read through a padded copy so that the 12-byte fetch never leaves the test buffer
-            load_row12(img + (size_t)(jy + r) * pitch, jx, lw, t);
-            load_row12(img + (size_t)(jy + r + 1) * pitch, jx, lw, b);
-            int s1, s2;
-            mismatch_row9(t, b, jw00, jw01, jw10, jw11, Tv[r], Tx[r], Ty[r], s1, s2);
-            g1 += s1; g2 += s2;
-            for (int x = 0; x < 9; ++x) {
-              auto Q = [&](int yy, int xx2) { return (int)img[(size_t)(jy + yy) * pitch + jx + xx2]; };
-              int jv = (Q(r, x) * jw00 + Q(r, x + 1) * jw01 + Q(r + 1, x) * jw10 + Q(r + 1, x + 1) * jw11 + 256) >> 9;
-              int df = jv - (int)Tv[r][x];
-              e1 += (long)df * Tx[r][x]; e2 += (long)df * Ty[r][x];
-            }
-          }
-          if (can && (e1 != g1 || e2 != g2)) bad++;
-        }
-      }
     }
   }
   printf("%%ld bad, %%ld interior, %%ld border\n", bad, n_int, n_brd);

@@ -1,15 +1,13 @@
 """GPU tests of every run-time dispatch path of the KLT tracker (ov2_fb_klt) and the pyramid build (ov2_pyr_build).
 
-ov2_fb_klt picks its kernel and code path at run time: one warp per keypoint (fb_klt_kernel, OV2_KLT_WPC = 2 / 4 / 8 warps
-per CTA, persistent or not, a global work counter once the grid exceeds the resident CTAs) or three keypoints per warp
-(fb_klt3_kernel, OV2_KLT_MODE=3 and n >= 96, with or without the depth buckets, deferring what it cannot take to a second
-fb_klt_kernel launch); word-aligned or byte / reflected template and search reads; 32-bit or split 64-bit mismatch sums.
+ov2_fb_klt tracks every keypoint with one fb_klt_kernel launch, one warp per keypoint, and picks its code paths from the
+input: a global work counter once the grid exceeds the resident CTAs; word-aligned or byte / reflected template and search
+reads; 32-bit or split 64-bit mismatch sums.
 The pyramid runs a fused TMA kernel only for 3 extra levels, level 3 >= 8 x 8 and a 16-byte-aligned level 0, and
 pyr_down_kernel otherwise.  Every case here is compared bit for bit with oracle/image_ref.py (fb_klt_ref,
 build_pyramid_ref) and, where cv2 is importable, the KLT statuses with fb_klt_cv2.  Oracle results are computed once per
 module and shared between parametrisations (fb_klt_ref costs ~3 ms per keypoint).
 """
-import re
 from contextlib import contextmanager
 
 import numpy as np
@@ -21,7 +19,7 @@ from test_frontend_gpu import _klt_assert, _klt_inputs
 
 pytestmark = pytest.mark.gpu
 
-ENV = ("OV2_KLT_MODE", "OV2_KLT_WPC", "OV2_KLT_PERSIST", "OV2_KLT_BUCKET", "OV2_KLT_DEBUG", "OV2_PYR_UNFUSED")
+ENV = ("OV2_PYR_UNFUSED",)
 
 
 def _env(monkeypatch, **kv):
@@ -41,14 +39,6 @@ def _launches(ctx):
         got.update({k: n for k, (_, n) in ctx.profile_report().items()})
     finally:
         ctx.profile(False)
-
-
-def _klt3_lines(capfd):
-    """(keypoints, deferred) of every '[klt3]' line OV2_KLT_DEBUG printed since the last read (echoed to stdout, so that
-    `pytest -rA` reports the counts)."""
-    lines = [(int(a), int(b)) for a, b in re.findall(r"\[klt3\] (\d+) keypoints, (\d+) deferred", capfd.readouterr().err)]
-    print("klt3 (keypoints, deferred):", lines)
-    return lines
 
 
 def _oracle(prevs, curs, kps, pri, lv, fidx, idx=None):
@@ -181,7 +171,7 @@ def test_pyramid_unfused_equals_fused(ctx, monkeypatch, w, h):
             assert np.array_equal(got["1"][f][lvl], ref[lvl]), (f, lvl)
 
 
-# ---------------------------------------------------------------- 2. KLT: every launch variant on one input set
+# ---------------------------------------------------------------- 2. KLT: the default launch on one input set
 @pytest.fixture(scope="module")
 def klt_set():
     """640 x 480, 3 frames, ~1 100 keypoints (FAST corners + border bands), per-keypoint depths 0 - 3, a few empty slots,
@@ -209,41 +199,14 @@ def klt_pyr(ctx, klt_set):
     cp.close()
 
 
-MODE1 = [dict(OV2_KLT_MODE=1, OV2_KLT_WPC=wpc, OV2_KLT_PERSIST=p) for wpc in (2, 4, 8) for p in (0, 1)]
-MODE3 = [dict(OV2_KLT_MODE=3), dict(OV2_KLT_MODE=3, OV2_KLT_BUCKET=0)]
-
-
-@pytest.mark.parametrize("env", MODE1 + MODE3, ids=lambda e: "-".join(f"{k[8:]}{v}" for k, v in e.items()))
-def test_klt_launch_variants(ctx, monkeypatch, klt_set, klt_pyr, env):
-    """One warp per keypoint with 2 / 4 / 8 warps per CTA, persistent or not; three keypoints per warp with and without
-    the depth buckets: the same bits as the oracle for every keypoint."""
-    _env(monkeypatch, **env)
+def test_klt_default_launch(ctx, monkeypatch, klt_set, klt_pyr):
+    """The whole set in one fb_klt_kernel launch: the same bits as the oracle for every keypoint."""
+    _env(monkeypatch)
     s = klt_set
     with _launches(ctx) as k:
         got = _track(ctx, *klt_pyr, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
-    _assert_same(got, s["ref"], env)
-    mode3 = env["OV2_KLT_MODE"] == 3
-    assert ("fb_klt_deferred" in k) == mode3 and ("klt_bucket_kernel" in k) == (mode3 and "OV2_KLT_BUCKET" not in env), k
-
-
-@pytest.mark.parametrize("n", [95, 96, 97])
-@pytest.mark.parametrize("bucket", [1, 0])
-def test_klt_mode3_around_the_switch(ctx, monkeypatch, capfd, klt_set, klt_pyr, n, bucket):
-    """OV2_KLT_MODE=3 with n = 95 (below the n >= 96 switch: one-warp-per-keypoint kernel), 96 (32 full triples, lanes
-    30 - 31 of every warp without a keypoint) and 97 (a partial last triple), on a seeded subset of the set (several
-    frames, all depths)."""
-    _env(monkeypatch, OV2_KLT_MODE=3, OV2_KLT_BUCKET=bucket, OV2_KLT_DEBUG=1)
-    s = klt_set
-    idx = np.sort(np.random.default_rng(n).choice(len(s["kps"]), n, replace=False))
-    assert len(np.unique(s["fidx"][idx])) == 3 and len(np.unique(s["lv"][idx])) == 4
-    capfd.readouterr()
-    with _launches(ctx) as k:
-        got = _track(ctx, *klt_pyr, s["kps"][idx], s["pri"][idx], s["lv"][idx], frame_idx=s["fidx"][idx])
-    _assert_same(got, (s["ref"][0][idx], s["ref"][1][idx]), n)
-    lines = _klt3_lines(capfd)
-    assert ("fb_klt_deferred" in k) == (n >= 96) and len(lines) == (n >= 96), (k, lines)
-    if lines:
-        assert lines[0][0] == n and 0 < lines[0][1] < n, lines
+    _assert_same(got, s["ref"])
+    assert k == {"fb_klt_kernel": 1}, k
 
 
 # ---------------------------------------------------------------- 3. unaligned (device-aliased) level 0
@@ -268,17 +231,16 @@ def unaligned_set():
     return out
 
 
-@pytest.mark.parametrize("mode", [1, 3])
 @pytest.mark.parametrize("src", ["w333", "w334", "roi"])
-def test_klt_unaligned_level0(ctx, monkeypatch, capfd, unaligned_set, src, mode):
+def test_klt_unaligned_level0(ctx, monkeypatch, unaligned_set, src):
     """Pyramids aliasing device images whose level 0 is not word aligned (odd or 2-mod-4 pitch, a column ROI 3 bytes into
     a 352-byte row): the byte / reflected template staging and the plain search gather.  Equal to the oracle and to the
-    same frames tracked from host-built pyramids; in mode 3 every keypoint is deferred at its unaligned level 0."""
+    same frames tracked from host-built pyramids."""
     torch = pytest.importorskip("torch")
     w = 333 if src == "roi" else int(src[1:])
     s = unaligned_set[w]
     nf, h = 2, 245
-    _env(monkeypatch, OV2_KLT_MODE=mode, OV2_KLT_DEBUG=1)
+    _env(monkeypatch)
     hp, hc = _pyramids(ctx, s["prevs"], s["curs"])
     host = _track(ctx, hp, hc, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
     _assert_same(host, s["ref"], "host-built")
@@ -297,14 +259,8 @@ def test_klt_unaligned_level0(ctx, monkeypatch, capfd, unaligned_set, src, mode)
             torch.cuda.synchronize()
             pyr.build(d)
         keep.append(d)
-    capfd.readouterr()
     got = _track(ctx, dp, dc, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
     _assert_same(got, host, "device-aliased vs host-built")
-    lines = _klt3_lines(capfd)
-    if mode == 3:
-        assert lines == [(len(s["kps"]), len(s["kps"]))], lines
-    else:
-        assert lines == [], lines
     for p in (hp, hc, dp, dc):
         p.close()
     del keep
@@ -355,24 +311,16 @@ def high_gradient_set():
     assert high.mean() > 0.75, high.mean()
     ref = _oracle(prevs, curs, kps, pri, lv, fidx)
     assert ref[1].mean() > 0.8
-    return dict(prevs=prevs, curs=curs, kps=kps, pri=pri, lv=lv, fidx=fidx, ref=ref, n_high=int(high.sum()))
+    return dict(prevs=prevs, curs=curs, kps=kps, pri=pri, lv=lv, fidx=fidx, ref=ref)
 
 
-@pytest.mark.parametrize("mode", [1, 3])
-def test_klt_high_gradient_windows(ctx, monkeypatch, capfd, high_gradient_set, mode):
-    """Windows with sum(|Ix| + |Iy|) >= 262 000, where the mismatch sums need the split 64-bit reduction: bit-exact in
-    mode 1, and in mode 3, which defers every such keypoint to the one-warp-per-keypoint kernel."""
-    _env(monkeypatch, OV2_KLT_MODE=mode, OV2_KLT_DEBUG=1)
+def test_klt_high_gradient_windows(ctx, monkeypatch, high_gradient_set):
+    """Windows with sum(|Ix| + |Iy|) >= 262 000, where the mismatch sums need the split 64-bit reduction: bit-exact."""
+    _env(monkeypatch)
     s = high_gradient_set
     pp, cp = _pyramids(ctx, s["prevs"], s["curs"])
-    capfd.readouterr()
     got = _track(ctx, pp, cp, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
     _assert_same(got, s["ref"])
-    lines = _klt3_lines(capfd)
-    if mode == 3:
-        assert len(lines) == 1 and lines[0][0] == len(s["kps"]) and lines[0][1] >= s["n_high"], (lines, s["n_high"])
-    else:
-        assert lines == [], lines
     pp.close()
     cp.close()
 
@@ -409,23 +357,16 @@ def large_batch():
 
 
 def test_klt_large_batch_work_counter(ctx, monkeypatch, large_batch):
-    """12 800 keypoints: 1 600 CTAs of 8 warps (6 400 of 2), more than an H100 holds resident (at most 2 048 threads per
-    SM), so the persistent launches take the global work-counter path.  Default (persistent, 8 warps per CTA), 2 warps
-    per CTA, non-persistent and three-per-warp runs give identical outputs, equal to the oracle on its sample; empty
-    slots get status 0 and keep their prior."""
+    """12 800 keypoints: 1 600 CTAs of 8 warps, more than an H100 holds resident (at most 2 048 threads per SM), so the
+    launch takes the global work-counter path.  Equal to the oracle on its sample; empty slots get status 0 and keep
+    their prior."""
     torch = pytest.importorskip("torch")
     s = large_batch
     n = len(s["kps"])
     assert (n + 7) // 8 > 8 * torch.cuda.get_device_properties(0).multi_processor_count
     pp, cp = _pyramids(ctx, s["prevs"], s["curs"])
-    runs = {}
-    for name, env in (("default", {}), ("wpc2", dict(OV2_KLT_WPC=2)), ("persist0", dict(OV2_KLT_PERSIST=0)),
-                      ("mode3", dict(OV2_KLT_MODE=3))):
-        _env(monkeypatch, **env)
-        runs[name] = _track(ctx, pp, cp, s["kps"], s["pri"], s["lv"], per_frame=s["per"])
-    out, st = runs["default"]
-    for name, r in runs.items():
-        _assert_same(r, runs["default"], name)
+    _env(monkeypatch)
+    out, st = _track(ctx, pp, cp, s["kps"], s["pri"], s["lv"], per_frame=s["per"])
     _assert_same((out[s["idx"]], st[s["idx"]]), s["ref"], "oracle sample")
     assert not st[s["empty"]].any() and np.array_equal(out[s["empty"]], s["pri"][s["empty"]])
     assert st.mean() > 0.5
@@ -456,13 +397,12 @@ def small_sets():
     return out
 
 
-@pytest.mark.parametrize("mode", [1, 3])
 @pytest.mark.parametrize("w,h", SMALL)
-def test_klt_small_images_opencv_depth(ctx, monkeypatch, small_sets, w, h, mode):
+def test_klt_small_images_opencv_depth(ctx, monkeypatch, small_sets, w, h):
     """cv::buildOpticalFlowPyramid stops before a level <= 9 px, and calcOpticalFlowPyrLK / the reference track from the
     depth it reached (17 x 16: 0, 40 x 30: 1, 64 x 48 and 96 x 72: 2, 161 x 83: 3), whatever nbpyrlvl says and however many
     levels the pyramid holds: equal to the oracle (whose statuses equal cv2's)."""
-    _env(monkeypatch, OV2_KLT_MODE=mode)
+    _env(monkeypatch)
     s = small_sets[(w, h)]
     pp, cp = _pyramids(ctx, s["prev"][None], s["cur"][None])
     for key, lv in s["lvs"].items():
@@ -505,10 +445,9 @@ def _edge_check(s, got, kps, pri, lv, frames):
                 _klt_assert(out[m], st[m], s["prevs"][f], s["curs"][f], kps[m], pri[m], 9, int(lvl), min_frac=0.9)
 
 
-@pytest.mark.parametrize("mode", [1, 3])
-def test_klt_edge_inputs_first_frame(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs, mode):
+def test_klt_edge_inputs_first_frame(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs):
     """Fixed-stride addressing from first_frame = 1 with per_frame = 120 (frames 1 and 2 of a 3-frame pyramid)."""
-    _env(monkeypatch, OV2_KLT_MODE=mode)
+    _env(monkeypatch)
     e = edge_inputs
     kps, pri, lv = np.concatenate([e["kps"]] * 2), np.concatenate([e["pri"]] * 2), np.concatenate([e["lv"]] * 2)
     got = _track(ctx, *klt_pyr, kps, pri, lv, first_frame=1, per_frame=120)
@@ -516,10 +455,9 @@ def test_klt_edge_inputs_first_frame(ctx, monkeypatch, klt_set, klt_pyr, edge_in
     _edge_check(s, got, kps, pri, lv, np.repeat(np.array([1, 2]), 120))
 
 
-@pytest.mark.parametrize("mode", [1, 3])
-def test_klt_edge_inputs_ragged_frames(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs, mode):
+def test_klt_edge_inputs_ragged_frames(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs):
     """A ragged, non-monotonic frame_idx (2, 0, 1, 0, 2, ...)."""
-    _env(monkeypatch, OV2_KLT_MODE=mode)
+    _env(monkeypatch)
     e = edge_inputs
     fidx = np.random.default_rng(4).integers(0, 3, 120).astype(np.int32)
     fidx[:5] = [2, 0, 1, 0, 2]
