@@ -16,15 +16,15 @@
 //                       On an H100 SXM (700 W limit) the three-way VIMNMX3 issues at half the rate
 //                       of a two-way VIMNMX (1.7 vs 3.5 warp instructions / clock / SM), so the
 //                       count that matters is two-way-equivalent min/max per pixel pair (~96).
-//   fast_sweep_kernel   (F2, one warp per frame)  the order-dependent part: occupancy, mask discs
-//                       (cv::circle midpoint rasterisation) kept as a 1-bit/pixel bitmap in shared
-//                       memory, per-cell mask filter -> libstdc++ std::sort top-1 -> response >= 20
-//                       -> paint disc; adaptive nfast_th_ update (:546-552).
+//   fast_sweep_kernel   (F2, one CTA per frame, one warp per cell row: the wavefront of grid_sweep.cuh)  the
+//                       order-dependent part: occupancy, mask discs (cv::circle midpoint rasterisation) kept as
+//                       a 1-bit/pixel bitmap in shared memory, per-cell mask filter -> libstdc++ std::sort
+//                       top-1 -> response >= 20 -> paint disc; adaptive nfast_th_ update (:546-552).
 //   subpix_kernel       (S, one warp per point)  cv::cornerSubPix((3,3),(-1,-1),{30,0.01}).
 //
 // All integer work is bit-exact; S is float32/float64 with OpenCV's operation grouping
 // (compiled with -fmad=false; the one FMA OpenCV uses is spelled __fmaf_rn).
-#include "ov2_common.cuh"
+#include "grid_sweep.cuh"
 #include "stdsort_emul.h"
 
 #include <cuda.h>   // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
@@ -36,7 +36,6 @@ namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int MAX_CELL = 128;
-constexpr int MAX_RADIUS = MAX_CELL / 4;
 
 // Largest number of candidates a cell of size cs can hold.  A candidate lies in the interior [3, cs - 3)^2 at cell-local
 // x % 4 in {2, 3} and is a strict 3x3 maximum.  The nk = (cs - 6) / 4 + 1 column groups {4k + 2, 4k + 3} that meet the
@@ -286,192 +285,46 @@ __global__ void fast_cells_kernel(FastArgs A, const __grid_constant__ CUtensorMa
 // Sort keys are (response << 16) | candidate index (stdsort_emul.h).
 constexpr int SKEY_SHIFT = 16;
 constexpr int SKEY_IDX = (1 << SKEY_SHIFT) - 1;
-// fast_sweep_wave_kernel holds up to WAVE_REG_CAND candidates of a cell in registers (four per lane) and their sort keys in
+// fast_sweep_kernel holds up to WAVE_REG_CAND candidates of a cell in registers (four per lane) and their sort keys in
 // shared memory; a cell with more candidates reads them from the list and sorts in a global area (SweepArgs::skey_g).
 constexpr int WAVE_REG_CAND = 128;
 
-struct SweepArgs {
-    int w, h, cs, nwc, nhc, cap, radius, max_per_frame;
-    int* skey_g;                     // wave kernel: [count][warps][cap] sort keys of cells with > WAVE_REG_CAND candidates
-    int hw[MAX_RADIUS + 1];          // cv::circle half-widths per |dy|
-    const int32_t* kp_off;           // [count+1] or NULL
-    const float2* kps;               // existing keypoints
+struct SweepArgs : gsweep::SweepBase {
+    int cap, max_per_frame;
+    int* skey_g;                     // [count][warps][cap] sort keys of cells with > WAVE_REG_CAND candidates
     const uint32_t* cand; const int32_t* cand_n;
     int32_t* th;                     // in/out per frame
     int2* out_int;                   // [count][max_per_frame]
     int32_t* out_n;                  // [count]
 };
 
-__device__ __forceinline__ void paint_row(uint32_t* bm, int wpr, int W, int H, int y, int xa, int xb) {
-    if (y < 0 || y >= H) return;
-    xa = max(xa, 0);
-    xb = min(xb, W - 1);
-    if (xa > xb) return;
-    uint32_t* row = bm + (size_t)y * wpr;
-    int wa = xa >> 5, wb = xb >> 5;
-    for (int wi = wa; wi <= wb; ++wi) {
-        uint32_t m = 0xffffffffu;
-        if (wi == wa) m &= 0xffffffffu << (xa & 31);
-        if (wi == wb) m &= 0xffffffffu >> (31 - (xb & 31));
-        atomicOr(row + wi, m);
-    }
+// Shared-memory layout of fast_sweep_kernel: min(cap, WAVE_REG_CAND) sort keys per warp between the bitmap and the counters.
+constexpr int FSWEEP_MAX_WARPS = 16;
+__host__ __device__ inline gsweep::SweepSmem fast_sweep_smem(int w, int h, int nwc, int nhc, int cap, int nwarps) {
+    return gsweep::SweepSmem(w, h, nwc, nhc, nwarps, nwarps * min(cap, WAVE_REG_CAND) * 4, alignof(int));
 }
 
-__global__ void __launch_bounds__(32) fast_sweep_kernel(SweepArgs A) {
-    extern __shared__ uint32_t sm[];
-    const int lane = threadIdx.x, fr = blockIdx.x;
-    const int wpr = (A.w + 31) >> 5;
-    uint32_t* bm = sm;                                  // h * wpr words, bit = 1: mask is 0.0f there
-    int* skey = (int*)(sm + (size_t)A.h * wpr);         // cap sort keys
-    uint8_t* occ = (uint8_t*)(skey + A.cap);            // (nhc+1)*(nwc+1)
-    for (int i = lane; i < A.h * wpr; i += 32) bm[i] = 0;
-    const int nocc = (A.nhc + 1) * (A.nwc + 1);
-    for (int i = lane; i < nocc; i += 32) occ[i] = 0;
-    __syncwarp();
-    // existing keypoints: occupancy + discs (feature_extractor.cpp:471-474)
-    if (A.kp_off) {
-        const int k0 = A.kp_off[fr], k1 = A.kp_off[fr + 1];
-        const int nrows = 2 * A.radius + 1;
-        for (int k = k0; k < k1; ++k) {
-            float2 px = A.kps[k];
-            if (lane == 0) {
-                int rr = (int)(px.y / (float)A.cs), cc = (int)(px.x / (float)A.cs);
-                if (rr >= 0 && rr <= A.nhc && cc >= 0 && cc <= A.nwc) occ[rr * (A.nwc + 1) + cc] = 1;
-            }
-            int cx = __float2int_rn(px.x), cy = __float2int_rn(px.y);
-            for (int rI = lane; rI < nrows; rI += 32) {
-                int dy = rI - A.radius;
-                int hwv = A.hw[dy < 0 ? -dy : dy];
-                paint_row(bm, wpr, A.w, A.h, cy + dy, cx - hwv, cx + hwv);
-            }
-        }
-    }
-    __syncwarp();
+// The wavefront sweep of grid_sweep.cuh, one warp per cell row: exactly the sequential result in nwc + 2 nhc cell times
+// instead of nwc * nhc (pure latency; 0.070 ms, 3.5 % of the C2 step, on an H100 SXM at 700 W).  As many warps as the
+// shared memory allows, up to one per cell row (at most FSWEEP_MAX_WARPS).  Cell c's detection goes to slot c of the
+// frame's output (max_per_frame >= ncells), and the slots are compacted in cell order at the end.
+__global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_kernel(SweepArgs A) {
+    extern __shared__ __align__(16) uint8_t sm[];
+    const int tid = threadIdx.x, fr = blockIdx.x, nthreads = blockDim.x;
+    const int lane = tid & 31, warp = tid >> 5, nwarps = nthreads >> 5;
     const int ncells = A.nwc * A.nhc;
+    const gsweep::SweepSmem L = fast_sweep_smem(A.w, A.h, A.nwc, A.nhc, A.cap, nwarps);
+    const int wpr = L.wpr;
+    uint32_t* bm = reinterpret_cast<uint32_t*>(sm);
+    const int nskey = min(A.cap, WAVE_REG_CAND);
+    int* skey_sm = reinterpret_cast<int*>(sm + L.mid) + warp * nskey;
+    volatile int* progress = gsweep::progress_counters(L, sm);
+    const uint8_t* occ = sm + L.occ;
+    int* skey_big = A.skey_g ? A.skey_g + ((size_t)fr * nwarps + warp) * A.cap : nullptr;
+    gsweep::init_mask(A, L, sm, fr);
     const uint32_t* cand = A.cand + (size_t)fr * ncells * A.cap;
     const int32_t* cand_n = A.cand_n + (size_t)fr * ncells;
     int2* out = A.out_int + (size_t)fr * A.max_per_frame;
-    int nbkps = 0, nbempty = 0;
-    for (int cell = 0; cell < ncells; ++cell) {
-        const int r = cell / A.nwc, c = cell - r * A.nwc;
-        if (occ[r * (A.nwc + 1) + c]) continue;
-        nbempty++;
-        const int x0 = c * A.cs, y0 = r * A.cs;
-        if (!(x0 + A.cs < A.w - 1 && y0 + A.cs < A.h - 1)) continue;
-        const int n = cand_n[cell];
-        if (n == 0) continue;
-        // mask filter + ordered compaction of survivors into skey
-        int ns = 0, vmax = -1;
-        for (int base = 0; base < n; base += 32) {
-            int j = base + lane;
-            bool ok = false;
-            uint32_t cd = 0;
-            if (j < n) {
-                cd = cand[(size_t)cell * A.cap + j];
-                int kx = cd & 255, ky = (cd >> 8) & 255;
-                int mx = x0 + (kx >> 2), my = y0 + ky;
-                ok = ((bm[(size_t)my * wpr + (mx >> 5)] >> (mx & 31)) & 1u) == 0;
-            }
-            unsigned m = __ballot_sync(FULL, ok);
-            if (ok) {
-                int pos = ns + __popc(m & ((1u << lane) - 1));
-                skey[pos] = (int)((cd >> 16) << SKEY_SHIFT) | j;   // (response << 16) | candidate index
-                vmax = max(vmax, (int)(cd >> 16));
-            }
-            ns += __popc(m);
-        }
-        if (ns == 0) continue;
-        vmax = __reduce_max_sync(FULL, vmax);
-        __syncwarp();
-        // number of survivors sharing the maximal response, and the first of them in scan order
-        int nmax = 0, firstmax = 0x7fffffff;
-        for (int base = 0; base < ns; base += 32) {
-            int j = base + lane;
-            bool is = j < ns && (skey[j] >> SKEY_SHIFT) == vmax;
-            unsigned m = __ballot_sync(FULL, is);
-            if (m && firstmax == 0x7fffffff) firstmax = base + __ffs(m) - 1;
-            nmax += __popc(m);
-        }
-        int win_j;
-        if (nmax == 1 || ns <= 16) {
-            // unique maximum, or libstdc++ falls straight to (stable) insertion sort
-            win_j = skey[firstmax] & SKEY_IDX;
-        } else {
-            if (lane == 0) ov2sort::sort_desc_front(skey, ns);     // only skey[0] is read
-            __syncwarp();
-            win_j = skey[0] & SKEY_IDX;
-        }
-        __syncwarp();
-        if (vmax >= 20) {   // vkps.at(0).response >= 20
-            uint32_t cd = cand[(size_t)cell * A.cap + win_j];
-            int px = x0 + (int)(cd & 255), py = y0 + (int)((cd >> 8) & 255);
-            if (lane == 0 && nbkps < A.max_per_frame) out[nbkps] = make_int2(px, py);
-            nbkps++;
-            const int nrows = 2 * A.radius + 1;
-            for (int rI = lane; rI < nrows; rI += 32) {
-                int dy = rI - A.radius;
-                int hwv = A.hw[dy < 0 ? -dy : dy];
-                paint_row(bm, wpr, A.w, A.h, py + dy, px - hwv, px + hwv);
-            }
-            __syncwarp();
-        }
-    }
-    for (int i = nbkps + lane; i < A.max_per_frame; i += 32) out[i] = make_int2(-1, -1);
-    if (lane == 0) {
-        A.out_n[fr] = nbkps;
-        int th = A.th[fr];
-        if ((double)nbkps < 0.5 * (double)nbempty && nbempty > 10) th = (int)((double)th * 0.66);
-        else if (nbkps == nbempty) th = (int)((double)th * 1.5);
-        A.th[fr] = th;
-    }
-}
-
-// Wavefront variant: the sequential cell order is the semantics, but a cell only reads mask bits of its own area, and a disc
-// (radius cs / 4) reaches no further than the neighbouring cells - so cell (r, c) needs (r, c-1), (r-1, c-1), (r-1, c) and
-// (r-1, c+1) finished, nothing else.  One warp per cell row, row r trailing row r-1 by two cells (as ss_sweep_kernel does):
-// exactly the sequential result in nwc + 2 nhc cell times instead of nwc * nhc (pure latency; 0.070 ms, 3.5 % of the C2 step,
-// on an H100 SXM at 700 W).  Detections are kept per cell and put in cell order at the end.
-constexpr int FSWEEP_MAX_WARPS = 16;
-
-__global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kernel(SweepArgs A) {
-    extern __shared__ uint32_t sm[];
-    __shared__ int s_cnt[2];
-    const int tid = threadIdx.x, fr = blockIdx.x, nthreads = blockDim.x;
-    const int lane = tid & 31, warp = tid >> 5, nwarps = nthreads >> 5;
-    const int wpr = (A.w + 31) >> 5, ncells = A.nwc * A.nhc;
-    uint32_t* bm = sm;                                                        // h * wpr words, bit = 1: mask is 0.0f there
-    int2* det = reinterpret_cast<int2*>(sm + (((size_t)A.h * wpr + 1) & ~(size_t)1));   // per cell, x < 0: none
-    const int nskey = min(A.cap, WAVE_REG_CAND);
-    int* skey_all = reinterpret_cast<int*>(det + ncells);                    // [nwarps][nskey] sort keys
-    volatile int* progress = reinterpret_cast<volatile int*>(skey_all + (size_t)nwarps * nskey);   // [nhc]
-    uint8_t* occ = reinterpret_cast<uint8_t*>(const_cast<int*>(progress) + A.nhc);       // (nhc+1)*(nwc+1)
-    int* skey_sm = skey_all + (size_t)warp * nskey;
-    int* skey_big = A.skey_g ? A.skey_g + ((size_t)fr * nwarps + warp) * A.cap : nullptr;
-    for (int i = tid; i < A.h * wpr; i += nthreads) bm[i] = 0;
-    for (int i = tid; i < ncells; i += nthreads) det[i] = make_int2(-1, -1);
-    for (int i = tid; i < A.nhc; i += nthreads) progress[i] = 0;
-    const int nocc = (A.nhc + 1) * (A.nwc + 1);
-    for (int i = tid; i < nocc; i += nthreads) occ[i] = 0;
-    __syncthreads();
-    const int nrows = 2 * A.radius + 1;
-    // existing keypoints: occupancy + discs (feature_extractor.cpp:471-474); painting commutes (atomicOr)
-    if (A.kp_off) {
-        const int k0 = A.kp_off[fr], k1 = A.kp_off[fr + 1];
-        for (int k = k0 + tid; k < k1; k += nthreads) {
-            const float2 px = A.kps[k];
-            const int rr = (int)(px.y / (float)A.cs), cc = (int)(px.x / (float)A.cs);
-            if (rr >= 0 && rr <= A.nhc && cc >= 0 && cc <= A.nwc) occ[rr * (A.nwc + 1) + cc] = 1;
-            const int cx = __float2int_rn(px.x), cy = __float2int_rn(px.y);
-            for (int rI = 0; rI < nrows; ++rI) {
-                const int dy = rI - A.radius;
-                const int hwv = A.hw[dy < 0 ? -dy : dy];
-                paint_row(bm, wpr, A.w, A.h, cy + dy, cx - hwv, cx + hwv);
-            }
-        }
-    }
-    __syncthreads();
-    const uint32_t* cand = A.cand + (size_t)fr * ncells * A.cap;
-    const int32_t* cand_n = A.cand_n + (size_t)fr * ncells;
     // A cell's candidates do not depend on any other cell, and the row's cell-to-cell chain is what the frame waits for: the
     // count and the first WAVE_REG_CAND candidates of cell c + 2 are requested (five independent loads; the list's slots past
     // the count are allocated, and dropped below) before cell c is worked on, so no global-memory latency is left in the chain.
@@ -501,11 +354,8 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
             uint32_t cdv[4];                                                   // the first WAVE_REG_CAND: four per lane
 #pragma unroll
             for (int q = 0; q < 4; ++q) cdv[q] = 32 * q + lane < n ? cur.v[q] : 0u;
-            if (r > 0) {
-                const int need = min(c + 2, A.nwc);                            // row r-1 has finished cell c+1 (or its last cell)
-                while (progress[r - 1] < need) __nanosleep(40);
-                __threadfence_block();
-            }
+            gsweep::wave_wait(progress, nwarps, r, c, A.nwc);
+            int2 det = make_int2(-1, -1);
             if (n > 0) {
                 // mask filter + ordered compaction of survivors into skey (shared memory, or the global area for big cells)
                 const bool big = n > WAVE_REG_CAND;                            // uniform
@@ -559,56 +409,48 @@ __global__ void __launch_bounds__(FSWEEP_MAX_WARPS * 32, 1) fast_sweep_wave_kern
                         const int wq = win_j >> 5;                              // uniform
                         const uint32_t mine = wq == 0 ? cdv[0] : (wq == 1 ? cdv[1] : (wq == 2 ? cdv[2] : cdv[3]));
                         const uint32_t cd = win_j < WAVE_REG_CAND ? __shfl_sync(FULL, mine, win_j & 31) : __ldg(ccand + win_j);
-                        const int px = x0 + (int)(cd & 255), py = y0 + (int)((cd >> 8) & 255);
-                        if (lane == 0) det[cell] = make_int2(px, py);
-                        for (int rI = lane; rI < nrows; rI += 32) {
-                            const int dy = rI - A.radius;
-                            const int hwv = A.hw[dy < 0 ? -dy : dy];
-                            paint_row(bm, wpr, A.w, A.h, py + dy, px - hwv, px + hwv);
-                        }
+                        det = make_int2(x0 + (int)(cd & 255), y0 + (int)((cd >> 8) & 255));
+                        gsweep::paint_disc(A, bm, wpr, det.x, det.y, lane, 32);
                         __syncwarp();
                     }
                 }
             }
-            __threadfence_block();                                            // discs before the counter
-            __syncwarp();
-            if (lane == 0) progress[r] = c + 1;
+            if (lane == 0) out[cell] = det;
+            gsweep::wave_publish(progress, nwarps, r, c, lane);
         }
     }
     __syncthreads();
-    // assembly in cell order + the adaptive threshold (feature_extractor.cpp:546-552)
-    int2* out = A.out_int + (size_t)fr * A.max_per_frame;
+    // compaction in cell order + the adaptive threshold (feature_extractor.cpp:546-552).  A detection only moves left, so
+    // each round reads its 128 slots (four loads in flight, one L2 latency) before it writes any of them.
     if (warp == 0) {
         int nbkps = 0, nbempty = 0;
-        for (int base = 0; base < ncells; base += 32) {
-            const int cell = base + lane;
-            bool empty = false, has = false;
-            int2 d = make_int2(-1, -1);
-            if (cell < ncells) {
+        for (int base = 0; base < ncells; base += 128) {
+            int2 d[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int cell = base + 32 * q + lane;
+                d[q] = cell < ncells ? out[cell] : make_int2(-1, -1);
+            }
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int cell = base + 32 * q + lane;
                 const int r = cell / A.nwc, c = cell - r * A.nwc;
-                empty = !occ[r * (A.nwc + 1) + c];
-                d = det[cell];
-                has = d.x >= 0;
+                const bool empty = cell < ncells && !occ[r * (A.nwc + 1) + c], has = d[q].x >= 0;
+                const unsigned mh = __ballot_sync(FULL, has);
+                if (has) out[nbkps + __popc(mh & ((1u << lane) - 1))] = d[q];
+                nbkps += __popc(mh);
+                nbempty += __popc(__ballot_sync(FULL, empty));
             }
-            const unsigned mh = __ballot_sync(FULL, has);
-            if (has) {
-                const int pos = nbkps + __popc(mh & ((1u << lane) - 1));
-                if (pos < A.max_per_frame) out[pos] = d;
-            }
-            nbkps += __popc(mh);
-            nbempty += __popc(__ballot_sync(FULL, empty));
         }
+        for (int i = nbkps + lane; i < A.max_per_frame; i += 32) out[i] = make_int2(-1, -1);
         if (lane == 0) {
             A.out_n[fr] = nbkps;
             int th = A.th[fr];
             if ((double)nbkps < 0.5 * (double)nbempty && nbempty > 10) th = (int)((double)th * 0.66);
             else if (nbkps == nbempty) th = (int)((double)th * 1.5);
             A.th[fr] = th;
-            s_cnt[0] = nbkps;
         }
     }
-    __syncthreads();
-    for (int i = s_cnt[0] + tid; i < A.max_per_frame; i += nthreads) out[i] = make_int2(-1, -1);
 }
 
 // ---------------------------------------------------------------------------------- S
@@ -781,23 +623,6 @@ void subpix_mask(float* mask) {
     }
 }
 
-// OpenCV's filled-circle rasterisation (midpoint algorithm): half-width per |dy|
-void circle_halfwidths(int radius, int* hw) {
-    for (int i = 0; i <= radius; ++i) hw[i] = -1;
-    int err = 0, dx = radius, dy = 0, plus = 1, minus = (radius << 1) - 1;
-    while (dx >= dy) {
-        if (dx > hw[dy]) hw[dy] = dx;
-        if (dy > hw[dx]) hw[dx] = dy;
-        dy++;
-        err += plus;
-        plus += 2;
-        int mask = (err <= 0) - 1;
-        err -= minus & mask;
-        dx += mask;
-        minus -= mask & 2;
-    }
-}
-
 }  // namespace
 
 // Host side of the TMA staging: a 3-D tiled tensor map {W, H, frames} over the level-0 images, box
@@ -868,69 +693,27 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     if (ncells == 0 || max_per_frame < ncells)
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_grid_fast: max_per_frame < number of cells");
     const int cap = fast_cell_cap(cellsize);
-    // sweep: the wavefront kernel (one warp per cell row) unless its shared memory (mask bitmap, per-cell detections, per-warp
-    // sort keys, row progress, occupancy; the carve-up at the top of fast_sweep_wave_kernel) is over 200 KB or
-    // OV2_FAST_SWEEP=seq; else one warp per frame, which needs the bitmap, cap sort keys and the occupancy
-    const size_t wpr = (size_t)(W + 31) / 32;
-    const int nw = nhc < FSWEEP_MAX_WARPS ? nhc : FSWEEP_MAX_WARPS;
-    const int nskey = cap < WAVE_REG_CAND ? cap : WAVE_REG_CAND;
-    size_t wsmem = ((((size_t)H * wpr + 1) & ~(size_t)1)) * 4 + (size_t)nwc * nhc * 8 + (size_t)nw * nskey * 4 + (size_t)nhc * 4 +
-                   (size_t)(nhc + 1) * (nwc + 1);
-    wsmem = (wsmem + 15) & ~(size_t)15;
-    size_t smem = (size_t)H * wpr * 4 + (size_t)cap * 4 + (size_t)(nhc + 1) * (nwc + 1);
-    smem = (smem + 15) & ~(size_t)15;
-    const char* fs = getenv("OV2_FAST_SWEEP");
-    const bool wave = wsmem <= 200 * 1024 && !(fs && fs[0] == 's');
-    if (!wave && smem > 227 * 1024)
+    // sweep warps: one per cell row, up to FSWEEP_MAX_WARPS, as many as fit the shared memory
+    int nw = nhc < FSWEEP_MAX_WARPS ? nhc : FSWEEP_MAX_WARPS;
+    while (nw > 1 && fast_sweep_smem(W, H, nwc, nhc, cap, nw).bytes > gsweep::SMEM_LIMIT) --nw;
+    const size_t smem = fast_sweep_smem(W, H, nwc, nhc, cap, nw).bytes;
+    if (smem > gsweep::SMEM_LIMIT)
         return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_grid_fast: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-
-    const void* d = nullptr;
+    DetectArgs D;
+    if ((st = stage_detect_args(ctx, "ov2_grid_fast", count, max_per_frame, curkp_offsets, curkps, fast_th_inout, sizeof(int32_t),
+                                out_pts, out_counts, out_pts_int, &D)) != OV2_OK)
+        return st;
     void* o = nullptr;
-    int nkp_total = 0;
-    const int32_t* d_off = nullptr;
-    const float2* d_kps = nullptr;
-    if (curkp_offsets) {
-        if ((st = ov2_stage_in(ctx, curkp_offsets, sizeof(int32_t) * (size_t)(count + 1), &d)) != OV2_OK) return st;
-        d_off = (const int32_t*)d;
-        // number of keypoints: need offsets[count] on the host
-        if (ov2_is_device_ptr(curkp_offsets)) {
-            OV2_CUDA(ctx, cudaMemcpyAsync(&nkp_total, curkp_offsets + count, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-            OV2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        } else {
-            nkp_total = curkp_offsets[count];
-        }
-        if (nkp_total > 0) {
-            if (!curkps) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_grid_fast: curkps is NULL");
-            if ((st = ov2_stage_in(ctx, curkps, sizeof(float) * 2 * (size_t)nkp_total, &d)) != OV2_OK) return st;
-            d_kps = (const float2*)d;
-        }
-    }
-    int32_t* d_th = nullptr;
-    if ((st = ov2_stage_out(ctx, fast_th_inout, sizeof(int32_t) * (size_t)count, &o, true)) != OV2_OK) return st;
-    d_th = (int32_t*)o;
-    float2* d_out = nullptr;
-    if ((st = ov2_stage_out(ctx, out_pts, sizeof(float) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    d_out = (float2*)o;
-    int32_t* d_cnt = nullptr;
-    if ((st = ov2_stage_out(ctx, out_counts, sizeof(int32_t) * (size_t)count, &o)) != OV2_OK) return st;
-    d_cnt = (int32_t*)o;
-    int2* d_int = nullptr;
-    if (out_pts_int) {
-        if ((st = ov2_stage_out(ctx, out_pts_int, sizeof(int32_t) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    } else {
-        if ((st = ov2_scratch(ctx, sizeof(int32_t) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    }
-    d_int = (int2*)o;
     uint32_t* d_cand = nullptr;
     int32_t* d_candn = nullptr;
     if ((st = ov2_scratch(ctx, sizeof(uint32_t) * (size_t)count * ncells * cap, &o)) != OV2_OK) return st;
     d_cand = (uint32_t*)o;
     if ((st = ov2_scratch(ctx, sizeof(int32_t) * (size_t)count * ncells, &o)) != OV2_OK) return st;
     d_candn = (int32_t*)o;
-    int* d_skey = nullptr;      // sort keys of the wave kernel's cells with more candidates than it keeps in registers
-    if (wave && cap > WAVE_REG_CAND) {
+    int* d_skey = nullptr;      // sort keys of the cells with more candidates than the sweep keeps in registers
+    if (cap > WAVE_REG_CAND) {
         if ((st = ov2_scratch(ctx, sizeof(int) * (size_t)count * nw * cap, &o)) != OV2_OK) return st;
         d_skey = (int*)o;
     }
@@ -938,34 +721,19 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
     FastArgs FA;
     FA.img = pyr->l0; FA.w = W; FA.h = H; FA.pitch = (int)pyr->l0_pitch; FA.fstride = (long long)pyr->l0_fstride;
     FA.first = first; FA.cs = cellsize; FA.nwc = nwc; FA.nhc = nhc; FA.cap = cap;
-    FA.th = d_th; FA.cand = d_cand; FA.cand_n = d_candn;
+    FA.th = (int32_t*)D.state; FA.cand = d_cand; FA.cand_n = d_candn;
     if ((st = launch_fast_cells(ctx, pyr, FA, count)) != OV2_OK) return st;
     SweepArgs SA;
-    SA.w = W; SA.h = H; SA.cs = cellsize; SA.nwc = nwc; SA.nhc = nhc; SA.cap = cap;
-    SA.radius = cellsize / 4; SA.max_per_frame = max_per_frame;
-    SA.skey_g = d_skey;
-    circle_halfwidths(SA.radius, SA.hw);
-    SA.kp_off = d_off; SA.kps = d_kps; SA.cand = d_cand; SA.cand_n = d_candn; SA.th = d_th;
-    SA.out_int = d_int; SA.out_n = d_cnt;
-    if (wave) {
-        static size_t wave_attr[16] = {0};
-        if (wsmem > 48 * 1024 && wsmem > wave_attr[ctx->device & 15]) {
-            OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-            wave_attr[ctx->device & 15] = wsmem;
-        }
-        OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_wave_kernel<<<count, nw * 32, wsmem, ctx->stream>>>(SA));
-    } else {
-        if (smem > 48 * 1024)
-            OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_kernel<<<count, 32, smem, ctx->stream>>>(SA));
+    gsweep::init_base(SA, W, H, cellsize, D.kp_off, D.kps);
+    SA.cap = cap; SA.max_per_frame = max_per_frame; SA.skey_g = d_skey;
+    SA.cand = d_cand; SA.cand_n = d_candn; SA.th = (int32_t*)D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
+    static size_t smem_attr[16] = {0};
+    if (smem > 48 * 1024 && smem > smem_attr[ctx->device & 15]) {
+        OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        smem_attr[ctx->device & 15] = smem;
     }
-    SubpixArgs PA;
-    PA.img = pyr->l0; PA.w = W; PA.h = H; PA.pitch = (int)pyr->l0_pitch; PA.fstride = (long long)pyr->l0_fstride;
-    PA.first = first; PA.max_per_frame = max_per_frame; PA.n = count * max_per_frame;
-    PA.in_int = d_int; PA.out = d_out; PA.do_subpix = do_subpix;
-    PA.iters = nullptr;
-    subpix_mask(PA.mask);
-    OV2_LAUNCH(ctx, "subpix_kernel", subpix_kernel<false><<<div_up(PA.n, 4), 128, 0, ctx->stream>>>(PA));
+    OV2_LAUNCH(ctx, "fast_sweep_kernel", fast_sweep_kernel<<<count, nw * 32, smem, ctx->stream>>>(SA));
+    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, D.ints, D.out, do_subpix, nullptr)) != OV2_OK) return st;
     return ov2_end(ctx);
 }
 
@@ -1003,8 +771,6 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
     return ov2_end(ctx);
 }
 
-// Internal (not part of the C ABI): cornerSubPix stage S on integer points produced by another detector
-// (frontend_sscale.cu).  Same launch as inside ov2_grid_fast; slots holding (-1, -1) stay empty.
 ov2_status ov2_subpix_launch(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame, const int2* d_int,
                              float2* d_out, int do_subpix, int32_t* d_iters) {
     SubpixArgs PA;

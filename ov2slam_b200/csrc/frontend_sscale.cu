@@ -16,16 +16,13 @@
 // to HBM: 4 B/pixel written once, read at most twice) and ss_sweep_kernel (one CTA per frame, one warp per cell row in a
 // wavefront that reproduces the sequential cell order, 1 bit/pixel mask in shared memory).
 #include "ov2_common.cuh"
+#include "grid_sweep.cuh"
 #include "sscale_math.cuh"
-
-ov2_status ov2_subpix_launch(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int max_per_frame, const int2* d_int,
-                             float2* d_out, int do_subpix, int32_t* d_iters);   // frontend_fast.cu
 
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int SS_MAX_CELL = 64;
-constexpr int SS_MAX_RADIUS = SS_MAX_CELL / 4;
 
 struct RespArgs {
     const uint8_t* img; int w, h, pitch; long long fstride;
@@ -83,33 +80,15 @@ __global__ void __launch_bounds__(256) ss_response_kernel(RespArgs A) {
     }
 }
 
-struct SweepArgs {
-    int w, h, cs, nwc, nhc, radius, max_per_frame;
-    int hw[SS_MAX_RADIUS + 1];       // cv::circle half-widths per |dy|
+struct SweepArgs : gsweep::SweepBase {
+    int max_per_frame;
     int roi_x, roi_y, roi_w, roi_h;
-    const int32_t* kp_off;           // [count+1] or NULL
-    const float2* kps;
     const float* resp;               // [count][ncells][cs*cs]
     const float2* cellmax;           // [count][ncells] first maximum per cell (value, index bits)
     double* quality;                 // in/out per frame
     int2* out_int;                   // [count][max_per_frame]
     int32_t* out_n;                  // [count]
 };
-
-__device__ __forceinline__ void paint_row(uint32_t* bm, int wpr, int W, int H, int y, int xa, int xb) {
-    if (y < 0 || y >= H) return;
-    xa = max(xa, 0);
-    xb = min(xb, W - 1);
-    if (xa > xb) return;
-    uint32_t* row = bm + (size_t)y * wpr;
-    const int wa = xa >> 5, wb = xb >> 5;
-    for (int wi = wa; wi <= wb; ++wi) {
-        uint32_t m = 0xffffffffu;
-        if (wi == wa) m &= 0xffffffffu << (xa & 31);
-        if (wi == wb) m &= 0xffffffffu >> (31 - (xb & 31));
-        atomicOr(row + wi, m);
-    }
-}
 
 constexpr int SWEEP_MAX_WARPS = 32;
 
@@ -138,46 +117,27 @@ __device__ __forceinline__ void cell_argmax_warp(const float* __restrict__ resp,
     best_v = bv; best_i = bi;
 }
 
-// The reference walks the cells in row-major order and every detection paints a disc of radius cs / 4 into the mask, so a
-// cell depends on the cells before it - but a disc reaches at most cs / 4 pixels into the NEIGHBOURING cells.  Cell (r, c)
-// therefore only needs (r, c-1), (r-1, c-1), (r-1, c) and (r-1, c+1) to be finished: one WARP per cell row, row r trailing
-// row r-1 by two cells (wavefront), gives exactly the sequential result in (nwc + 2 nhc) cell times instead of nwc * nhc.
-// progress[r] = number of cells of row r that are finished (volatile shared memory; discs are painted with shared atomics
-// before the counter moves).
+// Shared-memory layout of ss_sweep_kernel: two detections per cell (int2, x < 0: none) between the bitmap and the counters.
+__host__ __device__ inline gsweep::SweepSmem ss_sweep_smem(int w, int h, int nwc, int nhc, int nwarps) {
+    return gsweep::SweepSmem(w, h, nwc, nhc, nwarps, (gsweep::SweepSmem::off)nwc * nhc * 2 * sizeof(int2), alignof(int2));
+}
+
+// The wavefront sweep of grid_sweep.cuh, one warp per cell row.
 __global__ void __launch_bounds__(SWEEP_MAX_WARPS * 32, 1) ss_sweep_kernel(SweepArgs A) {
-    extern __shared__ uint32_t sm[];
+    extern __shared__ __align__(16) uint8_t sm[];
     __shared__ int s_n;
     const int tid = threadIdx.x, fr = blockIdx.x, nthreads = blockDim.x;
     const int lane = tid & 31, warp = tid >> 5, nwarps = nthreads >> 5;
-    const int wpr = (A.w + 31) >> 5, ncells = A.nwc * A.nhc, cs = A.cs;
-    uint32_t* bm = sm;                                            // h * wpr words, bit = 1: mask is 0.0f there
-    int2* firstd = reinterpret_cast<int2*>(sm + (((size_t)A.h * wpr + 1) & ~(size_t)1));   // per cell, x < 0: none (8-byte aligned)
+    const int ncells = A.nwc * A.nhc, cs = A.cs;
+    const gsweep::SweepSmem L = ss_sweep_smem(A.w, A.h, A.nwc, A.nhc, nwarps);
+    const int wpr = L.wpr;
+    uint32_t* bm = reinterpret_cast<uint32_t*>(sm);
+    int2* firstd = reinterpret_cast<int2*>(sm + L.mid);
     int2* secondd = firstd + ncells;
-    volatile int* progress = reinterpret_cast<volatile int*>(secondd + ncells);             // [nhc]
-    uint8_t* occ = reinterpret_cast<uint8_t*>(const_cast<int*>(progress) + A.nhc);          // (nhc+1)*(nwc+1)
-    for (int i = tid; i < A.h * wpr; i += nthreads) bm[i] = 0;
+    volatile int* progress = gsweep::progress_counters(L, sm);
+    const uint8_t* occ = sm + L.occ;
     for (int i = tid; i < ncells; i += nthreads) { firstd[i] = make_int2(-1, -1); secondd[i] = make_int2(-1, -1); }
-    for (int i = tid; i < A.nhc; i += nthreads) progress[i] = 0;
-    const int nocc = (A.nhc + 1) * (A.nwc + 1);
-    for (int i = tid; i < nocc; i += nthreads) occ[i] = 0;
-    __syncthreads();
-    const int nrows = 2 * A.radius + 1;
-    // existing keypoints: occupancy + discs (feature_extractor.cpp:316-319); painting commutes (atomicOr)
-    if (A.kp_off) {
-        const int k0 = A.kp_off[fr], k1 = A.kp_off[fr + 1];
-        for (int k = k0 + tid; k < k1; k += nthreads) {
-            const float2 px = A.kps[k];
-            const int rr = (int)(px.y / (float)cs), cc = (int)(px.x / (float)cs);
-            if (rr >= 0 && rr <= A.nhc && cc >= 0 && cc <= A.nwc) occ[rr * (A.nwc + 1) + cc] = 1;
-            const int cx = __float2int_rn(px.x), cy = __float2int_rn(px.y);
-            for (int rI = 0; rI < nrows; ++rI) {
-                const int dy = rI - A.radius;
-                const int hwv = A.hw[dy < 0 ? -dy : dy];
-                paint_row(bm, wpr, A.w, A.h, cy + dy, cx - hwv, cx + hwv);
-            }
-        }
-    }
-    __syncthreads();
+    gsweep::init_mask(A, L, sm, fr);
     const double quality = A.quality[fr];
     const float* resp = A.resp + (size_t)fr * ncells * (size_t)(cs * cs);
     constexpr int NV = 40;                                        // register-resident cells: cs * cs <= 1280 (cs <= 35)
@@ -200,12 +160,7 @@ __global__ void __launch_bounds__(SWEEP_MAX_WARPS * 32, 1) ss_sweep_kernel(Sweep
                     v[q] = i < npx ? __ldg(rc + i) : -INFINITY;
                 }
             }
-            if (r > 0) {
-                // wait until row r-1 has finished cell c+1 (or its last cell)
-                const int need = min(c + 2, A.nwc);
-                while (progress[r - 1] < need) __nanosleep(40);   // yield the issue slots to the rows that are working
-                __threadfence_block();
-            }
+            gsweep::wave_wait(progress, nwarps, r, c, A.nwc);
             if (search) {
                 const float2 cm = A.cellmax[(size_t)fr * ncells + cell];
                 for (int round = 0; round < 2; ++round) {
@@ -250,18 +205,12 @@ __global__ void __launch_bounds__(SWEEP_MAX_WARPS * 32, 1) ss_sweep_kernel(Sweep
                     if (px < A.roi_x || py < A.roi_y || px >= A.roi_x + A.roi_w || py >= A.roi_y + A.roi_h) break;   // `continue` of the cell loop
                     if ((double)mx >= quality) {
                         if (lane == 0) (round == 0 ? firstd : secondd)[cell] = make_int2(px, py);
-                        for (int rI = lane; rI < nrows; rI += 32) {
-                            const int dy = rI - A.radius;
-                            const int hwv = A.hw[dy < 0 ? -dy : dy];
-                            paint_row(bm, wpr, A.w, A.h, py + dy, px - hwv, px + hwv);
-                        }
+                        gsweep::paint_disc(A, bm, wpr, px, py, lane, 32);
                         __syncwarp();
                     }
                 }
             }
-            __threadfence_block();                                // discs before the counter
-            __syncwarp();
-            if (lane == 0) progress[r] = c + 1;
+            gsweep::wave_publish(progress, nwarps, r, c, lane);
         }
     }
     __syncthreads();
@@ -297,22 +246,6 @@ __global__ void __launch_bounds__(SWEEP_MAX_WARPS * 32, 1) ss_sweep_kernel(Sweep
     for (int i = s_n + tid; i < A.max_per_frame; i += nthreads) out[i] = make_int2(-1, -1);
 }
 
-void circle_halfwidths(int radius, int* hw) {   // cv::circle(filled) rasterisation, as in frontend_fast.cu
-    for (int i = 0; i <= radius; ++i) hw[i] = -1;
-    int err = 0, dx = radius, dy = 0, plus = 1, minus = (radius << 1) - 1;
-    while (dx >= dy) {
-        if (hw[dy] < dx) hw[dy] = dx;
-        if (hw[dx] < dy) hw[dx] = dy;
-        dy++;
-        err += plus;
-        plus += 2;
-        const int mask = (err <= 0) - 1;
-        err -= minus & mask;
-        dx += mask;
-        minus -= mask & 2;
-    }
-}
-
 }  // namespace
 
 extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int count, int cellsize,
@@ -333,47 +266,17 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
         if (ov2_is_device_ptr(roi_xywh)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_detect_single_scale: roi must be a host pointer");
         for (int i = 0; i < 4; ++i) roi[i] = roi_xywh[i];
     }
-    // ss_sweep_kernel's shared memory: mask bitmap, two detections per cell, row progress, occupancy
-    const size_t wpr = (size_t)(W + 31) / 32;
-    size_t sweep_smem = (((size_t)H * wpr + 1) & ~(size_t)1) * 4 + (size_t)ncells * sizeof(int2) * 2 + (size_t)nhc * sizeof(int) +
-                        (size_t)(nhc + 1) * (nwc + 1);
-    sweep_smem = (sweep_smem + 15) & ~(size_t)15;
-    if (sweep_smem > 227 * 1024)
+    const int nw = nhc < SWEEP_MAX_WARPS ? nhc : SWEEP_MAX_WARPS;       // one warp per cell row (wavefront)
+    const size_t sweep_smem = ss_sweep_smem(W, H, nwc, nhc, nw).bytes;
+    if (sweep_smem > gsweep::SMEM_LIMIT)
         return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_detect_single_scale: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-    const void* d = nullptr;
+    DetectArgs D;
+    if ((st = stage_detect_args(ctx, "ov2_detect_single_scale", count, max_per_frame, curkp_offsets, curkps, quality_inout,
+                                sizeof(double), out_pts, out_counts, out_pts_int, &D)) != OV2_OK)
+        return st;
     void* o = nullptr;
-    int nkp_total = 0;
-    const int32_t* d_off = nullptr;
-    const float2* d_kps = nullptr;
-    if (curkp_offsets) {
-        if ((st = ov2_stage_in(ctx, curkp_offsets, sizeof(int32_t) * (size_t)(count + 1), &d)) != OV2_OK) return st;
-        d_off = (const int32_t*)d;
-        if (ov2_is_device_ptr(curkp_offsets)) {
-            OV2_CUDA(ctx, cudaMemcpyAsync(&nkp_total, curkp_offsets + count, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-            OV2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        } else {
-            nkp_total = curkp_offsets[count];
-        }
-        if (nkp_total > 0) {
-            if (!curkps) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_detect_single_scale: curkps is NULL");
-            if ((st = ov2_stage_in(ctx, curkps, sizeof(float) * 2 * (size_t)nkp_total, &d)) != OV2_OK) return st;
-            d_kps = (const float2*)d;
-        }
-    }
-    if ((st = ov2_stage_out(ctx, quality_inout, sizeof(double) * (size_t)count, &o, true)) != OV2_OK) return st;
-    double* d_q = (double*)o;
-    if ((st = ov2_stage_out(ctx, out_pts, sizeof(float) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    float2* d_out = (float2*)o;
-    if ((st = ov2_stage_out(ctx, out_counts, sizeof(int32_t) * (size_t)count, &o)) != OV2_OK) return st;
-    int32_t* d_cnt = (int32_t*)o;
-    if (out_pts_int) {
-        if ((st = ov2_stage_out(ctx, out_pts_int, sizeof(int32_t) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    } else {
-        if ((st = ov2_scratch(ctx, sizeof(int32_t) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    }
-    int2* d_int = (int2*)o;
     const size_t cell_px = (size_t)cellsize * cellsize;
     if ((st = ov2_scratch(ctx, sizeof(float) * (size_t)count * ncells * cell_px, &o)) != OV2_OK) return st;
     float* d_resp = (float*)o;
@@ -390,16 +293,13 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
         OV2_LAUNCH(ctx, "ss_response_kernel", ss_response_kernel<<<dim3(ncells, count), 256, smem, ctx->stream>>>(RA));
     }
     SweepArgs SA;
-    SA.w = W; SA.h = H; SA.cs = cellsize; SA.nwc = nwc; SA.nhc = nhc; SA.radius = cellsize / 4; SA.max_per_frame = max_per_frame;
-    circle_halfwidths(SA.radius, SA.hw);
+    gsweep::init_base(SA, W, H, cellsize, D.kp_off, D.kps);
+    SA.max_per_frame = max_per_frame;
     SA.roi_x = roi[0]; SA.roi_y = roi[1]; SA.roi_w = roi[2]; SA.roi_h = roi[3];
-    SA.kp_off = d_off; SA.kps = d_kps; SA.resp = d_resp; SA.cellmax = d_cellmax; SA.quality = d_q; SA.out_int = d_int; SA.out_n = d_cnt;
-    {
-        if (sweep_smem > 48 * 1024)
-            OV2_CUDA(ctx, cudaFuncSetAttribute(ss_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sweep_smem));
-        const int nw = nhc < SWEEP_MAX_WARPS ? nhc : SWEEP_MAX_WARPS;       // one warp per cell row (wavefront)
-        OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, sweep_smem, ctx->stream>>>(SA));
-    }
-    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, do_subpix, nullptr)) != OV2_OK) return st;
+    SA.resp = d_resp; SA.cellmax = d_cellmax; SA.quality = (double*)D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
+    if (sweep_smem > 48 * 1024)
+        OV2_CUDA(ctx, cudaFuncSetAttribute(ss_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sweep_smem));
+    OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, sweep_smem, ctx->stream>>>(SA));
+    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, D.ints, D.out, do_subpix, nullptr)) != OV2_OK) return st;
     return ov2_end(ctx);
 }

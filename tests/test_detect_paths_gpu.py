@@ -99,23 +99,28 @@ def oracle():
 
 
 # ---------------------------------------------------------------------------------------------------------- formulas
-def _fast_sweep_path(w, h, cs, seq_env=False):
-    """The sweep ov2_grid_fast launches (frontend_fast.cu, ov2_grid_fast): 'wave', 'seq' or 'capacity'."""
+def _fast_sweep_smem(w, h, cs, nw):
+    """Shared memory of fast_sweep_kernel at nw warps (grid_sweep.cuh SweepSmem, frontend_fast.cu fast_sweep_smem): the
+    bitmap, min(cap, 128) sort keys per warp, row progress counters when nw > 1, occupancy.  Vectorised over w and h."""
     nwc, nhc = w // cs, h // cs
     wpr = (w + 31) // 32
-    nw = min(nhc, 16)
-    cap = _cell_cap(cs)
-    wsmem = (((h * wpr + 1) & ~1) * 4 + nwc * nhc * 8 + nw * min(cap, 128) * 4 + nhc * 4 + (nhc + 1) * (nwc + 1) + 15) & ~15
-    smem = (h * wpr * 4 + cap * 4 + (nhc + 1) * (nwc + 1) + 15) & ~15
-    if wsmem <= 200 * 1024 and not seq_env:
-        return "wave"
-    return "seq" if smem <= 227 * 1024 else "capacity"
+    return (h * wpr * 4 + nw * min(_cell_cap(cs), 128) * 4 + np.where(nw > 1, nhc * 4, 0) + (nhc + 1) * (nwc + 1) + 15) & ~15
+
+
+def _fast_sweep_warps(w, h, cs):
+    """Warps ov2_grid_fast gives fast_sweep_kernel: the most, up to one per cell row and 16, whose shared memory fits 227 KB;
+    0: refused with OV2_ERR_CAPACITY.  Vectorised over w and h (at least one cell row)."""
+    nhc = np.asarray(h) // cs
+    nw = np.zeros(np.broadcast(np.asarray(w), nhc).shape, np.int64)
+    for k in range(1, 17):          # the layout grows with the warp count
+        nw = np.where((k <= nhc) & (_fast_sweep_smem(w, h, cs, k) <= 227 * 1024), k, nw)
+    return int(nw) if nw.ndim == 0 else nw
 
 
 def _sscale_fits(w, h, cs):
     nwc, nhc = w // cs, h // cs
     wpr = (w + 31) // 32
-    smem = (((h * wpr + 1) & ~1) * 4 + nwc * nhc * 16 + nhc * 4 + (nhc + 1) * (nwc + 1) + 15) & ~15
+    smem = (((h * wpr + 1) & ~1) * 4 + nwc * nhc * 16 + (nhc * 4 if nhc > 1 else 0) + (nhc + 1) * (nwc + 1) + 15) & ~15
     return smem <= 227 * 1024
 
 
@@ -258,43 +263,19 @@ def test_shipped_configurations(ctx, oracle, w, h, chain, src):
 
 
 # ---------------------------------------------------------------------------------------------------------- grid FAST sweeps
-def test_grid_fast_wave_equals_sequential_sweep(ctx, oracle, monkeypatch):
-    """OV2_FAST_SWEEP=seq forces the one-warp-per-frame fast_sweep_kernel where the wavefront kernel would run (640x480 at
-    cells 50 and 16, with ragged keypoints): both give the oracle's answer.  The profiler label is the same for both
-    kernels, so the path is pinned by the host's shared-memory formula."""
-    w, h = 640, 480
-    names = [f"tex:{40 + i}" for i in range(2)]
-    imgs = np.stack([oracle.image(n, w, h) for n in names])
-    pyr = _pyr(ctx, imgs)
-    for cs in (50, 16):
-        kl = [_kps(cs + f, w, h, 30, cs) for f in range(2)]
-        res = {}
-        for mode in ("wave", "seq"):
-            if mode == "seq":
-                monkeypatch.setenv("OV2_FAST_SWEEP", "seq")
-            else:
-                monkeypatch.delenv("OV2_FAST_SWEEP", raising=False)
-            assert _fast_sweep_path(w, h, cs, mode == "seq") == mode
-            th = np.array([10, 10], np.int32)
-            res[mode] = _grid_fast(ctx, pyr, cs, 0, 2, th, kl)
-            _check_fast(oracle, names, imgs, cs, kl, [10, 10], res[mode], th, tag="ragged")
-        for a, b in zip(res["wave"], res["seq"]):
-            assert np.array_equal(a, b)
-    pyr.close()
-
-
-@pytest.mark.parametrize("w,h,cs", [(1280, 720, 8), (1600, 1000, 50)])
-def test_grid_fast_automatic_sequential_fallback(ctx, oracle, w, h, cs):
-    """Geometries whose wavefront shared memory is over 200 KB: ov2_grid_fast falls back to the sequential sweep by itself
-    (1280x720 at cell 8 for the per-cell detections, 1600x1000 at cell 50 for the bitmap)."""
-    assert _fast_sweep_path(w, h, cs) == "seq"
+@pytest.mark.parametrize("w,h,cs,nw", [(1280, 720, 8, 16), (1600, 1000, 50, 16), (1600, 1150, 50, 3), (1600, 1153, 50, 1)])
+def test_grid_fast_sweep_warps_from_budget(ctx, oracle, w, h, cs, nw):
+    """fast_sweep_kernel takes as many warps as its shared memory allows: 16 at 1280x720 cell 8 (14 400 cells) and at
+    1600x1000 cell 50; 3 at 1600x1150 cell 50, where the bitmap leaves room for few sort-key areas; 1 at 1600x1153 cell 50,
+    which sweeps the rows in order without progress counters."""
+    assert _fast_sweep_warps(w, h, cs) == nw
     names = [f"tex:{60 + cs}"]
     imgs = np.stack([oracle.image(n, w, h) for n in names])
     pyr = _pyr(ctx, imgs)
     kl = [_kps(cs, w, h, 50, cs)]
     th = np.array([10], np.int32)
     out = _grid_fast(ctx, pyr, cs, 0, 1, th, kl)
-    _check_fast(oracle, names, imgs, cs, kl, [10], out, th, tag="fallback")
+    _check_fast(oracle, names, imgs, cs, kl, [10], out, th, tag="budget")
     assert out[2][0] > 0
     pyr.close()
 
@@ -302,7 +283,7 @@ def test_grid_fast_automatic_sequential_fallback(ctx, oracle, w, h, cs):
 def test_grid_fast_capacity_refusal_then_recovers(ctx, oracle):
     """1920x1080: the mask bitmap alone is over 227 KB, so ov2_grid_fast refuses with OV2_ERR_CAPACITY (decided on the host,
     before anything is enqueued); the same context then runs a normal call correctly."""
-    assert _fast_sweep_path(1920, 1080, 50) == "capacity"
+    assert _fast_sweep_warps(1920, 1080, 50) == 0
     big = api.Pyramid(ctx, 1, 1920, 1080, 0)
     big.build(synth.make_frame(3, 1920, 1080)[None])
     th = np.array([10], np.int32)
@@ -376,14 +357,11 @@ def _tie_cells(im, cs, th):
     return sum(1 for _, n, m in st if n > 16 and m > 1)
 
 
-@pytest.mark.parametrize("sweep", ["wave", "seq"])
-def test_grid_fast_tie_sort(ctx, oracle, monkeypatch, sweep):
+def test_grid_fast_tie_sort(ctx, oracle):
     """Cells where more than 16 candidates survive the mask and the top response is tied: the winner is the one the
     libstdc++ std::sort emulation (stdsort_emul.h) puts first.  The dot lattice (every candidate has the same response)
     has 54 such cells at cell 50; uniform noise frames (seeds 0 and 1) have 9 between them at threshold 10.  The test
     asserts at least 50 and 8."""
-    if sweep == "seq":
-        monkeypatch.setenv("OV2_FAST_SWEEP", "seq")
     w, h = 640, 480
     names = ["lattice", "noise:0", "noise:1"]
     imgs = np.stack([oracle.image(n, w, h) for n in names])
@@ -406,15 +384,12 @@ def _max_candidates(im, cs, th):
                for y in range(0, h - cs - 1, cs) for x in range(0, w - cs - 1, cs))
 
 
-@pytest.mark.parametrize("sweep", ["wave", "seq"])
 @pytest.mark.parametrize("name,cs,th0", CAPACITY_CASES)
-def test_grid_fast_dense_cells(ctx, oracle, monkeypatch, name, cs, th0, sweep):
+def test_grid_fast_dense_cells(ctx, oracle, name, cs, th0):
     """Cells with up to the full candidate capacity (the lattice reaches the bound exactly at cell 45: 200; noise at
     threshold 0 reaches 128 at cell 50, 213 at 64 and 820 at 128): every candidate is kept (no OV2_ERR_CAPACITY) and the
-    result equals the oracle, through ov2_grid_fast and through batch mode, with both sweeps.  Above 128 candidates the
-    wave kernel reads the cell's list from global memory and sorts in its global key area."""
-    if sweep == "seq":
-        monkeypatch.setenv("OV2_FAST_SWEEP", "seq")
+    result equals the oracle, through ov2_grid_fast and through batch mode.  Above 128 candidates the sweep reads the
+    cell's list from global memory and sorts in its global key area."""
     w, h = 640, 480
     im = oracle.image(name, w, h)
     mc = oracle._get(("maxcand", name, cs, th0), lambda: _max_candidates(im, cs, th0))

@@ -425,3 +425,25 @@ def test_brief_table_extractor_parses_generated_32_format():
     assert np.array_equal(mod.parse(txt), t.astype(np.int8))
     with pytest.raises(SystemExit):
         mod.parse(txt.replace("<< 7)", "<< 6)", 1))
+
+
+def test_fast_sweep_refuses_no_geometry_the_two_kernel_sweep_ran():
+    """Grid FAST's sweep used to pick between a wavefront kernel (when its shared memory was at most 200 KB) and a one-warp
+    kernel (at most 227 KB); both formulas are kept here as they were.  Every geometry either of them ran, the one
+    wavefront kernel runs, and every geometry the old wavefront kernel ran keeps its warp count (cells 8 to 128, images up
+    to 4096 x 4096)."""
+    from test_detect_paths_gpu import _cell_cap, _fast_sweep_warps
+    ws = np.arange(8, 4097, 5)[:, None]
+    for cs in range(8, 129):
+        w = ws[ws >= cs][:, None]
+        h = w.T
+        nwc, nhc = w // cs, h // cs
+        wpr = (w + 31) // 32
+        cap = _cell_cap(cs)
+        old_nw = np.minimum(nhc, 16)
+        wave = ((((h * wpr + 1) & ~1) * 4 + nwc * nhc * 8 + old_nw * min(cap, 128) * 4 + nhc * 4 + (nhc + 1) * (nwc + 1) + 15)
+                & ~15) <= 200 * 1024
+        seq = ((h * wpr * 4 + cap * 4 + (nhc + 1) * (nwc + 1) + 15) & ~15) <= 227 * 1024
+        nw = _fast_sweep_warps(w, h, cs)
+        assert (nw > 0)[wave | seq].all(), cs
+        assert (nw == old_nw)[wave].all(), cs
