@@ -1641,7 +1641,6 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
         H.off_pch = take(in_off, sizeof(int2) * (size_t)H.pch_cap);
         const double avg = npts > 0 ? (double)nobs / (double)npts : 0.0;
         H.sg = avg <= 5.0 ? 4 : (avg <= 12.0 ? 8 : 32);
-        if (getenv("OV2_BA_SG")) { const int e = atoi(getenv("OV2_BA_SG")); if (e == 4 || e == 8 || e == 32) H.sg = e; }
     }
     const size_t no = nobs > 0 ? nobs : 1, np = npts > 0 ? npts : 1;
     // results (Result record + outlier flags) of all windows sit together in the output region, the 'active' bytes of all
@@ -1687,21 +1686,18 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     // with two CTAs per SM still possible
     H.smem_sacc_off = schur / sizeof(double);
     H.schur_smem = 0;
-    const char* ssm = getenv("OV2_BA_SCHUR_SMEM");
-    if (H.n_max > 0 && s + schur + (size_t)WARPS * H.blk * sizeof(double) <= 190 * 1024 && !(ssm && atoi(ssm) == 0) &&
-               (single_window || (ssm && atoi(ssm) == 2))) {
+    if (H.n_max > 0 && single_window && s + schur + (size_t)WARPS * H.blk * sizeof(double) <= 190 * 1024) {
         // mode 2 (default for a single window when it fits: reduced systems up to n = 48 with at most 195 keyframes in the
         // window's keyframe table): one private block per warp, one
         // CTA per SM.  Batches keep the RED path: there two CTAs per SM (different windows overlapping their latency-bound
         // phases) are worth more than the faster accumulation - measured 5.1 k vs 4.1 k solves/s on the C3 batch.
         H.schur_smem = 2;
         schur += (size_t)WARPS * H.blk * sizeof(double);
-    }
-    // mode 3 (default up to n = 96, single windows and batches): owner mode, see schur_owner_phase
-    // Single windows spread over many CTAs stay on mode 2 when it fits (measured C3: 119 us vs 236 us per solve in the
-    // Schur phase at 148 CTAs - there the phase is latency, not RED bound); batches (1-2 CTAs per window) take mode 3.
-    // Its host-side pair sort counts over all ncam^2 keyframe pairs, so it is limited to windows of <= MAX_CAMS keyframes.
-    if (H.n_max > 0 && H.n_max <= 96 && ncam <= MAX_CAMS && ((ssm && atoi(ssm) == 3) || (!ssm && !(single_window && H.schur_smem == 2)))) {
+    } else if (H.n_max > 0 && H.n_max <= 96 && ncam <= MAX_CAMS) {
+        // mode 3 (up to n = 96, single windows and batches): owner mode, see schur_owner_phase
+        // Single windows spread over many CTAs stay on mode 2 when it fits (measured C3: 119 us vs 236 us per solve in the
+        // Schur phase at 148 CTAs - there the phase is latency, not RED bound); batches (1-2 CTAs per window) take mode 3.
+        // Its host-side pair sort counts over all ncam^2 keyframe pairs, so it is limited to windows of <= MAX_CAMS keyframes.
         const size_t R = (size_t)WARPS * (32 / H.sg);
         size_t tile = (R * (size_t)owner_tile_pitch(H.n_max) + 2 * R) * sizeof(double);
         const size_t stage = (size_t)WARPS * PCH * 26 * sizeof(double);
@@ -1762,6 +1758,7 @@ static void fill_prob(const ov2_ba_problem* pb, const ov2_ba_opts* opts, const H
     P.acc = (double*)(dwork + H.w_acc); P.total = (double*)(dwork + H.w_total); P.scal = (double*)(dwork + H.w_scal);
     P.z = (double*)(dwork + H.w_z); P.sc_cam = (double*)(dwork + H.w_sccam); P.panel = (double*)(dwork + H.w_panel);
     P.counts = (double*)(dwork + H.w_counts); P.bar = (unsigned*)(dwork + H.w_bar); P.result = (Result*)(dwork + H.w_result);
+    // OV2_BA_TRACE selects no path: it records per-phase times and prints the window's plan (read back by the plan tests)
     P.trace = getenv("OV2_BA_TRACE") ? (unsigned long long*)(dwork + H.w_trace) : nullptr;
     P.ncv_max = H.ncv_max; P.blk = H.blk; P.solve_blocked = H.solve_blocked;
     P.sg = H.sg;   // lanes per landmark in the per-landmark phases
@@ -1856,6 +1853,8 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     int gcap = nprob == 1 ? resident : (resident / nprob < 1 ? 1 : resident / nprob);
     if (nprob > 1 && gcap > 16) gcap = 16;
     if (G > gcap) G = gcap;
+    // OV2_BA_CTAS sets the group size within the cap: ranks that share one GPU need small groups to be co-resident, and
+    // the group barrier and panel split are tested at chosen sizes.  Every size solves the same way.
     if (getenv("OV2_BA_CTAS")) { int e = atoi(getenv("OV2_BA_CTAS")); if (e >= 1 && e <= gcap) G = e; }
     if (world > 1 && G < 2) G = 2;
     int ngroups = nprob < resident / G ? nprob : resident / G;
@@ -1953,7 +1952,6 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         int nthr = nprob >= 8 ? 8 : 1;
         const unsigned hc = std::thread::hardware_concurrency();
         if (hc > 0 && (unsigned)nthr > hc) nthr = (int)hc;
-        if (getenv("OV2_BA_PACK_THREADS")) { const int e = atoi(getenv("OV2_BA_PACK_THREADS")); if (e >= 1 && e <= 64) nthr = e; }
         std::atomic<int> next(0);
         std::atomic<const char*> perr(nullptr);
         auto worker = [&]() {

@@ -342,12 +342,9 @@ bool g_tables_loaded[64] = {false};
 // 0.279 / 0.199 at cover 2.58 (1024); the lines cross near cover 1.4.
 constexpr float DENSE_COVER = 1.4f;
 
-// Fixed-stride ORB-fallback calls only (ragged frame_idx calls keep the per-window kernel); OV2_DESC_DENSE=0 / 1
-// forces the per-window / dense path for those calls.
+// Fixed-stride ORB-fallback calls only (ragged frame_idx calls keep the per-window kernel).
 bool use_dense(const int32_t* frame_idx, int per_frame, int w, int h) {
     if (frame_idx || w < 63 || h < 63) return false;   // below 63 px no keypoint is valid
-    const char* e = getenv("OV2_DESC_DENSE");
-    if (e && *e) return atoi(e) != 0;
     return (double)per_frame * 26.0 * 26.0 >= (double)DENSE_COVER * (w - 36) * (h - 36);
 }
 

@@ -26,11 +26,9 @@
 // (compiled with -fmad=false; the one FMA OpenCV uses is spelled __fmaf_rn).
 #include "grid_sweep.cuh"
 #include "stdsort_emul.h"
-
-#include <cuda.h>   // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint)
+#include "tma_util.cuh"
 
 #include <math.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -74,33 +72,6 @@ struct FastSmem {
         bytes = sc + 2 * cs * scp;
     }
 };
-
-// ---- TMA staging (sm_90a): one elected thread issues a single cp.async.bulk.tensor that lands
-// the whole cell ROI (box BOXW x cs bytes of frame z) in shared memory and completes on an mbarrier.
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1, 0x989680;\n"   /* suspend-time hint: sleep, do not spin (the spin was 7.6 % of the kernel's instructions) */
-        "@P1 bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(phase) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int x, int y, int z) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z)
-                 : "memory");
-}
 
 // ---------------------------------------------------------------------------------- F1
 // Per polarity: the best arc extreme over the 16 arcs of 9 contiguous ring pixels, on two pixels at once.  e[k] = d[k] + 256
@@ -158,9 +129,9 @@ __global__ void fast_cells_kernel(FastArgs A, const __grid_constant__ CUtensorMa
     // cell's ROI begins `off` bytes into each staged row.  Box columns beyond the image are zero.
     const int off = x0 & 15;
     if (use_tma && tid == 0) {
-        mbar_init(&s_bar, 1);
-        mbar_expect_tx(&s_bar, (uint32_t)(rp * cs));
-        tma_load_3d(smem, &tmap, &s_bar, x0 - off, y0, A.first + fr);
+        tma::mbar_init(&s_bar, 1);
+        tma::mbar_expect_tx(&s_bar, (uint32_t)(rp * cs));
+        tma::load_3d(smem, &tmap, &s_bar, x0 - off, y0, A.first + fr);
     }
     {
         uint32_t* scw = reinterpret_cast<uint32_t*>(sc);
@@ -168,7 +139,7 @@ __global__ void fast_cells_kernel(FastArgs A, const __grid_constant__ CUtensorMa
     }
     if (use_tma) {
         __syncthreads();             // barrier init visible to every waiter
-        mbar_wait(&s_bar, 0);
+        tma::mbar_wait_suspend(&s_bar, 0);
     } else {
         const uint8_t* img = A.img + A.fstride * (A.first + fr) + (size_t)y0 * A.pitch + (x0 - off);
         const int avail = A.w - (x0 - off);
@@ -625,24 +596,6 @@ void subpix_mask(float* mask) {
 
 }  // namespace
 
-// Host side of the TMA staging: a 3-D tiled tensor map {W, H, frames} over the level-0 images, box
-// {rp, cs, 1} (rp = cs + 15 rounded up to 16 bytes: the box starts on the 16-byte boundary at or below the cell).  Falls back to plain loads
-// of the same box when the images do not meet the TMA alignment rules (user-aliased level 0 with an odd pitch).
-typedef CUresult (*ov2_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                        const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                        CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static ov2_encode_tiled_fn tma_encoder() {
-    static ov2_encode_tiled_fn fn = []() -> ov2_encode_tiled_fn {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            return nullptr;
-        return (ov2_encode_tiled_fn)p;
-    }();
-    return fn;
-}
-
 template <int HH>
 static ov2_status launch_fast_cells_hh(ov2_ctx* ctx, const FastArgs& FA, int nframes_grid, const CUtensorMap& tmap, int use_tma,
                                       int rp) {
@@ -656,24 +609,15 @@ static ov2_status launch_fast_cells_hh(ov2_ctx* ctx, const FastArgs& FA, int nfr
     return OV2_OK;
 }
 
+// TMA staging: a 3-D tiled tensor map {W, H, frames} over the level-0 images, box {rp, cs, 1} (rp = cs + 15 rounded up to
+// 16 bytes: the box starts on the 16-byte boundary at or below the cell).  Plain loads of the same box when the images do
+// not meet the TMA alignment rules (user-aliased level 0 with an odd pitch or base) or the driver lacks the encoder.
 static ov2_status launch_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, const FastArgs& FA, int nframes_grid) {
     const int cs = FA.cs;
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
-    int use_tma = 0;
     const int rp = (cs + 15 + 15) & ~15;      // staged box width, TMA or not
-    const char* env = getenv("OV2_NO_TMA");
-    ov2_encode_tiled_fn enc = (env && atoi(env)) ? nullptr : tma_encoder();
-    if (enc && ((uintptr_t)FA.img % 16) == 0 && FA.pitch % 16 == 0 && FA.fstride % 16 == 0) {
-        cuuint64_t dims[3] = {(cuuint64_t)FA.w, (cuuint64_t)FA.h, (cuuint64_t)pyr->batch};
-        cuuint64_t strides[2] = {(cuuint64_t)FA.pitch, (cuuint64_t)FA.fstride};
-        cuuint32_t box[3] = {(cuuint32_t)rp, (cuuint32_t)cs, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)FA.img, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r == CUDA_SUCCESS) use_tma = 1;
-    }
+    const int use_tma = tma::make_u8_3d(&tmap, FA.img, FA.w, FA.h, pyr->batch, FA.pitch, FA.fstride, rp, cs) ? 1 : 0;
     return cs <= 64 ? launch_fast_cells_hh<32>(ctx, FA, nframes_grid, tmap, use_tma, rp)
                     : launch_fast_cells_hh<64>(ctx, FA, nframes_grid, tmap, use_tma, rp);
 }

@@ -8,7 +8,6 @@
 #include "ov2_common.cuh"
 #include "tma_util.cuh"
 
-#include <stdlib.h>
 #include <string.h>
 
 namespace {
@@ -328,8 +327,7 @@ ov2_status ov2_pyr_load_level0(ov2_ctx* ctx, ov2_pyr* p, const uint8_t* images, 
 // levels 1.. from level 0 (kernels only)
 ov2_status ov2_pyr_make_levels(ov2_ctx* ctx, ov2_pyr* p, int first, int count) {
     // fused path: the reference's pyramid depth (3 extra levels), level 3 at least 8 x 8, level 0 TMA-addressable
-    const char* nf = getenv("OV2_PYR_UNFUSED");
-    if (p->nlev == 4 && p->w[3] >= 8 && p->h[3] >= 8 && !(nf && atoi(nf))) {
+    if (p->nlev == 4 && p->w[3] >= 8 && p->h[3] >= 8) {
         CUtensorMap tmap;
         memset(&tmap, 0, sizeof(tmap));
         if (tma::make_u8_3d(&tmap, p->l0, p->w[0], p->h[0], p->batch, p->l0_pitch, p->l0_fstride, P0, H0T)) {

@@ -65,7 +65,7 @@ extern "C" ov2_status ov2_frontend_step(ov2_ctx* ctx, ov2_pyr* prev, ov2_pyr* cu
     ov2_ctx::StepGraph* g = nullptr;
     for (auto& e : ctx->step_graphs)
         if (e.key == key) { g = &e; break; }
-    const bool use_graphs = !ctx->profiling && !getenv("OV2_NO_GRAPH");
+    const bool use_graphs = !ctx->profiling;
     const bool host_images = !ov2_is_device_ptr(a->prev_images);
 
     ov2_status st = ov2_batch_begin(ctx);     // resets the arena, opens batch mode

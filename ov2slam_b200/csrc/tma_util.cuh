@@ -28,6 +28,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
         "TMA_WAIT_DONE:\n"
         "}\n" ::"r"(smem_u32(bar)), "r"(phase) : "memory");
 }
+// The same wait with a suspend-time hint: the waiting threads sleep instead of spinning.  For grid FAST's one-copy cells
+// the spin was 7.6 % of the kernel's instructions.
+__device__ __forceinline__ void mbar_wait_suspend(uint64_t* bar, uint32_t phase) {
+    asm volatile(
+        "{\n"
+        ".reg .pred P1;\n"
+        "TMA_WAIT_LOOP:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1, 0x989680;\n"
+        "@P1 bra TMA_WAIT_DONE;\n"
+        "bra TMA_WAIT_LOOP;\n"
+        "TMA_WAIT_DONE:\n"
+        "}\n" ::"r"(smem_u32(bar)), "r"(phase) : "memory");
+}
 __device__ __forceinline__ void load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int x, int y, int z) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z)

@@ -20,6 +20,7 @@ ov2_ctx* thread_context() {
     static thread_local ThreadCtx t;
     if (!t.tried) {
         t.tried = true;
+        // the reference's call takes no device: OV2_DEVICE names the GPU (default 0)
         const char* e = getenv("OV2_DEVICE");
         if (ov2_create(e ? atoi(e) : 0, &t.ctx) != OV2_OK) {
             fprintf(stderr, "[ov2b200] CLAHE: no CUDA device - the GPU front-end has no CPU fallback\n");

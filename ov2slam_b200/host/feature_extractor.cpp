@@ -36,6 +36,7 @@ State& st() { static State s; return s; }
 // make `im` the current device image (uploaded only if it is not already there); false (and reports) on failure
 bool load_image(State& s, const cv::Mat& im) {
     if (!s.ctx) {
+        // the reference's class takes no device: OV2_DEVICE names the GPU (default 0)
         const char* e = getenv("OV2_DEVICE");
         if (ov2_create(e ? atoi(e) : 0, &s.ctx) != OV2_OK) {
             fprintf(stderr, "[ov2b200] FeatureExtractor: no CUDA device - the GPU front-end has no CPU fallback\n");

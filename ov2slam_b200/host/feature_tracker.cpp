@@ -31,6 +31,7 @@ namespace {
 std::mutex g_mu;
 std::unordered_map<std::thread::id, FeatureTracker::ThreadState*>* g_states = nullptr;
 int env_device() {
+    // the reference's class takes no device: OV2_DEVICE names the GPU (default 0)
     const char* e = getenv("OV2_DEVICE");
     return e ? atoi(e) : 0;
 }

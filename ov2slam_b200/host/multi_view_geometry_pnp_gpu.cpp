@@ -43,6 +43,7 @@ bool MultiViewGeometry::ceresPnP(const std::vector<Eigen::Vector2d, Eigen::align
     PnpState& s = pnp_state();
     std::lock_guard<std::mutex> lk(s.mu);
     if (!s.ctx && !s.failed) {
+        // the reference's class takes no device: OV2_DEVICE names the GPU (default 0)
         const char* e = getenv("OV2_DEVICE");
         if (ov2_create(e ? atoi(e) : 0, &s.ctx) != OV2_OK) {
             fprintf(stderr, "[ov2b200] ceresPnP: no CUDA device - the GPU path has no CPU fallback\n");

@@ -1,4 +1,5 @@
-"""Per-phase device time of the persistent local-BA kernel (OV2_BA_TRACE=1 prints one line per solve on stderr)."""
+"""Per-phase device time of the persistent local-BA kernel (OV2_BA_TRACE=1 prints one line per solve on stderr, with the
+plan, Schur mode included, that each window's shape selects) at several group sizes."""
 import os
 import sys
 
@@ -13,13 +14,9 @@ opt = api.Optimizer(ctx)
 clone = lambda d: {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in d.items()}
 c3 = synth.make_ba_problem(3, 10, 2000, 8000)
 c5 = synth.make_ba_problem(5, 50, 20000, 150000)
-for smem in ("3", "2", "0"):
-    os.environ["OV2_BA_SCHUR_SMEM"] = smem
-    for name, pb, gs in (("C3", c3, ("16", "32", "64", "148")), ("C5", c5, ("296",))):
-        if name == "C5" and smem != "2":
-            continue
-        for g in gs:
-            os.environ["OV2_BA_CTAS"] = g
-            for _ in range(3):
-                print(name, "smem", smem, "ctas", g, file=sys.stderr, flush=True)
-                opt.local_ba(clone(pb))
+for name, pb, gs in (("C3", c3, ("16", "32", "64", "148")), ("C5", c5, ("296",))):
+    for g in gs:
+        os.environ["OV2_BA_CTAS"] = g
+        for _ in range(3):
+            print(name, "ctas", g, file=sys.stderr, flush=True)
+            opt.local_ba(clone(pb))

@@ -3,11 +3,13 @@
     python scripts/bench_describe.py [--batch 256] [--launches 50] [--warmup 5]
 
 Workload: C2's geometry (640 x 480 frames, 40 px cells), resident on the device: the tracked set (1024 keypoints per
-frame) and the new set (one slot per cell, 12 x 16 = 192 per frame, about 108 valid), each with OV2_DESC_DENSE=0 and =1
-forced, alternated in one process, timed with CUDA events over `launches` calls after warm-up (median of three
-windows).  Then, in a separate pass with per-kernel events, the dense path's smoothing and gather kernel times.  Then
-a sweep of per_frame at the same batch for the crossover of the density rule in frontend_desc.cu: cover =
-per_frame * 26^2 / ((w - 36)(h - 36)).  Checks that both paths return the same bytes on every set.  Prints the card's
+frame) and the new set (one slot per cell, 12 x 16 = 192 per frame, about 108 valid).  Each set is described by a ragged
+frame_idx call, which always takes the per-window path (describe_kernel), and by a fixed-stride call on the same points,
+which takes the path the density rule in frontend_desc.cu picks, alternated in one process and timed with CUDA events
+over `launches` calls after warm-up (median of three windows).  dense_ms is the fixed-stride time where the rule picks
+the dense path, and null where it does not.  Then, in a separate pass with per-kernel events, the dense path's smoothing
+and gather kernel times.  Then a sweep of per_frame at the same batch over the rule's crossover: cover =
+per_frame * 26^2 / ((w - 36)(h - 36)).  Checks that both calls return the same bytes on every set.  Prints the card's
 name, power limit and SM clock read in the same run, and one JSON line; writes nothing."""
 from __future__ import annotations
 
@@ -54,8 +56,12 @@ def main():
         p[rng.random(len(p)) >= frac_valid] = -1.0           # empty slots (x < 0)
         return torch.from_numpy(p).cuda()
 
-    def call(pts, per_frame, out):
-        fe.describe_brief(pyr, pts, out[0], out[1], n=pts.shape[0], per_frame=per_frame)
+    def call(pts, per_frame, out, fidx):
+        """The ragged call when `fidx` is given (always the per-window path), else the fixed-stride call."""
+        if fidx is not None:
+            fe.describe_brief(pyr, pts, out[0], out[1], n=pts.shape[0], frame_idx=fidx)
+        else:
+            fe.describe_brief(pyr, pts, out[0], out[1], n=pts.shape[0], per_frame=per_frame)
 
     def outputs(n):
         return (torch.empty((n, 32), dtype=torch.uint8, device="cuda"), torch.empty(n, dtype=torch.uint8, device="cuda"))
@@ -72,36 +78,43 @@ def main():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / launches
 
+    def kernels(pts, per_frame, fidx, reps=1):
+        """{kernel: (total ms, launches)} of `reps` calls (per-kernel events serialise the launches)."""
+        out = outputs(pts.shape[0])
+        call(pts, per_frame, out, fidx)
+        ctx.profile(True)
+        for _ in range(reps):
+            call(pts, per_frame, out, fidx)
+        rep = ctx.profile_report()
+        ctx.profile(False)
+        return rep
+
     def compare(pts, per_frame, launches, warmup, windows=3):
-        """ms per call of each forced path (median of `windows` alternated windows) and whether the bytes agree."""
-        res, ms = {}, {"0": [], "1": []}
+        """ms per call of the ragged (per-window) and the fixed-stride call (median of `windows` alternated windows), the
+        latter null unless the rule picks the dense path, and whether the bytes agree."""
+        # frame_idx[i] = i // per_frame: the frames of the fixed-stride call
+        fidx = torch.arange(pts.shape[0] // per_frame, dtype=torch.int32, device="cuda").repeat_interleave(per_frame)
+        assert set(kernels(pts, per_frame, fidx)) == {"describe_kernel"}
+        dense = "describe_dense_kernel" in kernels(pts, per_frame, None)
+        res, ms = {}, {True: [], False: []}
         for _ in range(windows):
-            for mode in ("0", "1"):
-                os.environ["OV2_DESC_DENSE"] = mode
+            for ragged in (True, False):
                 out = outputs(pts.shape[0])
-                ms[mode].append(timed(lambda: call(pts, per_frame, out), launches, warmup))
-                res[mode] = out
-        os.environ.pop("OV2_DESC_DENSE", None)
-        same = bool(torch.equal(res["0"][0], res["1"][0]) and torch.equal(res["0"][1], res["1"][1]))
-        return sorted(ms["0"])[windows // 2], sorted(ms["1"])[windows // 2], same
+                f = fidx if ragged else None
+                ms[ragged].append(timed(lambda: call(pts, per_frame, out, f), launches, warmup))
+                res[ragged] = out
+        same = bool(torch.equal(res[True][0], res[False][0]) and torch.equal(res[True][1], res[False][1]))
+        return sorted(ms[True])[windows // 2], sorted(ms[False])[windows // 2] if dense else None, same
 
     sets = {"tracked": (point_set(NKP), NKP), "new": (point_set(ncell, 108 / ncell), ncell)}
     report = {}
     for name, (pts, per_frame) in sets.items():
         pw, dn, same = compare(pts, per_frame, args.launches, args.warmup)
-        # kernel times of the dense path, per call (separate pass: per-kernel events serialise the launches)
-        os.environ["OV2_DESC_DENSE"] = "1"
-        out = outputs(pts.shape[0])
-        call(pts, per_frame, out)
-        ctx.profile(True)
-        for _ in range(10):
-            call(pts, per_frame, out)
-        rep = ctx.profile_report()
-        ctx.profile(False)
-        os.environ.pop("OV2_DESC_DENSE", None)
+        # kernel times of the dense path, per call
+        rep = kernels(pts, per_frame, None, 10) if dn is not None else None
         report[name] = {"per_frame": per_frame, "n": int(pts.shape[0]), "per_window_ms": pw, "dense_ms": dn,
-                        "speedup_dense": pw / dn, "bit_equal": same,
-                        "dense_kernels_ms": {k: v[0] / v[1] for k, v in rep.items()}}
+                        "speedup_dense": pw / dn if dn is not None else None, "bit_equal": same,
+                        "dense_kernels_ms": {k: v[0] / v[1] for k, v in rep.items()} if rep is not None else None}
     band = (w - 36) * (h - 36)
     sweep = []
     for per_frame in SWEEP:

@@ -252,15 +252,3 @@ def test_localba_bal_structure_fixture(ctx):
     assert np.abs(gpu["pose"] - ref["pose"]).max() <= 1e-6
     assert np.abs(gpu["lm_invdepth"] - ref["lm_invdepth"]).max() <= 1e-6
     assert (flags != r["flags"]).sum() <= 3
-
-
-@pytest.mark.parametrize("env", [{"OV2_BA_SCHUR_SMEM": "3"}, {"OV2_BA_SCHUR_SMEM": "0"}, {"OV2_BA_SCHUR_SMEM": "3", "OV2_BA_SG": "8"},
-                                 {"OV2_BA_SG": "32"}], ids=["owner", "red", "owner-sg8", "sg32"])
-def test_localba_optional_kernel_modes(ctx, monkeypatch, env):
-    """Paths of the persistent kernel that other windows take by default, forced on a SINGLE window: the owner-mode Schur
-    phase that batches use (pair-sorted Gram blocks + DMMA landmark rows), the plain RED path, and the other sub-group widths
-    of the per-landmark phases."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    _check(ctx, synth.make_ba_problem(3, 10, 2000, 8000))
-    _check(ctx, synth.make_ba_problem(42, 10, 1000, 4000, stereo=True))

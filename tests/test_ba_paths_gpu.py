@@ -151,12 +151,14 @@ def single_solve(ctx, pb, **opts):
 
 
 # ----------------------------------------------------------------------------- windows
-def boundary_window(ncv, stereo, ncam=None):
-    """`ncv` optimised keyframes (all used), two constant ones unless `ncam` asks for more; four residuals per landmark in a
-    mono window, five in a stereo one (two observations, each with its right-camera twin, and the anchor's right one)."""
+def boundary_window(ncv, stereo, ncam=None, per=None):
+    """`ncv` optimised keyframes (all used), two constant ones unless `ncam` asks for more; `per` non-anchor observations per
+    landmark, by default four in a mono window (four residuals) and two in a stereo one (five residuals: each observation
+    with its right-camera twin, and the anchor's right one)."""
     ncam = ncv + 2 if ncam is None else ncam
+    per = (2 if stereo else 4) if per is None else per
     npts = 60 * ncv
-    return synth.make_ba_problem(100 + 7 * ncv + ncam + (1 if stereo else 0), ncam, npts, (2 if stereo else 4) * npts, nconst=ncam - ncv,
+    return synth.make_ba_problem(100 + 7 * ncv + ncam + (1 if stereo else 0), ncam, npts, per * npts, nconst=ncam - ncv,
                                  stereo=stereo)
 
 
@@ -183,19 +185,41 @@ BOUNDARY = [  # ncv, ncam, branch
     (16, 18, dict(mode=3, nt=10, blocked=0)),
     (17, 19, dict(mode=0, blocked=1)),
     (16, 300, dict(mode=0, blocked=0, camtab="shared")),
+    (8, 300, dict(mode=0, blocked=0, camtab="shared")),
 ]
 
 
 @pytest.mark.parametrize("stereo", [False, True], ids=["mono", "stereo"])
 @pytest.mark.parametrize("ncv,ncam,branch", BOUNDARY, ids=["mode2-n48", "mode3-nt3-200kf", "mode3-nt6-n54", "mode3-nt6-n72", "mode3-nt10-n78",
-                                                           "mode3-nt10-n96-gj", "red-blocked-n102", "red-gj-300kf"])
+                                                           "mode3-nt10-n96-gj", "red-blocked-n102", "red-gj-300kf", "red-gj-n48-300kf"])
 def test_plan_branch_boundaries(ctx, capfd, monkeypatch, ncv, ncam, branch, stereo):
     """Each side of every single-window branch boundary: mode 2 up to 8 optimised keyframes (and <= 195 in all), owner mode
     with 3, 6 and 10 tiles, the largest Gauss-Jordan (n = 96) and the smallest blocked Cholesky (n = 102), and RED with
-    Gauss-Jordan on a window of more than 256 keyframes (owner mode is barred there)."""
+    Gauss-Jordan on windows of more than 256 keyframes (owner mode is barred there) at n = 96 and n = 48."""
     pb = boundary_window(ncv, stereo, ncam)
     assert W.used_keyframes(pb).sum() == ncv
     assert_plan(ctx, capfd, monkeypatch, pb, sg=4, **branch)
+    check(ctx, pb)
+
+
+TRACK_WINDOWS = {  # branch: (keyframes, non-anchor observations per landmark) of the mono and of the stereo window
+    "mode3-nt3-sg8": (dict(mode=3, nt=3, sg=8), (200, 8), (200, 4)),
+    "mode2-sg8": (dict(mode=2, sg=8), (10, 8), (10, 4)),
+    "mode2-sg32": (dict(mode=2, sg=32), (20, 14), (10, 9)),
+}
+
+
+@pytest.mark.parametrize("stereo", [False, True], ids=["mono", "stereo"])
+@pytest.mark.parametrize("which", list(TRACK_WINDOWS))
+def test_lanes_per_landmark_at_n48(ctx, capfd, monkeypatch, which, stereo):
+    """8 optimised keyframes (n = 48) with longer tracks than the boundary windows: owner mode with 3 tiles and 8 lanes per
+    landmark (the 200-keyframe table bars mode 2), and the private per-warp blocks of mode 2 with 8 and with 32 lanes (every
+    landmark of the stereo window is seen by all 10 keyframes, 19 residuals; the mono one by 15 of 20, 14 residuals)."""
+    branch, *shapes = TRACK_WINDOWS[which]
+    ncam, per = shapes[stereo]
+    pb = boundary_window(8, stereo, ncam, per)
+    assert W.used_keyframes(pb).sum() == 8
+    assert_plan(ctx, capfd, monkeypatch, pb, blocked=0, **branch)
     check(ctx, pb)
 
 
@@ -438,23 +462,6 @@ def test_batch_mixing_every_plan(ctx):
             assert np.array_equal(got["pose"][-1800:], pb["pose"][-1800:])
         if name == "all-constant":
             assert np.array_equal(got["pose"], pb["pose"])
-
-
-def test_batch_with_private_block_windows(ctx, capfd, monkeypatch):
-    """OV2_BA_SCHUR_SMEM=2 gives batch windows that fit the private per-warp blocks mode 2 (<= 8 optimised keyframes) next to
-    RED windows in one launch: every window equals its single solve."""
-    pbs = [boundary_window(8, False), boundary_window(8, True), boundary_window(12, False), boundary_window(17, False),
-           W.drop_landmark_residuals(synth.make_ba_problem(502, 10, 900, 1800), np.arange(900)[np.arange(900) % 3 != 0])]
-    singles = [single_solve(ctx, pb) for pb in pbs]
-    monkeypatch.setenv("OV2_BA_SCHUR_SMEM", "2")
-    monkeypatch.setenv("OV2_BA_TRACE", "1")
-    capfd.readouterr()
-    batch = [W.clone(pb) for pb in pbs]
-    res, flags = api.local_ba_batch(ctx, batch)
-    monkeypatch.delenv("OV2_BA_TRACE")
-    assert _read_trace(capfd)["mode"] == 2               # the trace reports the first window's plan
-    for k in range(len(pbs)):
-        assert_same_as_single(res[k], flags[k], batch[k], singles[k])
 
 
 def test_batch_reuses_groups(ctx, capfd, monkeypatch):

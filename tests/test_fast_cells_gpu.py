@@ -11,6 +11,7 @@ import pytest
 
 from ov2slam_b200 import api, synth
 from oracle import image_ref as R
+from test_frontend_gpu import unaligned_device_frames
 
 pytestmark = pytest.mark.gpu
 
@@ -38,14 +39,17 @@ def _cap(cs):
 
 @pytest.mark.parametrize("staging", ["tma", "plain"])
 @pytest.mark.parametrize("cs", [50, 35, 16, 8, 64, 65, 128])
-def test_fast_cell_full_candidate_lists_match_oracle(ctx, monkeypatch, cs, staging):
-    if staging == "plain":
-        monkeypatch.setenv("OV2_NO_TMA", "1")
+def test_fast_cell_full_candidate_lists_match_oracle(ctx, cs, staging):
+    """`plain`: the same frames through a device-aliased level 0 whose base the TMA rules reject (plain-load staging)."""
     nw, cap = W // cs, _cap(cs)
     top = 0
     for name, im in _frames().items():
         pyr = api.Pyramid(ctx, 1, W, H, 0)
-        pyr.build(im[None])
+        if staging == "plain":
+            d, args = unaligned_device_frames(im[None])
+            pyr.build(**args)
+        else:
+            pyr.build(im[None])
         fe = api.FeatureExtractor(ctx)
         for th in THRESHOLDS:
             cells = fe.debug_fast_cells(pyr, 0, cs, th)

@@ -90,6 +90,22 @@ def test_product_never_imports_oracle():
             assert not re.search(r'#include\s+"[^"]*oracle/', txt), p
 
 
+def test_product_reads_only_non_selecting_environment_variables():
+    """Every kernel path is chosen from the input.  The library and the host shims read three variables, none of which
+    picks a path: OV2_BA_TRACE (per-phase times and the plan on stderr), OV2_BA_CTAS (the local-BA group size, which ranks
+    sharing one GPU need so that their kernels are co-resident) and OV2_DEVICE (the GPU of the drop-in classes, whose
+    reference signatures take none).  The mocks under tests/helpers read their log paths and are not product code."""
+    names = set()
+    for d in ("csrc", "host"):
+        for p in (ROOT / "ov2slam_b200" / d).rglob("*"):
+            if p.suffix in (".cu", ".cuh", ".h", ".cpp", ".hpp"):
+                txt = p.read_text()
+                calls = re.findall(r"\bgetenv\s*\(([^)]*)\)", txt)
+                assert all(re.fullmatch(r'\s*"\w+"\s*', c) for c in calls), (p, calls)
+                names |= {c.strip().strip('"') for c in calls}
+    assert names == {"OV2_BA_TRACE", "OV2_BA_CTAS", "OV2_DEVICE"}, names
+
+
 def test_klt_level_setup_lane_code_matches_definition(tmp_path):
     """ov2slam_b200/csrc/klt_setup.cuh (the per-lane staging / Scharr / template code the KLT kernel
     runs) compiled for the host and checked against the definition (reflect-101 neighbourhood, Scharr

@@ -15,18 +15,9 @@ import pytest
 
 from ov2slam_b200 import api, synth
 from oracle import image_ref as R
-from test_frontend_gpu import _klt_assert, _klt_inputs
+from test_frontend_gpu import _klt_assert, _klt_inputs, unaligned_device_frames
 
 pytestmark = pytest.mark.gpu
-
-ENV = ("OV2_PYR_UNFUSED",)
-
-
-def _env(monkeypatch, **kv):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in kv.items():
-        monkeypatch.setenv(k, str(v))
 
 
 @contextmanager
@@ -125,10 +116,7 @@ def test_pyramid_device_level0_alignment(ctx, src, extra):
         d = torch.from_numpy(wide).cuda()
         args = dict(images=d.data_ptr() + x0, count=nf, row_stride=W, frame_stride=W * h)
     else:
-        d = torch.zeros(nf * h * w + 32, dtype=torch.uint8, device="cuda")
-        off = (16 - d.data_ptr() % 16) % 16 + 1
-        d[off:off + nf * h * w] = torch.from_numpy(imgs.reshape(-1)).cuda()
-        args = dict(images=d.data_ptr() + off, count=nf, row_stride=w, frame_stride=w * h)
+        d, args = unaligned_device_frames(imgs)
     torch.cuda.synchronize()
     with _launches(ctx) as k:
         pyr.build(**args)
@@ -152,23 +140,25 @@ def test_pyramid_build_one_slot_leaves_the_others(ctx, extra):
 
 
 @pytest.mark.parametrize("w,h", [(640, 480), (752, 480)])
-def test_pyramid_unfused_equals_fused(ctx, monkeypatch, w, h):
-    """OV2_PYR_UNFUSED=1 (one pyr_down_kernel launch per level) gives the fused kernel's bytes."""
+def test_pyramid_unaligned_level0_equals_fused(ctx, w, h):
+    """The same images built from an aligned level 0 (the fused kernel) and from a device view one byte past a 16-byte
+    boundary (one pyr_down_kernel launch per level) give the same bytes."""
     imgs = np.stack([synth.make_frame(420 + i, w, h) for i in range(3)])
     got = {}
-    for unfused in ("0", "1"):
-        _env(monkeypatch, OV2_PYR_UNFUSED=unfused)
+    for unfused in (False, True):
         pyr = api.Pyramid(ctx, 3, w, h, 3)
+        d, args = unaligned_device_frames(imgs) if unfused else (None, dict(images=imgs))
         with _launches(ctx) as k:
-            pyr.build(imgs)
-        assert ("pyr_levels_kernel" in k) == (unfused == "0") and k.get("pyr_down_kernel", 0) == (3 if unfused == "1" else 0), k
+            pyr.build(**args)
+        assert ("pyr_levels_kernel" in k) != unfused and k.get("pyr_down_kernel", 0) == (3 if unfused else 0), k
         got[unfused] = [[pyr.download(f, lvl) for lvl in range(4)] for f in range(3)]
         pyr.close()
+        del d
     for f in range(3):
         ref = R.build_pyramid_ref(imgs[f], 3)
         for lvl in range(4):
-            assert np.array_equal(got["0"][f][lvl], got["1"][f][lvl]), (f, lvl)
-            assert np.array_equal(got["1"][f][lvl], ref[lvl]), (f, lvl)
+            assert np.array_equal(got[False][f][lvl], got[True][f][lvl]), (f, lvl)
+            assert np.array_equal(got[True][f][lvl], ref[lvl]), (f, lvl)
 
 
 # ---------------------------------------------------------------- 2. KLT: the default launch on one input set
@@ -199,9 +189,8 @@ def klt_pyr(ctx, klt_set):
     cp.close()
 
 
-def test_klt_default_launch(ctx, monkeypatch, klt_set, klt_pyr):
+def test_klt_default_launch(ctx, klt_set, klt_pyr):
     """The whole set in one fb_klt_kernel launch: the same bits as the oracle for every keypoint."""
-    _env(monkeypatch)
     s = klt_set
     with _launches(ctx) as k:
         got = _track(ctx, *klt_pyr, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
@@ -232,7 +221,7 @@ def unaligned_set():
 
 
 @pytest.mark.parametrize("src", ["w333", "w334", "roi"])
-def test_klt_unaligned_level0(ctx, monkeypatch, unaligned_set, src):
+def test_klt_unaligned_level0(ctx, unaligned_set, src):
     """Pyramids aliasing device images whose level 0 is not word aligned (odd or 2-mod-4 pitch, a column ROI 3 bytes into
     a 352-byte row): the byte / reflected template staging and the plain search gather.  Equal to the oracle and to the
     same frames tracked from host-built pyramids."""
@@ -240,7 +229,6 @@ def test_klt_unaligned_level0(ctx, monkeypatch, unaligned_set, src):
     w = 333 if src == "roi" else int(src[1:])
     s = unaligned_set[w]
     nf, h = 2, 245
-    _env(monkeypatch)
     hp, hc = _pyramids(ctx, s["prevs"], s["curs"])
     host = _track(ctx, hp, hc, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
     _assert_same(host, s["ref"], "host-built")
@@ -314,9 +302,8 @@ def high_gradient_set():
     return dict(prevs=prevs, curs=curs, kps=kps, pri=pri, lv=lv, fidx=fidx, ref=ref)
 
 
-def test_klt_high_gradient_windows(ctx, monkeypatch, high_gradient_set):
+def test_klt_high_gradient_windows(ctx, high_gradient_set):
     """Windows with sum(|Ix| + |Iy|) >= 262 000, where the mismatch sums need the split 64-bit reduction: bit-exact."""
-    _env(monkeypatch)
     s = high_gradient_set
     pp, cp = _pyramids(ctx, s["prevs"], s["curs"])
     got = _track(ctx, pp, cp, s["kps"], s["pri"], s["lv"], frame_idx=s["fidx"])
@@ -356,7 +343,7 @@ def large_batch():
     return dict(prevs=prevs, curs=curs, kps=kps, pri=pri, lv=lv, per=per, idx=idx, empty=np.nonzero(empty)[0], ref=ref)
 
 
-def test_klt_large_batch_work_counter(ctx, monkeypatch, large_batch):
+def test_klt_large_batch_work_counter(ctx, large_batch):
     """12 800 keypoints: 1 600 CTAs of 8 warps, more than an H100 holds resident (at most 2 048 threads per SM), so the
     launch takes the global work-counter path.  Equal to the oracle on its sample; empty slots get status 0 and keep
     their prior."""
@@ -365,7 +352,6 @@ def test_klt_large_batch_work_counter(ctx, monkeypatch, large_batch):
     n = len(s["kps"])
     assert (n + 7) // 8 > 8 * torch.cuda.get_device_properties(0).multi_processor_count
     pp, cp = _pyramids(ctx, s["prevs"], s["curs"])
-    _env(monkeypatch)
     out, st = _track(ctx, pp, cp, s["kps"], s["pri"], s["lv"], per_frame=s["per"])
     _assert_same((out[s["idx"]], st[s["idx"]]), s["ref"], "oracle sample")
     assert not st[s["empty"]].any() and np.array_equal(out[s["empty"]], s["pri"][s["empty"]])
@@ -398,11 +384,10 @@ def small_sets():
 
 
 @pytest.mark.parametrize("w,h", SMALL)
-def test_klt_small_images_opencv_depth(ctx, monkeypatch, small_sets, w, h):
+def test_klt_small_images_opencv_depth(ctx, small_sets, w, h):
     """cv::buildOpticalFlowPyramid stops before a level <= 9 px, and calcOpticalFlowPyrLK / the reference track from the
     depth it reached (17 x 16: 0, 40 x 30: 1, 64 x 48 and 96 x 72: 2, 161 x 83: 3), whatever nbpyrlvl says and however many
     levels the pyramid holds: equal to the oracle (whose statuses equal cv2's)."""
-    _env(monkeypatch)
     s = small_sets[(w, h)]
     pp, cp = _pyramids(ctx, s["prev"][None], s["cur"][None])
     for key, lv in s["lvs"].items():
@@ -445,9 +430,8 @@ def _edge_check(s, got, kps, pri, lv, frames):
                 _klt_assert(out[m], st[m], s["prevs"][f], s["curs"][f], kps[m], pri[m], 9, int(lvl), min_frac=0.9)
 
 
-def test_klt_edge_inputs_first_frame(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs):
+def test_klt_edge_inputs_first_frame(ctx, klt_set, klt_pyr, edge_inputs):
     """Fixed-stride addressing from first_frame = 1 with per_frame = 120 (frames 1 and 2 of a 3-frame pyramid)."""
-    _env(monkeypatch)
     e = edge_inputs
     kps, pri, lv = np.concatenate([e["kps"]] * 2), np.concatenate([e["pri"]] * 2), np.concatenate([e["lv"]] * 2)
     got = _track(ctx, *klt_pyr, kps, pri, lv, first_frame=1, per_frame=120)
@@ -455,9 +439,8 @@ def test_klt_edge_inputs_first_frame(ctx, monkeypatch, klt_set, klt_pyr, edge_in
     _edge_check(s, got, kps, pri, lv, np.repeat(np.array([1, 2]), 120))
 
 
-def test_klt_edge_inputs_ragged_frames(ctx, monkeypatch, klt_set, klt_pyr, edge_inputs):
+def test_klt_edge_inputs_ragged_frames(ctx, klt_set, klt_pyr, edge_inputs):
     """A ragged, non-monotonic frame_idx (2, 0, 1, 0, 2, ...)."""
-    _env(monkeypatch)
     e = edge_inputs
     fidx = np.random.default_rng(4).integers(0, 3, 120).astype(np.int32)
     fidx[:5] = [2, 0, 1, 0, 2]
