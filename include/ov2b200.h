@@ -170,6 +170,14 @@ OV2_API ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* 
                       const uint8_t* nbpyrlvl, int nbpyrlvl_all,
                       const float* kps, float* priors_inout, uint8_t* status_out);
 
+/* Measurement hook: ov2_fb_klt with the same arguments and results, plus counts_out (2 n int32): level set-ups (template
+ * built) at 2 i and Lucas-Kanade iterations at 2 i + 1, forward and backward tracks of keypoint i together.  A second
+ * instantiation of the kernel; ov2_fb_klt carries no counter. */
+OV2_API ov2_status ov2_debug_klt_counts(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
+                      int n, const int32_t* frame_idx, int first_frame, int per_frame,
+                      const uint8_t* nbpyrlvl, int nbpyrlvl_all,
+                      const float* kps, float* priors_inout, uint8_t* status_out, int32_t* counts_out);
+
 /* ------------------------------------------------------------------ F + S: grid FAST + cornerSubPix
  * Replaces FeatureExtractor::detectGridFAST(im, ncellsize, vcurkps, roi)
  * (/root/reference/src/feature_extractor.cpp:443-570; include/feature_extractor.hpp:41-42) with

@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_debug_klt_counts", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -128,6 +128,7 @@ def load():
     lib.ov2_remap.argtypes = [vp, vp, vp, sz, sz, vp, sz, sz, i32]
     lib.ov2_pyr_build_remap.argtypes = [vp, vp, vp, vp, sz, sz, i32, i32]
     lib.ov2_fb_klt.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp]
+    lib.ov2_debug_klt_counts.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp, vp]
     lib.ov2_grid_fast.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_detect_single_scale.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_pnp_solve.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, C.c_float, i32, i32, vp, vp, vp]
@@ -370,10 +371,11 @@ class FeatureTracker:
         self.fmax_px_precision = float(np.float32(fmax_px_precision))
 
     def fb_klt_tracking(self, prev: Pyramid, cur: Pyramid, nwinsize, nbpyrlvl, ferr, fmax_fbklt_dist,
-                        kps, priors_inout, status_out, n=None, frame_idx=None, first_frame=0, per_frame=None):
+                        kps, priors_inout, status_out, n=None, frame_idx=None, first_frame=0, per_frame=None, counts_out=None):
         """fbKltTracking over a (ragged or fixed-stride) batch.  nbpyrlvl: int or per-keypoint uint8
         array.  kps / priors_inout: (n, 2) float32; status_out: (n,) uint8.  Arrays may be numpy
-        (host) or CUDA tensors (device)."""
+        (host) or CUDA tensors (device).  counts_out ((n, 2) int32, measurement only): the same tracking through the
+        counting kernel, which also returns each keypoint's level set-ups and iterations (forward + backward)."""
         if n is None:
             n = int(kps.shape[0])
         prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
@@ -383,9 +385,12 @@ class FeatureTracker:
             lv_ptr, lv_all = _ptr(nbpyrlvl), 0
         if frame_idx is None and per_frame is None:
             per_frame = max(n, 1)
-        self.ctx.check(self.ctx.lib.ov2_fb_klt(self.ctx.h, prev.h_, cur.h_, C.byref(prm), n, _ptr(frame_idx),
-                                               int(first_frame), int(per_frame or 0), lv_ptr, lv_all,
-                                               _ptr(kps), _ptr(priors_inout), _ptr(status_out)))
+        args = (self.ctx.h, prev.h_, cur.h_, C.byref(prm), n, _ptr(frame_idx), int(first_frame), int(per_frame or 0), lv_ptr,
+                lv_all, _ptr(kps), _ptr(priors_inout), _ptr(status_out))
+        if counts_out is None:
+            self.ctx.check(self.ctx.lib.ov2_fb_klt(*args))
+        else:
+            self.ctx.check(self.ctx.lib.ov2_debug_klt_counts(*args, _ptr(counts_out)))
 
     def line_min_sad(self, left: Pyramid, right: Pyramid, level: int, pts, nwinsize, goleft, xprior_out, l1err_out,
                      n=None, frame_idx=None, first_frame=0, per_frame=None):

@@ -50,18 +50,64 @@ __device__ __forceinline__ long long warp_sum64(int s) {
     return ((long long)shi << 16) + (long long)slo;
 }
 
+// The lane's search taps for the window origin (jx, jy): rows jy + lane_row and +1, columns jx + lane_col .. +3, four bytes
+// per row packed into one word each (byte k = column jx + lane_col + k).  Three ways to the same bytes, chosen per origin
+// (warp-uniform): aligned words and a funnel shift on a word-aligned level, byte loads elsewhere inside the image, and
+// reflect-101 addresses for a window that overlaps the border (the values of the reflected border
+// cv::buildOpticalFlowPyramid gives the search levels).  Jlane = level image + lane_row * Jpitch; offsets within one level
+// image fit 32 bits.
+__device__ __forceinline__ void gather_taps(const uint8_t* Jlane, int Jpitch, int lw, int lh, int jx,
+                                            int jy, int lane_row, int lane_col, bool packed_ok, unsigned& top, unsigned& bot) {
+    using kltsetup::WIN;
+    const int x = jx + lane_col;
+    if (jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh) {
+        const int o = jy * Jpitch;
+        if (packed_ok) {
+            const uint32_t* w = reinterpret_cast<const uint32_t*>(Jlane + (o + (x & ~3)));
+            const uint32_t* wb = reinterpret_cast<const uint32_t*>(Jlane + (o + Jpitch + (x & ~3)));
+            const unsigned sh = (unsigned)(x & 3) * 8u;
+            const unsigned t0 = __ldg(w), b0 = __ldg(wb);
+            unsigned t1 = 0, b1 = 0;
+            if (sh) { t1 = __ldg(w + 1); b1 = __ldg(wb + 1); }   // the next word may lie past the row's end when sh = 0
+            top = kltsetup::funnel_r(t0, t1, sh);
+            bot = kltsetup::funnel_r(b0, b1, sh);
+        } else {
+            const uint8_t* q = Jlane + (o + x);
+            top = __ldg(q) | (unsigned)__ldg(q + 1) << 8 | (unsigned)__ldg(q + 2) << 16 | (unsigned)__ldg(q + 3) << 24;
+            q += Jpitch;
+            bot = __ldg(q) | (unsigned)__ldg(q + 1) << 8 | (unsigned)__ldg(q + 2) << 16 | (unsigned)__ldg(q + 3) << 24;
+        }
+        return;
+    }
+    const uint8_t* r0 = Jlane + (kltsetup::reflect101_any(jy + lane_row, lh) - lane_row) * Jpitch;
+    const uint8_t* r1 = Jlane + (kltsetup::reflect101_any(jy + lane_row + 1, lh) - lane_row) * Jpitch;
+    top = 0;
+    bot = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int xr = kltsetup::reflect101_any(x + k, lw);
+        top |= (unsigned)__ldg(r0 + xr) << (8 * k);
+        bot |= (unsigned)__ldg(r1 + xr) << (8 * k);
+    }
+}
+
 // One calcOpticalFlowPyrLK track for one point (whole warp cooperates).
 // Ipyr = template pyramid, Jpyr = search pyramid.  nxt: in = initial guess, out = result.
+// COUNT (measurement instantiation): work gains 1 << 16 per level set-up that builds the template and 1 per iteration that
+// forms the mismatch sums (one register for both: the product instantiation has none to spare).
+template <bool COUNT>
 __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
-                         int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sP, int* sD, int lane) {
+                         int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sP, int* sD, int lane,
+                         int& work) {
     using kltsetup::WIN;
-    using kltsetup::DW;          // search patch width
     // lane l < 27 owns the three horizontally adjacent window pixels 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..),
-    // so the search-image taps of a lane are 4 consecutive bytes on two rows (packed fast path below); the integer
-    // window sums are order independent.
+    // so the search-image taps of a lane are 4 consecutive bytes on two rows; the integer window sums are order independent.
     constexpr int PER_LANE = 3;
     const float half = (WIN - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
+    // (double)minEig < 1e-4 <=> minEig < 0x1.a36e3p-14f, the smallest float >= 1e-4 (1e-4 is not a float)
+    const float MIN_EIG = 0x1.a36e3p-14f;
+    const int lane_row = lane / 3, lane_col = 3 * (lane - 3 * (lane / 3));
     bool status = true;
     float err = 0.f;
 
@@ -71,7 +117,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
         const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
         const bool packed_ok = ((reinterpret_cast<uintptr_t>(Jimg) | (uintptr_t)Jpitch) & 3) == 0;   // aliased level 0 may be unaligned
-        const int lane_row = lane / 3, lane_col = 3 * (lane - 3 * (lane / 3));
+        const uint8_t* Jlane = Jimg + lane_row * Jpitch;
         const float sc = 1.f / (float)(1 << level);
         float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
         float2 nextPt;
@@ -85,6 +131,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
             if (level == 0) { status = false; err = 0.f; }
             continue;
         }
+        if (COUNT) work += 1 << 16;
         float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
         int iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
         int iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
@@ -93,7 +140,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
 
         // ---- level set-up (klt_setup.cuh): 12 x 12 neighbourhood -> shared memory (aligned words on the
         //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window + exact
-        //      integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2.
+        //      integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2; lanes 27..31 get zeros.
         __syncwarp();
         const bool tmpl_aligned = ((reinterpret_cast<uintptr_t>(Iimg) | (uintptr_t)Ipitch) & 3) == 0;
         const int off = kltsetup::stage_patch(lane, Iimg, Ipitch, lw, lh, ix, iy, tmpl_aligned, sP);
@@ -118,101 +165,60 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         const bool b32 = __reduce_add_sync(FULL, sabs) < 262000;
         // |window sums| <= 81 * 4080^2 = 1.35e9 < 2^31 for the 9 x 9 window: one exact 32-bit redux each
         // (the b sums of the iterations can reach 2.7e9 and keep the split 64-bit reduction)
-        float A11 = __int2float_rn(__reduce_add_sync(FULL, sA11)) * FLT_SCALE;
-        float A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * FLT_SCALE;
-        float A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * FLT_SCALE;
+        const float A11 = __int2float_rn(__reduce_add_sync(FULL, sA11)) * FLT_SCALE;
+        const float A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * FLT_SCALE;
+        const float A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * FLT_SCALE;
         float D = A11 * A22 - A12 * A12;
-        float minEig = (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * WIN * WIN);
+        const float minEig = (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * WIN * WIN);
         err = minEig;
-        if ((double)minEig < 1e-4 || D < 1.1920928955078125e-07f) {
+        if (minEig < MIN_EIG || D < 1.1920928955078125e-07f) {
             if (level == 0) status = false;
             continue;
         }
         D = 1.f / D;
+        // the template values as the iterations use them: sign-extended once per level, not once per iteration
+        int I0 = Iv[0], I1 = Iv[1], I2 = Iv[2];
+        int X0 = Ixv[0], X1 = Ixv[1], X2 = Ixv[2];
+        int Y0 = Iyv[0], Y1 = Iyv[1], Y2 = Iyv[2];
         nextPt.x -= half;
         nextPt.y -= half;
         float2 prevDelta = make_float2(0.f, 0.f);
-        // the lane's packed search taps are kept while the integer origin (jx, jy) of the window does not move
-        // (sub-pixel steps only change the bilinear weights)
+        // The lane's taps are gathered when the integer origin (jx, jy) of the window moves and kept while it does not
+        // (sub-pixel steps only change the bilinear weights).  Lanes 27..31 keep zero taps against a zero template, so every
+        // lane runs the same straight-line arithmetic.  nxt is written where the loop ends, not every iteration: the
+        // values are those OpenCV leaves in nextPts at each exit.
         int cjx = INT_MIN, cjy = INT_MIN;
         unsigned top = 0, bot = 0;
-        for (int j = 0; j < max_iter; ++j) {
+        int j = 0;
+        for (; j < max_iter; ++j) {
             const int jx = __float2int_rd(nextPt.x), jy = __float2int_rd(nextPt.y);
-            const bool same = (jx == cjx) & (jy == cjy);
-            if (!same && (jx < -WIN || jx >= lw || jy < -WIN || jy >= lh)) {
-                if (level == 0) status = false;
-                break;
+            if ((jx != cjx) | (jy != cjy)) {
+                if (jx < -WIN || jx >= lw || jy < -WIN || jy >= lh) {
+                    if (j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
+                    if (level == 0) status = false;
+                    break;
+                }
+                if (lane < 27) gather_taps(Jlane, Jpitch, lw, lh, jx, jy, lane_row, lane_col, packed_ok, top, bot);
+                cjx = jx;
+                cjy = jy;
             }
+            if (COUNT) ++work;
             a = nextPt.x - (float)jx;
             b = nextPt.y - (float)jy;
             iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
             iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
             iw10 = __float2int_rn((1.f - a) * b * 16384.f);
             iw11 = 16384 - iw00 - iw01 - iw10;
-            int sb1 = 0, sb2 = 0;
-            if (same || (packed_ok && jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh)) {
-                // interior, word-aligned level (warp-uniform): the lane's 4 + 4 taps come from two aligned
-                // 32-bit words per row (funnel shift), the 14-bit bilinear weights are applied with
-                // dp2a (u16 x u8 pairs): 4 loads + 6 dp2a per lane instead of 12 byte loads + 12 IMADs.
-                // Same integers as the byte path (signed 16-bit weights x unsigned bytes, exact in int32).
-                if (lane < 27) {
-                    if (!same) {
-                        const uint8_t* q = Jimg + (size_t)(jy + lane_row) * Jpitch + (jx + lane_col);
-                        const uintptr_t qa = reinterpret_cast<uintptr_t>(q);
-                        const unsigned sh = (unsigned)(qa & 3) * 8u;
-                        const uint32_t* w = reinterpret_cast<const uint32_t*>(qa & ~(uintptr_t)3);
-                        const uint32_t* wb = reinterpret_cast<const uint32_t*>((qa & ~(uintptr_t)3) + Jpitch);
-                        const unsigned t0 = __ldg(w), b0 = __ldg(wb);
-                        unsigned t1 = 0, b1w = 0;
-                        if (sh) { t1 = __ldg(w + 1); b1w = __ldg(wb + 1); }
-                        top = kltsetup::funnel_r(t0, t1, sh);
-                        bot = kltsetup::funnel_r(b0, b1w, sh);
-                    }
-                    const unsigned W01 = ((unsigned)iw00 & 0xFFFFu) | ((unsigned)iw01 << 16);
-                    const unsigned W23 = ((unsigned)iw10 & 0xFFFFu) | ((unsigned)iw11 << 16);
-                    const int j0 = kltsetup::dp2a_lo_su16(W01, top, kltsetup::dp2a_lo_su16(W23, bot, 256)) >> 9;
-                    const int j1 = kltsetup::dp2a_lo_su16(W01, top >> 8, kltsetup::dp2a_lo_su16(W23, bot >> 8, 256)) >> 9;
-                    const int j2 = kltsetup::dp2a_hi_su16(W01, top, kltsetup::dp2a_hi_su16(W23, bot, 256)) >> 9;
-                    const int d0 = j0 - (int)Iv[0], d1 = j1 - (int)Iv[1], d2 = j2 - (int)Iv[2];
-                    sb1 = d0 * (int)Ixv[0] + d1 * (int)Ixv[1] + d2 * (int)Ixv[2];
-                    sb2 = d0 * (int)Iyv[0] + d1 * (int)Iyv[1] + d2 * (int)Iyv[2];
-                }
-                cjx = jx;
-                cjy = jy;
-            } else if (jx >= 0 && jy >= 0 && jx + WIN < lw && jy + WIN < lh) {
-                // interior (warp-uniform): every lane gathers its own 4 taps straight from L1/L2
-                if (lane < 27) {
-                    const uint8_t* src = Jimg + (size_t)(jy + lane_row) * Jpitch + (jx + lane_col);
-#pragma unroll
-                    for (int k = 0; k < PER_LANE; ++k) {
-                        const uint8_t* q = src + k;
-                        int jval = ((int)__ldg(q) * iw00 + (int)__ldg(q + 1) * iw01 + (int)__ldg(q + Jpitch) * iw10 +
-                                    (int)__ldg(q + Jpitch + 1) * iw11 + (1 << 8)) >> 9;
-                        int diff = jval - (int)Iv[k];
-                        sb1 += diff * (int)Ixv[k];
-                        sb2 += diff * (int)Iyv[k];
-                    }
-                }
-            } else {
-                __syncwarp();
-                for (int i = lane; i < DW * DW; i += 32) {
-                    int r = i / DW, c = i - r * DW;
-                    int y = kltsetup::reflect101_any(jy + r, lh), x = kltsetup::reflect101_any(jx + c, lw);
-                    sP[i] = __ldg(Jimg + (size_t)y * Jpitch + x);
-                }
-                __syncwarp();
-                if (lane < 27) {
-                    const uint8_t* src = sP + lane_row * DW + lane_col;
-#pragma unroll
-                    for (int k = 0; k < PER_LANE; ++k) {
-                        const uint8_t* q = src + k;
-                        int jval = ((int)q[0] * iw00 + (int)q[1] * iw01 + (int)q[DW] * iw10 + (int)q[DW + 1] * iw11 + (1 << 8)) >> 9;
-                        int diff = jval - (int)Iv[k];
-                        sb1 += diff * (int)Ixv[k];
-                        sb2 += diff * (int)Iyv[k];
-                    }
-                }
-            }
+            // the 14-bit bilinear weights as signed 16-bit pairs, applied to the packed taps with dp2a (u16 x u8 pairs):
+            // the same integers as (J00 iw00 + J01 iw01 + J10 iw10 + J11 iw11 + 2^8) >> 9, exact in int32
+            const unsigned W01 = __byte_perm((unsigned)iw00, (unsigned)iw01, 0x5410);
+            const unsigned W23 = __byte_perm((unsigned)iw10, (unsigned)iw11, 0x5410);
+            const int j0 = kltsetup::dp2a_lo_su16(W01, top, kltsetup::dp2a_lo_su16(W23, bot, 256)) >> 9;
+            const int j1 = kltsetup::dp2a_lo_su16(W01, top >> 8, kltsetup::dp2a_lo_su16(W23, bot >> 8, 256)) >> 9;
+            const int j2 = kltsetup::dp2a_hi_su16(W01, top, kltsetup::dp2a_hi_su16(W23, bot, 256)) >> 9;
+            const int d0 = j0 - I0, d1 = j1 - I1, d2 = j2 - I2;
+            const int sb1 = d0 * X0 + d1 * X1 + d2 * X2;
+            const int sb2 = d0 * Y0 + d1 * Y1 + d2 * Y2;
             float b1, b2;
             if (b32) {
                 b1 = __int2float_rn(__reduce_add_sync(FULL, sb1)) * FLT_SCALE;
@@ -221,35 +227,35 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
                 b1 = __ll2float_rn(warp_sum64(sb1)) * FLT_SCALE;
                 b2 = __ll2float_rn(warp_sum64(sb2)) * FLT_SCALE;
             }
-            float2 delta = make_float2((A12 * b2 - A22 * b1) * D, (A12 * b1 - A11 * b2) * D);
+            const float2 delta = make_float2((A12 * b2 - A22 * b1) * D, (A12 * b1 - A11 * b2) * D);
             nextPt.x += delta.x;
             nextPt.y += delta.y;
-            nxt = make_float2(nextPt.x + half, nextPt.y + half);
             // delta.ddot(delta) <= epsilon^2 is a double comparison in OpenCV; a float evaluation (relative error
             // < 2e-7) decides it except within 1e-6 of the threshold, where the double expression is evaluated
-            {
-                const float q = delta.x * delta.x + delta.y * delta.y;
-                bool conv;
-                if (q < eps_lo) conv = true;
-                else if (q > eps_hi) conv = false;
-                else conv = (double)delta.x * (double)delta.x + (double)delta.y * (double)delta.y <= eps2;
-                if (conv) break;
+            const float q = delta.x * delta.x + delta.y * delta.y;
+            bool conv = q < eps_lo;
+            if (!conv && !(q > eps_hi)) conv = (double)delta.x * (double)delta.x + (double)delta.y * (double)delta.y <= eps2;
+            if (conv) {
+                nxt = make_float2(nextPt.x + half, nextPt.y + half);
+                break;
             }
             // (double)|f| < 0.01  <=>  |f| <= 0.01f: 0.01f = 0.00999999977... is the largest float below 0.01
             if (j > 0 && fabsf(delta.x + prevDelta.x) <= 0.01f && fabsf(delta.y + prevDelta.y) <= 0.01f) {
-                nxt.x -= delta.x * 0.5f;
-                nxt.y -= delta.y * 0.5f;
+                nxt = make_float2((nextPt.x + half) - delta.x * 0.5f, (nextPt.y + half) - delta.y * 0.5f);
                 break;
             }
             prevDelta = delta;
         }
+        if (j == max_iter && j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
     }
     err_out = err;
     return status;
 }
 
 // One keypoint, whole warp: forward track, checks, backward track, forward-backward test (feature_tracker.cpp:35-137).
-__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane) {
+// counts (measurement instantiation): level set-ups and iterations of both tracks, at 2 i and 2 i + 1.
+template <bool COUNT>
+__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane, int32_t* counts) {
     const int frame = A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame;
     int maxlevel = A.lvls ? (int)A.lvls[i] : A.lvl_all;
     if (maxlevel > A.prev.nlev - 1) maxlevel = A.prev.nlev - 1;  // feature_tracker.cpp:50-52
@@ -257,10 +263,11 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     const float2 kp = A.kps[i];
     float2 fwd = A.priors[i];
     float err = 0.f;
+    int work = 0;
     // x < 0 marks an empty slot of a fixed-stride batch (the detectors pad their output with (-1, -1),
     // ov2_describe uses the same rule): status 0, prior untouched, no work
-    bool ok = kp.x >= 0.f &&
-              lk_track(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err, sPw, sDw, lane);
+    bool ok = kp.x >= 0.f && lk_track<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
+                                             err, sPw, sDw, lane, work);
     // feature_tracker.cpp:79-101
     if (ok && err > A.ferr) ok = false;
     if (ok) {
@@ -271,7 +278,8 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
         // backward: template from the current image at the forward result, search the previous image
         float2 back = kp;
         float err2 = 0.f;
-        bool ok2 = lk_track(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw, lane);
+        bool ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw,
+                                   lane, work);
         if (!ok2) ok = false;
         else {
             float dx = kp.x - back.x, dy = kp.y - back.y;
@@ -282,26 +290,34 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     if (lane == 0) {
         A.priors[i] = fwd;
         A.status[i] = ok ? 1 : 0;
+        if (COUNT) {
+            counts[2 * i] = work >> 16;
+            counts[2 * i + 1] = work & 0xFFFF;
+        }
     }
 }
 
 // Keypoints need very different iteration counts (1 .. 30 per level), so a static warp <-> keypoint
 // assignment leaves SM slots idle while the slowest warp of a CTA finishes.  When the grid exceeds the
-// resident CTAs, the launch fills the GPU once and every warp pulls the next keypoint from a global counter.
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A) {
+// resident CTAs, the launch fills the GPU once and every warp pulls the next keypoint from a global counter;
+// it asks for the next index before tracking the current one, so the atomic's round trip overlaps the track.
+template <bool COUNT>
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A, int32_t* counts) {
     __shared__ __align__(16) uint8_t sPall[WARPS_PER_CTA][kltsetup::SP_BYTES];
     __shared__ __align__(16) int sDall[WARPS_PER_CTA][kltsetup::SD_INTS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int i = blockIdx.x * WARPS_PER_CTA + warp;;) {
-        if (A.work_counter) {
-            int nxt_i = 0;
-            if (lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
-            i = __shfl_sync(FULL, nxt_i, 0);
-        }
-        if (i >= A.n) return;
-        klt_one(A, i, sPall[warp], sDall[warp], lane);
+    int i = blockIdx.x * WARPS_PER_CTA + warp;
+    if (A.work_counter) {
+        int first = 0;
+        if (lane == 0) first = atomicAdd(A.work_counter, 1);
+        i = __shfl_sync(FULL, first, 0);
+    }
+    while (i < A.n) {
+        int nxt_i = 0;
+        if (A.work_counter && lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
+        klt_one<COUNT>(A, i, sPall[warp], sDall[warp], lane, counts);
         if (!A.work_counter) return;
-        __syncwarp();
+        i = __shfl_sync(FULL, nxt_i, 0);
     }
 }
 
@@ -314,11 +330,10 @@ int optflow_levels(const ov2_pyr* p, int win, int maxlevel) {
     return maxlevel;
 }
 
-}  // namespace
-
-extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
-                                 int n, const int32_t* frame_idx, int first_frame, int per_frame, const uint8_t* nbpyrlvl,
-                                 int nbpyrlvl_all, const float* kps, float* priors_inout, uint8_t* status_out) {
+// ov2_fb_klt, and with counts_out the counting instantiation of the kernel behind ov2_debug_klt_counts
+ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm, int n,
+                      const int32_t* frame_idx, int first_frame, int per_frame, const uint8_t* nbpyrlvl, int nbpyrlvl_all,
+                      const float* kps, float* priors_inout, uint8_t* status_out, int32_t* counts_out) {
     if (!ctx || !prev || !cur || !prm || n < 0) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: bad arguments");
     if (n == 0) return OV2_OK;  // feature_tracker.cpp:43-46
     if (!kps || !priors_inout || !status_out || (!frame_idx && per_frame <= 0))
@@ -357,9 +372,14 @@ extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_py
     A.priors = (float2*)o;
     if ((st = ov2_stage_out(ctx, status_out, (size_t)n, &o)) != OV2_OK) return st;
     A.status = (uint8_t*)o;
+    int32_t* d_counts = nullptr;
+    if (counts_out) {
+        if ((st = ov2_stage_out(ctx, counts_out, sizeof(int32_t) * 2 * (size_t)n, &o)) != OV2_OK) return st;
+        d_counts = (int32_t*)o;
+    }
     int grid = div_up(n, WARPS_PER_CTA), per_sm = 0;
     A.work_counter = nullptr;
-    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel, WARPS_PER_CTA * 32, 0));
+    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false>, WARPS_PER_CTA * 32, 0));
     const int resident = per_sm * ctx->sm_count;
     if (grid > resident) {
         if ((st = ov2_scratch(ctx, sizeof(int), &o)) != OV2_OK) return st;
@@ -367,6 +387,30 @@ extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_py
         OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
         grid = resident;
     }
-    OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A)));
+    if (d_counts)
+        OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<true><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, d_counts)));
+    else
+        OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, nullptr)));
     return ov2_end(ctx);
+}
+
+}  // namespace
+
+extern "C" ov2_status ov2_fb_klt(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
+                                 int n, const int32_t* frame_idx, int first_frame, int per_frame, const uint8_t* nbpyrlvl,
+                                 int nbpyrlvl_all, const float* kps, float* priors_inout, uint8_t* status_out) {
+    return klt_launch(ctx, prev, cur, prm, n, frame_idx, first_frame, per_frame, nbpyrlvl, nbpyrlvl_all, kps, priors_inout,
+                      status_out, nullptr);
+}
+
+// Measurement hook: ov2_fb_klt with the same arguments and results, plus the work each keypoint took: counts_out[2 i] level
+// set-ups (template built) and counts_out[2 i + 1] iterations (mismatch sums formed), forward and backward tracks together.
+// A second instantiation of the kernel: the product launch carries no counter.
+extern "C" ov2_status ov2_debug_klt_counts(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm,
+                                           int n, const int32_t* frame_idx, int first_frame, int per_frame,
+                                           const uint8_t* nbpyrlvl, int nbpyrlvl_all, const float* kps, float* priors_inout,
+                                           uint8_t* status_out, int32_t* counts_out) {
+    if (!counts_out && n > 0) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_debug_klt_counts: null counts array");
+    return klt_launch(ctx, prev, cur, prm, n, frame_idx, first_frame, per_frame, nbpyrlvl, nbpyrlvl_all, kps, priors_inout,
+                      status_out, counts_out);
 }

@@ -12,6 +12,9 @@ that) and prints one JSON line:
                         levels 1-3 written once, for both images of every pair
   subpix                mean and histogram of cornerSubPix iterations per detected point (counting instantiation of the
                         kernel, run once on the step's integer detections; the product launch carries no counter)
+  klt                   level set-ups and Lucas-Kanade iterations per keypoint, forward and backward tracks together: means
+                        and histograms (counting instantiation of fb_klt_kernel, run once on the step's own keypoints,
+                        priors and depths; the product launch carries no counter)
   gpu                   card name, power limit and maximum SM clock, read in the same run
 
 Writes nothing."""
@@ -100,10 +103,27 @@ def main():
               "histogram": {str(k): int(v) for k, v in enumerate(np.bincount(it, minlength=31)) if v},
               "counting_kernel_matches_product": same}
 
+    # fb-KLT work on the step's own keypoints, priors and pyramid depths
+    n = B * bench.NKP
+    d_pri = wl.d_pri0.clone()
+    d_st = torch.empty(n, dtype=torch.uint8, device="cuda")
+    d_cnt = torch.empty((n, 2), dtype=torch.int32, device="cuda")
+    wl.ft.fb_klt_tracking(wl.pyr_prev_d, wl.pyr_cur_d, 9, wl.d_lv, 30.0, 0.5, wl.d_kps, d_pri, d_st, n=n, per_frame=bench.NKP,
+                          counts_out=d_cnt)
+    wl.d_pri.copy_(wl.d_pri0)
+    wl.ft.fb_klt_tracking(wl.pyr_prev_d, wl.pyr_cur_d, 9, wl.d_lv, 30.0, 0.5, wl.d_kps, wl.d_pri, wl.d_status, n=n,
+                          per_frame=bench.NKP)
+    torch.cuda.synchronize()
+    cnt = d_cnt.cpu().numpy()
+    klt = {"keypoints": int(n), "mean_setups": float(cnt[:, 0].mean()), "mean_iterations": float(cnt[:, 1].mean()),
+           "setups_histogram": {str(k): int(v) for k, v in enumerate(np.bincount(cnt[:, 0])) if v},
+           "iterations_histogram": {str(k): int(v) for k, v in enumerate(np.bincount(cnt[:, 1])) if v},
+           "counting_kernel_matches_product": bool(torch.equal(d_pri, wl.d_pri) and torch.equal(d_st, wl.d_status))}
+
     wl.close()
     ctx.close()
     print(json.dumps({"gpu": gpu[0] if gpu else None, "batch": B, "image": [W, H], "steps": args.steps, "step_ms": step_ms,
-                      "kernels_ms_sum": ksum, "kernels_ms_per_step": kernels, "pyramid": pyr, "subpix": subpix,
+                      "kernels_ms_sum": ksum, "kernels_ms_per_step": kernels, "pyramid": pyr, "subpix": subpix, "klt": klt,
                       "command": "python scripts/bench_step_kernels.py " + " ".join(sys.argv[1:])}), flush=True)
     return 0
 
