@@ -148,7 +148,8 @@ OV2_API ov2_status ov2_pyr_build_remap(ov2_ctx* ctx, ov2_pyr* pyr, const ov2_rem
  * USE_INITIAL_FLOW|LK_GET_MIN_EIGENVALS, the status/err/inBorder filter, the level-0 backward
  * pass and the forward-backward distance test, fused per keypoint. */
 typedef struct {
-    int   win;        /* nwinsize (9) */
+    int   win;        /* nwinsize: any size from 3 to 31, even sizes included (Size(win, win)); OV2_ERR_INVALID outside
+                         that range.  9 (every shipped configuration) runs its own kernel, every other size a general one */
     int   max_iter;   /* klt_convg_crit_.maxCount (30) */
     float eps;        /* klt_convg_crit_.epsilon (0.01f) */
     float ferr;       /* nklt_err (30) */

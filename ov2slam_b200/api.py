@@ -372,7 +372,8 @@ class FeatureTracker:
 
     def fb_klt_tracking(self, prev: Pyramid, cur: Pyramid, nwinsize, nbpyrlvl, ferr, fmax_fbklt_dist,
                         kps, priors_inout, status_out, n=None, frame_idx=None, first_frame=0, per_frame=None, counts_out=None):
-        """fbKltTracking over a (ragged or fixed-stride) batch.  nbpyrlvl: int or per-keypoint uint8
+        """fbKltTracking over a (ragged or fixed-stride) batch.  nwinsize: 3 .. 31, even sizes included (Ov2Error
+        otherwise).  nbpyrlvl: int or per-keypoint uint8
         array.  kps / priors_inout: (n, 2) float32; status_out: (n,) uint8.  Arrays may be numpy
         (host) or CUDA tensors (device).  counts_out ((n, 2) int32, measurement only): the same tracking through the
         counting kernel, which also returns each keypoint's level set-ups and iterations (forward + backward)."""

@@ -15,6 +15,11 @@
 // Scharr derivatives are computed on the fly from a 12x12 8-bit neighbourhood (reflect-101 at
 // the image edge, constant 0 outside the image - exactly the planes buildOpticalFlowPyramid
 // would have materialised), so the tracker reads only the 8-bit pyramid.
+//
+// Two kernels: fb_klt_kernel for the 9 x 9 window of every shipped configuration (three window pixels per lane, search
+// taps packed in registers), and fb_klt_win_kernel for every other window from 3 x 3 to 31 x 31 (lane c owns window
+// column c; template and staged image bytes in shared memory).  ov2_fb_klt picks one from nwinsize.  Both share the
+// per-keypoint forward / backward logic and the float32 steps below.
 #include <climits>
 #include "ov2_common.cuh"
 #include "klt_setup.cuh"
@@ -49,6 +54,41 @@ __device__ __forceinline__ long long warp_sum64(int s) {
     int shi = __reduce_add_sync(FULL, hi);
     return ((long long)shi << 16) + (long long)slo;
 }
+
+// ---- OpenCV's float32 steps of one LK level, shared by both trackers.  The weights, convergence and oscillation tests
+// are macros rather than inline functions: as calls they change how fb_klt_kernel is scheduled.
+
+// 14-bit bilinear weights of the sub-pixel offsets (a, b)
+#define LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11)                  \
+    iw00 = __float2int_rn((1.f - (a)) * (1.f - (b)) * 16384.f);  \
+    iw01 = __float2int_rn((a) * (1.f - (b)) * 16384.f);          \
+    iw10 = __float2int_rn((1.f - (a)) * (b) * 16384.f);          \
+    iw11 = 16384 - iw00 - iw01 - iw10
+
+// The minimal eigenvalue of the normal matrix over a win x win window (the error LK_GET_MIN_EIGENVALS reports).  A level
+// whose minEig < LK_MIN_EIG or determinant < LK_MIN_DET (FLT_EPSILON) is dropped.
+// (double)minEig < 1e-4 <=> minEig < 0x1.a36e3p-14f, the smallest float >= 1e-4 (1e-4 is not a float)
+__device__ __forceinline__ float lk_min_eig(float A11, float A12, float A22, int win) {
+    return (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * win * win);
+}
+constexpr float LK_MIN_EIG = 0x1.a36e3p-14f;
+constexpr float LK_MIN_DET = 1.1920928955078125e-07f;
+
+// the step from the mismatch sums, D = 1 / det
+__device__ __forceinline__ float2 lk_step(float A11, float A12, float A22, float D, float b1, float b2) {
+    return make_float2((A12 * b2 - A22 * b1) * D, (A12 * b1 - A11 * b2) * D);
+}
+
+// Declares bool conv: delta.ddot(delta) <= epsilon^2, a double comparison in OpenCV.  A float evaluation (relative error
+// < 2e-7) decides it except within 1e-6 of the threshold (eps_lo .. eps_hi), where the double expression is evaluated.
+#define LK_CONVERGED(conv, delta, eps2, eps_lo, eps_hi)                                                        \
+    const float conv##_q = (delta).x * (delta).x + (delta).y * (delta).y;                                        \
+    bool conv = conv##_q < (eps_lo);                                                                             \
+    if (!conv && !(conv##_q > (eps_hi)))                                                                         \
+    conv = (double)(delta).x * (double)(delta).x + (double)(delta).y * (double)(delta).y <= (eps2)
+
+// (double)|f| < 0.01  <=>  |f| <= 0.01f: 0.01f = 0.00999999977... is the largest float below 0.01
+#define LK_OSCILLATES(delta, prev) (fabsf((delta).x + (prev).x) <= 0.01f && fabsf((delta).y + (prev).y) <= 0.01f)
 
 // The lane's search taps for the window origin (jx, jy): rows jy + lane_row and +1, columns jx + lane_col .. +3, four bytes
 // per row packed into one word each (byte k = column jx + lane_col + k).  Three ways to the same bytes, chosen per origin
@@ -95,6 +135,8 @@ __device__ __forceinline__ void gather_taps(const uint8_t* Jlane, int Jpitch, in
 // Ipyr = template pyramid, Jpyr = search pyramid.  nxt: in = initial guess, out = result.
 // COUNT (measurement instantiation): work gains 1 << 16 per level set-up that builds the template and 1 per iteration that
 // forms the mismatch sums (one register for both: the product instantiation has none to spare).
+// lk_track_win repeats this level / iteration control flow (bounds tests, nxt at each exit, convergence, oscillation,
+// max_iter) for the other window sizes: a change to it here belongs there too.
 template <bool COUNT>
 __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
                          int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sP, int* sD, int lane,
@@ -105,8 +147,6 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
     constexpr int PER_LANE = 3;
     const float half = (WIN - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
-    // (double)minEig < 1e-4 <=> minEig < 0x1.a36e3p-14f, the smallest float >= 1e-4 (1e-4 is not a float)
-    const float MIN_EIG = 0x1.a36e3p-14f;
     const int lane_row = lane / 3, lane_col = 3 * (lane - 3 * (lane / 3));
     bool status = true;
     float err = 0.f;
@@ -133,10 +173,8 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         }
         if (COUNT) work += 1 << 16;
         float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
-        int iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
-        int iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
-        int iw10 = __float2int_rn((1.f - a) * b * 16384.f);
-        int iw11 = 16384 - iw00 - iw01 - iw10;
+        int iw00, iw01, iw10, iw11;
+        LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
 
         // ---- level set-up (klt_setup.cuh): 12 x 12 neighbourhood -> shared memory (aligned words on the
         //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window + exact
@@ -169,9 +207,9 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         const float A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * FLT_SCALE;
         const float A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * FLT_SCALE;
         float D = A11 * A22 - A12 * A12;
-        const float minEig = (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * WIN * WIN);
+        const float minEig = lk_min_eig(A11, A12, A22, WIN);
         err = minEig;
-        if (minEig < MIN_EIG || D < 1.1920928955078125e-07f) {
+        if (minEig < LK_MIN_EIG || D < LK_MIN_DET) {
             if (level == 0) status = false;
             continue;
         }
@@ -205,10 +243,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
             if (COUNT) ++work;
             a = nextPt.x - (float)jx;
             b = nextPt.y - (float)jy;
-            iw00 = __float2int_rn((1.f - a) * (1.f - b) * 16384.f);
-            iw01 = __float2int_rn(a * (1.f - b) * 16384.f);
-            iw10 = __float2int_rn((1.f - a) * b * 16384.f);
-            iw11 = 16384 - iw00 - iw01 - iw10;
+            LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
             // the 14-bit bilinear weights as signed 16-bit pairs, applied to the packed taps with dp2a (u16 x u8 pairs):
             // the same integers as (J00 iw00 + J01 iw01 + J10 iw10 + J11 iw11 + 2^8) >> 9, exact in int32
             const unsigned W01 = __byte_perm((unsigned)iw00, (unsigned)iw01, 0x5410);
@@ -227,20 +262,120 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
                 b1 = __ll2float_rn(warp_sum64(sb1)) * FLT_SCALE;
                 b2 = __ll2float_rn(warp_sum64(sb2)) * FLT_SCALE;
             }
-            const float2 delta = make_float2((A12 * b2 - A22 * b1) * D, (A12 * b1 - A11 * b2) * D);
+            const float2 delta = lk_step(A11, A12, A22, D, b1, b2);
             nextPt.x += delta.x;
             nextPt.y += delta.y;
-            // delta.ddot(delta) <= epsilon^2 is a double comparison in OpenCV; a float evaluation (relative error
-            // < 2e-7) decides it except within 1e-6 of the threshold, where the double expression is evaluated
-            const float q = delta.x * delta.x + delta.y * delta.y;
-            bool conv = q < eps_lo;
-            if (!conv && !(q > eps_hi)) conv = (double)delta.x * (double)delta.x + (double)delta.y * (double)delta.y <= eps2;
+            LK_CONVERGED(conv, delta, eps2, eps_lo, eps_hi);
             if (conv) {
                 nxt = make_float2(nextPt.x + half, nextPt.y + half);
                 break;
             }
-            // (double)|f| < 0.01  <=>  |f| <= 0.01f: 0.01f = 0.00999999977... is the largest float below 0.01
-            if (j > 0 && fabsf(delta.x + prevDelta.x) <= 0.01f && fabsf(delta.y + prevDelta.y) <= 0.01f) {
+            if (j > 0 && LK_OSCILLATES(delta, prevDelta)) {
+                nxt = make_float2((nextPt.x + half) - delta.x * 0.5f, (nextPt.y + half) - delta.y * 0.5f);
+                break;
+            }
+            prevDelta = delta;
+        }
+        if (j == max_iter && j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
+    }
+    err_out = err;
+    return status;
+}
+
+// One calcOpticalFlowPyrLK track with a win x win window, 3 <= win <= 31, any size but 9 (whole warp cooperates).  Lane c
+// owns window column c (klt_setup.cuh, win_*): the level set-up stages the (win + 3)^2 template neighbourhood, its Scharr
+// derivatives and the template into the warp's shared memory, and each move of the integer search origin stages the
+// (win + 1)^2 search bytes into the neighbourhood's buffer.  A lane's column sums are exact in int32, the window sums in
+// 64 bits.  Float32 steps and COUNT as in lk_track.  The level / iteration control flow repeats lk_track's (kept apart so that
+// fb_klt_kernel's code stays as it is): a change to it here belongs there too.
+template <bool COUNT>
+__device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
+                             int win, int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sN,
+                             int* sD, int lane, int& work) {
+    int* sG = sD + kltsetup::WD_INTS;
+    short* sI = reinterpret_cast<short*>(sG + kltsetup::WT_ELEMS);
+    const float half = (win - 1) * 0.5f;
+    const float FLT_SCALE = 1.f / (1 << 20);
+    bool status = true;
+    float err = 0.f;
+
+    for (int level = maxlevel; level >= 0; --level) {
+        const int lw = Ipyr.w[level], lh = Ipyr.h[level];
+        const uint8_t* Iimg = Ipyr.lvl[level] + Ipyr.fstride[level] * frame;
+        const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
+        const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
+        const float sc = 1.f / (float)(1 << level);
+        float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
+        float2 nextPt;
+        if (level == maxlevel) nextPt = make_float2(nxt.x * sc, nxt.y * sc);
+        else nextPt = make_float2(nxt.x * 2.f, nxt.y * 2.f);
+        nxt = nextPt;
+        prevPt.x -= half;
+        prevPt.y -= half;
+        const int ix = __float2int_rd(prevPt.x), iy = __float2int_rd(prevPt.y);
+        if (ix < -win || ix >= lw || iy < -win || iy >= lh) {
+            if (level == 0) { status = false; err = 0.f; }
+            continue;
+        }
+        if (COUNT) work += 1 << 16;
+        float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
+        int iw00, iw01, iw10, iw11;
+        LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
+        __syncwarp();                    // the previous level's iterations are done with sN
+        kltsetup::win_stage(lane, Iimg, Ipitch, lw, lh, ix - 1, iy - 1, win + 3, sN);
+        __syncwarp();
+        kltsetup::win_scharr(lane, sN, ix, iy, lw, lh, win, sD);
+        __syncwarp();
+        int sA11, sA12, sA22;
+        kltsetup::win_template(lane, sN, sD, win, iw00, iw01, iw10, iw11, sI, sG, sA11, sA12, sA22);
+        const float A11 = __ll2float_rn(warp_sum64(sA11)) * FLT_SCALE;
+        const float A12 = __ll2float_rn(warp_sum64(sA12)) * FLT_SCALE;
+        const float A22 = __ll2float_rn(warp_sum64(sA22)) * FLT_SCALE;
+        float D = A11 * A22 - A12 * A12;
+        const float minEig = lk_min_eig(A11, A12, A22, win);
+        err = minEig;
+        if (minEig < LK_MIN_EIG || D < LK_MIN_DET) {
+            if (level == 0) status = false;
+            continue;
+        }
+        D = 1.f / D;
+        nextPt.x -= half;
+        nextPt.y -= half;
+        float2 prevDelta = make_float2(0.f, 0.f);
+        // search bytes are staged when the integer origin (jx, jy) moves and kept while it does not
+        int cjx = INT_MIN, cjy = INT_MIN;
+        int j = 0;
+        for (; j < max_iter; ++j) {
+            const int jx = __float2int_rd(nextPt.x), jy = __float2int_rd(nextPt.y);
+            if ((jx != cjx) | (jy != cjy)) {
+                if (jx < -win || jx >= lw || jy < -win || jy >= lh) {
+                    if (j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
+                    if (level == 0) status = false;
+                    break;
+                }
+                __syncwarp();            // the template phase or the previous iteration is done with sN
+                kltsetup::win_stage(lane, Jimg, Jpitch, lw, lh, jx, jy, win + 1, sN);
+                __syncwarp();
+                cjx = jx;
+                cjy = jy;
+            }
+            if (COUNT) ++work;
+            a = nextPt.x - (float)jx;
+            b = nextPt.y - (float)jy;
+            LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
+            int sb1, sb2;
+            kltsetup::win_mismatch(lane, sN, sI, sG, win, iw00, iw01, iw10, iw11, sb1, sb2);
+            const float b1 = __ll2float_rn(warp_sum64(sb1)) * FLT_SCALE;
+            const float b2 = __ll2float_rn(warp_sum64(sb2)) * FLT_SCALE;
+            const float2 delta = lk_step(A11, A12, A22, D, b1, b2);
+            nextPt.x += delta.x;
+            nextPt.y += delta.y;
+            LK_CONVERGED(conv, delta, eps2, eps_lo, eps_hi);
+            if (conv) {
+                nxt = make_float2(nextPt.x + half, nextPt.y + half);
+                break;
+            }
+            if (j > 0 && LK_OSCILLATES(delta, prevDelta)) {
                 nxt = make_float2((nextPt.x + half) - delta.x * 0.5f, (nextPt.y + half) - delta.y * 0.5f);
                 break;
             }
@@ -254,8 +389,9 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
 
 // One keypoint, whole warp: forward track, checks, backward track, forward-backward test (feature_tracker.cpp:35-137).
 // counts (measurement instantiation): level set-ups and iterations of both tracks, at 2 i and 2 i + 1.
-template <bool COUNT>
-__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane, int32_t* counts) {
+// ANY_WIN: track with lk_track_win and a win x win window, else with lk_track (9 x 9).
+template <bool COUNT, bool ANY_WIN>
+__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane, int32_t* counts, int win) {
     const int frame = A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame;
     int maxlevel = A.lvls ? (int)A.lvls[i] : A.lvl_all;
     if (maxlevel > A.prev.nlev - 1) maxlevel = A.prev.nlev - 1;  // feature_tracker.cpp:50-52
@@ -266,8 +402,13 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     int work = 0;
     // x < 0 marks an empty slot of a fixed-stride batch (the detectors pad their output with (-1, -1),
     // ov2_describe uses the same rule): status 0, prior untouched, no work
-    bool ok = kp.x >= 0.f && lk_track<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
-                                             err, sPw, sDw, lane, work);
+    bool ok;
+    if constexpr (ANY_WIN)
+        ok = kp.x >= 0.f && lk_track_win<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, win, A.max_iter, A.eps2, A.eps_lo,
+                                                A.eps_hi, err, sPw, sDw, lane, work);
+    else
+        ok = kp.x >= 0.f && lk_track<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
+                                            err, sPw, sDw, lane, work);
     // feature_tracker.cpp:79-101
     if (ok && err > A.ferr) ok = false;
     if (ok) {
@@ -278,8 +419,13 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
         // backward: template from the current image at the forward result, search the previous image
         float2 back = kp;
         float err2 = 0.f;
-        bool ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw,
-                                   lane, work);
+        bool ok2;
+        if constexpr (ANY_WIN)
+            ok2 = lk_track_win<COUNT>(A.cur, A.prev, frame, fwd, back, 0, win, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw,
+                                      sDw, lane, work);
+        else
+            ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw,
+                                  lane, work);
         if (!ok2) ok = false;
         else {
             float dx = kp.x - back.x, dy = kp.y - back.y;
@@ -301,12 +447,10 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
 // assignment leaves SM slots idle while the slowest warp of a CTA finishes.  When the grid exceeds the
 // resident CTAs, the launch fills the GPU once and every warp pulls the next keypoint from a global counter;
 // it asks for the next index before tracking the current one, so the atomic's round trip overlaps the track.
-template <bool COUNT>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A, int32_t* counts) {
-    __shared__ __align__(16) uint8_t sPall[WARPS_PER_CTA][kltsetup::SP_BYTES];
-    __shared__ __align__(16) int sDall[WARPS_PER_CTA][kltsetup::SD_INTS];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int i = blockIdx.x * WARPS_PER_CTA + warp;
+// Both kernels run their warps through this loop: NW warps per CTA, sPw / sDw the warp's shared memory.
+template <int NW, bool COUNT, bool ANY_WIN>
+__device__ __forceinline__ void klt_warps(const KltArgs& A, int warp, int lane, uint8_t* sPw, int* sDw, int32_t* counts, int win) {
+    int i = blockIdx.x * NW + warp;
     if (A.work_counter) {
         int first = 0;
         if (lane == 0) first = atomicAdd(A.work_counter, 1);
@@ -315,10 +459,31 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt
     while (i < A.n) {
         int nxt_i = 0;
         if (A.work_counter && lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
-        klt_one<COUNT>(A, i, sPall[warp], sDall[warp], lane, counts);
+        klt_one<COUNT, ANY_WIN>(A, i, sPw, sDw, lane, counts, win);
         if (!A.work_counter) return;
         i = __shfl_sync(FULL, nxt_i, 0);
     }
+}
+
+template <bool COUNT>
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A, int32_t* counts) {
+    __shared__ __align__(16) uint8_t sPall[WARPS_PER_CTA][kltsetup::SP_BYTES];
+    __shared__ __align__(16) int sDall[WARPS_PER_CTA][kltsetup::SD_INTS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    klt_warps<WARPS_PER_CTA, COUNT, false>(A, warp, lane, sPall[warp], sDall[warp], counts, 9);
+}
+
+// Any window from 3 to 31 but 9.  Per warp: the staged bytes (WN_BYTES), then the derivative plane, the template
+// derivatives (ints) and the template intensities (shorts) in one int array; 11 272 bytes, 45 088 per CTA.
+constexpr int WIN_WARPS_PER_CTA = 4;
+constexpr int WIN_WARP_INTS = kltsetup::WD_INTS + kltsetup::WT_ELEMS + kltsetup::WT_ELEMS / 2;
+
+template <bool COUNT>
+__global__ void __launch_bounds__(WIN_WARPS_PER_CTA * 32) fb_klt_win_kernel(KltArgs A, int32_t* counts, int win) {
+    __shared__ __align__(16) uint8_t sNall[WIN_WARPS_PER_CTA][kltsetup::WN_BYTES];
+    __shared__ __align__(16) int sWall[WIN_WARPS_PER_CTA][WIN_WARP_INTS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    klt_warps<WIN_WARPS_PER_CTA, COUNT, true>(A, warp, lane, sNall[warp], sWall[warp], counts, win);
 }
 
 // Depth cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), maxlevel) reaches: it stops before a level whose width or
@@ -338,7 +503,8 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
     if (n == 0) return OV2_OK;  // feature_tracker.cpp:43-46
     if (!kps || !priors_inout || !status_out || (!frame_idx && per_frame <= 0))
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: null array");
-    if (prm->win != 9) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: only nwinsize = 9 is built (all reference configs)");
+    if (prm->win < 3 || prm->win > kltsetup::WMAX)
+        return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: nwinsize must be 3 .. 31");
     if (prev->nlev != cur->nlev || prev->w[0] != cur->w[0] || prev->h[0] != cur->h[0] || !prev->l0 || !cur->l0)
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: pyramids not built / mismatched");
     if (!frame_idx && (first_frame < 0 || first_frame + (n + per_frame - 1) / per_frame > prev->batch))
@@ -377,9 +543,15 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
         if ((st = ov2_stage_out(ctx, counts_out, sizeof(int32_t) * 2 * (size_t)n, &o)) != OV2_OK) return st;
         d_counts = (int32_t*)o;
     }
-    int grid = div_up(n, WARPS_PER_CTA), per_sm = 0;
+    // 9 x 9 (every shipped configuration) keeps its own kernel; every other size runs fb_klt_win_kernel
+    const int win = prm->win;
+    const int nw = win == 9 ? WARPS_PER_CTA : WIN_WARPS_PER_CTA;
+    int grid = div_up(n, nw), per_sm = 0;
     A.work_counter = nullptr;
-    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false>, WARPS_PER_CTA * 32, 0));
+    if (win == 9)
+        OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false>, WARPS_PER_CTA * 32, 0));
+    else
+        OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_win_kernel<false>, WIN_WARPS_PER_CTA * 32, 0));
     const int resident = per_sm * ctx->sm_count;
     if (grid > resident) {
         if ((st = ov2_scratch(ctx, sizeof(int), &o)) != OV2_OK) return st;
@@ -387,7 +559,14 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
         OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
         grid = resident;
     }
-    if (d_counts)
+    if (win != 9) {
+        if (d_counts)
+            OV2_LAUNCH(ctx, "fb_klt_win_kernel",
+                       (fb_klt_win_kernel<true><<<grid, WIN_WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, d_counts, win)));
+        else
+            OV2_LAUNCH(ctx, "fb_klt_win_kernel",
+                       (fb_klt_win_kernel<false><<<grid, WIN_WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, nullptr, win)));
+    } else if (d_counts)
         OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<true><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, d_counts)));
     else
         OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, nullptr)));

@@ -1,7 +1,9 @@
 // K (level set-up): template patch staging, Scharr derivatives and the int16 template / derivative
 // window of one Lucas-Kanade level, for the 9 x 9 window (all reference configurations,
 // /root/reference/src/feature_tracker.cpp:35-137 via cv::calcOpticalFlowPyrLK), and the reflect-101 /
-// dp2a / funnel-shift helpers that the tracker's iterations (frontend_klt.cu) use as well.
+// dp2a / funnel-shift helpers that the tracker's iterations (frontend_klt.cu) use as well.  The win_* functions at the
+// end are the same phases for every other window size from 3 to 31 (fb_klt_win_kernel), checked lane by lane in
+// tests/test_klt_win_lane_code.py.
 //
 // Written as plain per-lane functions (no warp intrinsics; the phases are separated by __syncwarp in
 // the kernel) so that tests/test_host_logic.py can compile the SAME code for the host and check it
@@ -218,6 +220,101 @@ KLT_HD void template_direct(int lane, const uint8_t* sP, int off, int iw00, int 
         sA11 += ixval * ixval;
         sA12 += ixval * iyval;
         sA22 += iyval * iyval;
+    }
+}
+
+// ---- Any window from 3 to 31 (fb_klt_win_kernel): lane c owns window column c, every row of it.
+//
+// Shared-memory layout per warp (win <= WMAX):
+//   sN  : (n rows) x WN_PITCH bytes, byte (r, c) = image (reflect101(y0 + r), reflect101(x0 + c)); the template level
+//         set-up stages the (win + 3)^2 neighbourhood from (ix - 1, iy - 1), the iterations the (win + 1)^2 search bytes
+//         from (jx, jy) into the same buffer.
+//   sD  : (win + 1) rows x WG_PITCH ints, Scharr (dx & 0xFFFF) | (dy << 16) at image (iy + r, ix + c); 0 outside the image.
+//   sI  : win rows x WG_PITCH shorts, the template intensities (5 fractional bits).
+//   sG  : win rows x WG_PITCH ints, the template derivatives (Ix & 0xFFFF) | (Iy << 16).
+// Per lane, |Ix|, |Iy| <= 4080 and |J - I| <= 8160, so 31 rows keep every per-lane sum below 2^31.
+constexpr int WMAX = 31;
+constexpr int WN_PITCH = 36;                       // bytes: the neighbourhood is at most 34 wide
+constexpr int WN_BYTES = (WMAX + 3) * WN_PITCH;    // 1224
+constexpr int WG_PITCH = 32;                       // elements of a derivative / template row
+constexpr int WD_INTS = (WMAX + 1) * WG_PITCH;     // 1024
+constexpr int WT_ELEMS = WMAX * WG_PITCH;          // 992
+
+// n x n bytes from origin (x0, y0), reflect-101 outside the image; lanes stride the columns (n <= 34).
+KLT_HD void win_stage(int lane, const uint8_t* img, int pitch, int lw, int lh, int x0, int y0, int n, uint8_t* sN) {
+    const bool inside = x0 >= 0 && y0 >= 0 && x0 + n <= lw && y0 + n <= lh;
+    for (int r = 0; r < n; ++r) {
+        const uint8_t* row = img + (size_t)(inside ? y0 + r : reflect101_any(y0 + r, lh)) * pitch;
+        for (int c = lane; c < n; c += 32) sN[r * WN_PITCH + c] = KLT_LDG8(row + (inside ? x0 + c : reflect101_any(x0 + c, lw)));
+    }
+}
+
+// Scharr of the staged (win + 3)^2 neighbourhood: lane c <= win fills derivative column c, rows 0 .. win, rolling the
+// three neighbourhood rows it reads down the column.
+KLT_HD void win_scharr(int lane, const uint8_t* sN, int ix, int iy, int lw, int lh, int win, int* sD) {
+    if (lane > win) return;
+    const int c = lane;
+    const bool xin = ix + c >= 0 && ix + c < lw;
+    const uint8_t* p = sN + c;
+    int a0 = p[0], a1 = p[1], a2 = p[2];
+    int b0 = p[WN_PITCH], b1 = p[WN_PITCH + 1], b2 = p[WN_PITCH + 2];
+    for (int r = 0; r <= win; ++r) {
+        const uint8_t* q = p + (r + 2) * WN_PITCH;
+        const int c0 = q[0], c1 = q[1], c2 = q[2];
+        const int y = iy + r;
+        int dx = 0, dy = 0;
+        if (xin && y >= 0 && y < lh) {
+            dx = ((a2 + c2) * 3 + b2 * 10) - ((a0 + c0) * 3 + b0 * 10);
+            dy = ((c0 - a0) + (c2 - a2)) * 3 + (c1 - a1) * 10;
+        }
+        sD[r * WG_PITCH + c] = (int)(((unsigned)dx & 0xFFFFu) | ((unsigned)dy << 16));
+        a0 = b0; a1 = b1; a2 = b2;
+        b0 = c0; b1 = c1; b2 = c2;
+    }
+}
+
+// The template window: lane c < win fills column c of sI / sG and returns its share of the normal-equation sums
+// (zeros for lanes >= win).  OpenCV's fixed point as in template_rows().
+KLT_HD void win_template(int lane, const uint8_t* sN, const int* sD, int win, int iw00, int iw01, int iw10, int iw11,
+                         short* sI, int* sG, int& sA11, int& sA12, int& sA22) {
+    sA11 = 0; sA12 = 0; sA22 = 0;
+    if (lane >= win) return;
+    const int c = lane;
+    const uint8_t* p = sN + WN_PITCH + c + 1;      // neighbourhood row r + 1, column c + 1 = image (iy + r, ix + c)
+    int t0 = p[0], t1 = p[1];
+    int dt0 = sD[c], dt1 = sD[c + 1];
+    for (int r = 0; r < win; ++r) {
+        const int b0 = p[(r + 1) * WN_PITCH], b1 = p[(r + 1) * WN_PITCH + 1];
+        const int db0 = sD[(r + 1) * WG_PITCH + c], db1 = sD[(r + 1) * WG_PITCH + c + 1];
+        const int ival = (t0 * iw00 + t1 * iw01 + b0 * iw10 + b1 * iw11 + (1 << 8)) >> 9;
+        const int ixval = ((int)(short)(dt0 & 0xFFFF) * iw00 + (int)(short)(dt1 & 0xFFFF) * iw01 +
+                           (int)(short)(db0 & 0xFFFF) * iw10 + (int)(short)(db1 & 0xFFFF) * iw11 + (1 << 13)) >> 14;
+        const int iyval = ((dt0 >> 16) * iw00 + (dt1 >> 16) * iw01 + (db0 >> 16) * iw10 + (db1 >> 16) * iw11 + (1 << 13)) >> 14;
+        sI[r * WG_PITCH + c] = (short)ival;
+        sG[r * WG_PITCH + c] = (int)(((unsigned)ixval & 0xFFFFu) | ((unsigned)iyval << 16));
+        sA11 += ixval * ixval;
+        sA12 += ixval * iyval;
+        sA22 += iyval * iyval;
+        t0 = b0; t1 = b1; dt0 = db0; dt1 = db1;
+    }
+}
+
+// One iteration's mismatch sums of lane c < win (zeros otherwise): J at the staged (win + 1)^2 search bytes,
+// (bilinear + 2^8) >> 9, minus the template, times its derivatives, summed down column c.
+KLT_HD void win_mismatch(int lane, const uint8_t* sN, const short* sI, const int* sG, int win, int iw00, int iw01, int iw10,
+                         int iw11, int& sb1, int& sb2) {
+    sb1 = 0; sb2 = 0;
+    if (lane >= win) return;
+    const int c = lane;
+    const uint8_t* p = sN + c;
+    int t0 = p[0], t1 = p[1];
+    for (int r = 0; r < win; ++r) {
+        const int b0 = p[(r + 1) * WN_PITCH], b1 = p[(r + 1) * WN_PITCH + 1];
+        const int d = ((t0 * iw00 + t1 * iw01 + b0 * iw10 + b1 * iw11 + (1 << 8)) >> 9) - sI[r * WG_PITCH + c];
+        const int g = sG[r * WG_PITCH + c];
+        sb1 += d * (int)(short)(g & 0xFFFF);
+        sb2 += d * (g >> 16);
+        t0 = b0; t1 = b1;
     }
 }
 
