@@ -40,7 +40,9 @@ struct KltArgs {
     float2* priors;
     uint8_t* status;
     int max_iter;
-    float ferr, fb_dist;
+    float eig_q;           // q < eig_q  <=>  minEig < LK_MIN_EIG, q the numerator of minEig (lk_eig_num)
+    float ferr_q;          // q > ferr_q  <=>  minEig > ferr
+    double fb_s;           // dx^2 + dy^2 > fb_s  <=>  sqrt(dx^2 + dy^2) > fb_dist (klt_setup.cuh, klt_fb_s)
     double eps2;           // epsilon^2 as OpenCV forms it (double)
     float eps_lo, eps_hi;  // float brackets of eps2: outside them the float evaluation of |delta|^2 decides
     int* work_counter;   // persistent launch: warps pull keypoint indices from this counter (null: one warp per index)
@@ -65,11 +67,13 @@ __device__ __forceinline__ long long warp_sum64(int s) {
     iw10 = __float2int_rn((1.f - (a)) * (b) * 16384.f);          \
     iw11 = 16384 - iw00 - iw01 - iw10
 
-// The minimal eigenvalue of the normal matrix over a win x win window (the error LK_GET_MIN_EIGENVALS reports).  A level
-// whose minEig < LK_MIN_EIG or determinant < LK_MIN_DET (FLT_EPSILON) is dropped.
+// The minimal eigenvalue of the normal matrix over a win x win window (the error LK_GET_MIN_EIGENVALS reports) is
+// minEig = RN(q / (2 win^2)) with q this numerator.  A level whose minEig < LK_MIN_EIG or determinant < LK_MIN_DET
+// (FLT_EPSILON) is dropped.  minEig is only ever compared, and RN(q / d) is monotone in q, so the trackers keep q and compare
+// it against thresholds klt_launch computes for the call's win (KltArgs::eig_q, ferr_q): same decisions, no division.
 // (double)minEig < 1e-4 <=> minEig < 0x1.a36e3p-14f, the smallest float >= 1e-4 (1e-4 is not a float)
-__device__ __forceinline__ float lk_min_eig(float A11, float A12, float A22, int win) {
-    return (A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / (float)(2 * win * win);
+__device__ __forceinline__ float lk_eig_num(float A11, float A12, float A22) {
+    return A22 + A11 - __fsqrt_rn((A11 - A22) * (A11 - A22) + 4.f * A12 * A12);
 }
 constexpr float LK_MIN_EIG = 0x1.a36e3p-14f;
 constexpr float LK_MIN_DET = 1.1920928955078125e-07f;
@@ -139,8 +143,8 @@ __device__ __forceinline__ void gather_taps(const uint8_t* Jlane, int Jpitch, in
 // max_iter) for the other window sizes: a change to it here belongs there too.
 template <bool COUNT>
 __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
-                         int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sP, int* sD, int lane,
-                         int& work) {
+                         int max_iter, double eps2, float eps_lo, float eps_hi, float eig_q, float& err_out, uint8_t* sP, int* sD,
+                         int lane, int& work) {
     using kltsetup::WIN;
     // lane l < 27 owns the three horizontally adjacent window pixels 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..),
     // so the search-image taps of a lane are 4 consecutive bytes on two rows; the integer window sums are order independent.
@@ -149,7 +153,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
     const float FLT_SCALE = 1.f / (1 << 20);
     const int lane_row = lane / 3, lane_col = 3 * (lane - 3 * (lane / 3));
     bool status = true;
-    float err = 0.f;
+    float err = 0.f;   // the numerator q of minEig (lk_eig_num)
 
     for (int level = maxlevel; level >= 0; --level) {
         const int lw = Ipyr.w[level], lh = Ipyr.h[level];
@@ -158,7 +162,7 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
         const bool packed_ok = ((reinterpret_cast<uintptr_t>(Jimg) | (uintptr_t)Jpitch) & 3) == 0;   // aliased level 0 may be unaligned
         const uint8_t* Jlane = Jimg + lane_row * Jpitch;
-        const float sc = 1.f / (float)(1 << level);
+        const float sc = __int_as_float((127 - level) << 23);   // 2^-level, exactly 1.f / (1 << level)
         float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
         float2 nextPt;
         if (level == maxlevel) nextPt = make_float2(nxt.x * sc, nxt.y * sc);
@@ -177,29 +181,33 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
 
         // ---- level set-up (klt_setup.cuh): 12 x 12 neighbourhood -> shared memory (aligned words on the
-        //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window + exact
-        //      integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2; lanes 27..31 get zeros.
+        //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window (as sign-extended ints) +
+        //      exact integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2; lanes 27..31 get zeros.
         __syncwarp();
         const bool tmpl_aligned = ((reinterpret_cast<uintptr_t>(Iimg) | (uintptr_t)Ipitch) & 3) == 0;
-        const int off = kltsetup::stage_patch(lane, Iimg, Ipitch, lw, lh, ix, iy, tmpl_aligned, sP);
-        __syncwarp();
-        short Iv[PER_LANE], Ixv[PER_LANE], Iyv[PER_LANE];
+        int Iv[PER_LANE], Ixv[PER_LANE], Iyv[PER_LANE];
         int sA11, sA12, sA22;
         if (tmpl_aligned && kltsetup::patch_interior(ix, iy, lw, lh)) {
             // interior (warp-uniform): interpolate first, differentiate after - same integers, one pass, no derivative patch
-            kltsetup::template_direct(lane, sP, off, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22);
-        } else {
-            kltsetup::scharr_rows(lane, sP, off, ix, iy, lw, lh, sD);
+            kltsetup::stage_interior(lane, Iimg, Ipitch, lw, ix, iy, sP);
             __syncwarp();
-            kltsetup::template_rows(lane, sP, off, sD, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22);
+            kltsetup::template_direct(lane, sP, (ix - 1) & 3, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22);
+        } else {
+            kltsetup::stage_border(lane, Iimg, Ipitch, lw, lh, ix, iy, sP);
+            __syncwarp();
+            kltsetup::scharr_rows(lane, sP, 0, ix, iy, lw, lh, sD);
+            __syncwarp();
+            kltsetup::template_rows(lane, sP, 0, sD, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22);
         }
+        // the template values as the iterations use them
+        const int I0 = Iv[0], I1 = Iv[1], I2 = Iv[2];
+        const int X0 = Ixv[0], X1 = Ixv[1], X2 = Ixv[2];
+        const int Y0 = Iyv[0], Y1 = Iyv[1], Y2 = Iyv[2];
         // |b sums| <= max|J - I| * sum|Ix| with |J - I| <= 8160 (both are 8-bit intensities with 5 fractional bits): when
         // 8160 * (sum|Ix| + sum|Iy|) < 2^31 the iterations' mismatch sums fit one exact 32-bit redux each (true for
         // every window whose mean |gradient| is below ~3200 of the possible 8160, i.e. anything but a synthetic
         // checkerboard; 8162 * 262000 < 2^31); otherwise the split 64-bit reduction is kept.  Same integers either way.
-        int sabs = 0;
-#pragma unroll
-        for (int k = 0; k < PER_LANE; ++k) sabs += abs((int)Ixv[k]) + abs((int)Iyv[k]);
+        const int sabs = abs(X0) + abs(X1) + abs(X2) + abs(Y0) + abs(Y1) + abs(Y2);
         const bool b32 = __reduce_add_sync(FULL, sabs) < 262000;
         // |window sums| <= 81 * 4080^2 = 1.35e9 < 2^31 for the 9 x 9 window: one exact 32-bit redux each
         // (the b sums of the iterations can reach 2.7e9 and keep the split 64-bit reduction)
@@ -207,17 +215,12 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
         const float A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * FLT_SCALE;
         const float A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * FLT_SCALE;
         float D = A11 * A22 - A12 * A12;
-        const float minEig = lk_min_eig(A11, A12, A22, WIN);
-        err = minEig;
-        if (minEig < LK_MIN_EIG || D < LK_MIN_DET) {
+        err = lk_eig_num(A11, A12, A22);
+        if (err < eig_q || D < LK_MIN_DET) {
             if (level == 0) status = false;
             continue;
         }
         D = 1.f / D;
-        // the template values as the iterations use them: sign-extended once per level, not once per iteration
-        int I0 = Iv[0], I1 = Iv[1], I2 = Iv[2];
-        int X0 = Ixv[0], X1 = Ixv[1], X2 = Ixv[2];
-        int Y0 = Iyv[0], Y1 = Iyv[1], Y2 = Iyv[2];
         nextPt.x -= half;
         nextPt.y -= half;
         float2 prevDelta = make_float2(0.f, 0.f);
@@ -290,21 +293,21 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
 // fb_klt_kernel's code stays as it is): a change to it here belongs there too.
 template <bool COUNT>
 __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
-                             int win, int max_iter, double eps2, float eps_lo, float eps_hi, float& err_out, uint8_t* sN,
-                             int* sD, int lane, int& work) {
+                             int win, int max_iter, double eps2, float eps_lo, float eps_hi, float eig_q, float& err_out,
+                             uint8_t* sN, int* sD, int lane, int& work) {
     int* sG = sD + kltsetup::WD_INTS;
     short* sI = reinterpret_cast<short*>(sG + kltsetup::WT_ELEMS);
     const float half = (win - 1) * 0.5f;
     const float FLT_SCALE = 1.f / (1 << 20);
     bool status = true;
-    float err = 0.f;
+    float err = 0.f;   // the numerator q of minEig (lk_eig_num)
 
     for (int level = maxlevel; level >= 0; --level) {
         const int lw = Ipyr.w[level], lh = Ipyr.h[level];
         const uint8_t* Iimg = Ipyr.lvl[level] + Ipyr.fstride[level] * frame;
         const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
         const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
-        const float sc = 1.f / (float)(1 << level);
+        const float sc = __int_as_float((127 - level) << 23);   // 2^-level, exactly 1.f / (1 << level)
         float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
         float2 nextPt;
         if (level == maxlevel) nextPt = make_float2(nxt.x * sc, nxt.y * sc);
@@ -332,9 +335,8 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
         const float A12 = __ll2float_rn(warp_sum64(sA12)) * FLT_SCALE;
         const float A22 = __ll2float_rn(warp_sum64(sA22)) * FLT_SCALE;
         float D = A11 * A22 - A12 * A12;
-        const float minEig = lk_min_eig(A11, A12, A22, win);
-        err = minEig;
-        if (minEig < LK_MIN_EIG || D < LK_MIN_DET) {
+        err = lk_eig_num(A11, A12, A22);
+        if (err < eig_q || D < LK_MIN_DET) {
             if (level == 0) status = false;
             continue;
         }
@@ -405,12 +407,12 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     bool ok;
     if constexpr (ANY_WIN)
         ok = kp.x >= 0.f && lk_track_win<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, win, A.max_iter, A.eps2, A.eps_lo,
-                                                A.eps_hi, err, sPw, sDw, lane, work);
+                                                A.eps_hi, A.eig_q, err, sPw, sDw, lane, work);
     else
         ok = kp.x >= 0.f && lk_track<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
-                                            err, sPw, sDw, lane, work);
-    // feature_tracker.cpp:79-101
-    if (ok && err > A.ferr) ok = false;
+                                            A.eig_q, err, sPw, sDw, lane, work);
+    // feature_tracker.cpp:79-101 (err > ferr and the distance test through the thresholds of KltArgs)
+    if (ok && err > A.ferr_q) ok = false;
     if (ok) {
         const float w0 = (float)A.cur.w[0], h0 = (float)A.cur.h[0];
         if (!(1.f <= fwd.x && fwd.x < w0 - 1.f && 1.f <= fwd.y && fwd.y < h0 - 1.f)) ok = false;
@@ -421,16 +423,15 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
         float err2 = 0.f;
         bool ok2;
         if constexpr (ANY_WIN)
-            ok2 = lk_track_win<COUNT>(A.cur, A.prev, frame, fwd, back, 0, win, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw,
-                                      sDw, lane, work);
+            ok2 = lk_track_win<COUNT>(A.cur, A.prev, frame, fwd, back, 0, win, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, A.eig_q,
+                                      err2, sPw, sDw, lane, work);
         else
-            ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, err2, sPw, sDw,
-                                  lane, work);
+            ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, A.eig_q, err2, sPw,
+                                  sDw, lane, work);
         if (!ok2) ok = false;
         else {
             float dx = kp.x - back.x, dy = kp.y - back.y;
-            double nrm = sqrt((double)dx * (double)dx + (double)dy * (double)dy);
-            if (nrm > (double)A.fb_dist) ok = false;
+            if ((double)dx * (double)dx + (double)dy * (double)dy > A.fb_s) ok = false;
         }
     }
     if (lane == 0) {
@@ -524,8 +525,9 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
     A.eps2 = (double)prm->eps * (double)prm->eps;
     A.eps_lo = (float)(A.eps2 * (1.0 - 1e-6));
     A.eps_hi = (float)(A.eps2 * (1.0 + 1e-6));
-    A.ferr = prm->ferr;
-    A.fb_dist = prm->fb_dist;
+    A.eig_q = kltsetup::klt_eig_q(prm->win, LK_MIN_EIG);
+    A.ferr_q = kltsetup::klt_ferr_q(prm->win, prm->ferr);
+    A.fb_s = kltsetup::klt_fb_s(prm->fb_dist);
     const void* d = nullptr;
     void* o = nullptr;
     if ((st = ov2_stage_in(ctx, frame_idx, sizeof(int32_t) * (size_t)n, &d)) != OV2_OK) return st;

@@ -7,7 +7,8 @@
 //
 // Written as plain per-lane functions (no warp intrinsics; the phases are separated by __syncwarp in
 // the kernel) so that tests/test_host_logic.py can compile the SAME code for the host and check it
-// against the definition, lane by lane (test_klt_level_setup_lane_code_matches_definition).
+// against the definition, lane by lane (test_klt_level_setup_lane_code_matches_definition, and
+// tests/test_klt_setup_host.py for the split staging and the int-output template functions the kernel calls).
 //
 // Shared-memory layout per warp:
 //   sP  : 12 rows x 16 bytes.  Row r holds image row iy-1+r; byte (r, c) of the 12 x 12 neighbourhood
@@ -16,8 +17,10 @@
 //   sD  : 10 rows x 12 ints, (dx & 0xFFFF) | (dy << 16) of the Scharr derivative at image position
 //         (iy + r, ix + c); 0 outside the image (cv::buildOpticalFlowPyramid's BORDER_CONSTANT planes).
 #pragma once
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
 
 #if defined(__CUDACC__)
 #define KLT_HD __host__ __device__ __forceinline__
@@ -55,24 +58,40 @@ KLT_HD int reflect101_any(int i, int n) {
 // true when the whole 12 x 12 neighbourhood (and therefore every Scharr tap) lies inside the image
 KLT_HD bool patch_interior(int ix, int iy, int lw, int lh) { return ix >= 1 && iy >= 1 && ix + PW - 1 <= lw && iy + PW - 1 <= lh; }
 
-// Phase 1 (all lanes).  Returns off.  `aligned`: image base and pitch are multiples of 4.
-KLT_HD int stage_patch(int lane, const uint8_t* img, int pitch, int lw, int lh, int ix, int iy, bool aligned, uint8_t* sP) {
-    if (aligned && patch_interior(ix, iy, lw, lh)) {
-        const int x0 = (ix - 1) & ~3;                 // first staged column (>= 0), word aligned
-        uint32_t* sPw = reinterpret_cast<uint32_t*>(sP);
-        for (int i = lane; i < PW * 4; i += 32) {
-            const int r = i >> 2, q = i & 3;
-            const int xw = x0 + 4 * q;
-            // a word starting at or beyond lw holds no byte the patch needs (and may lie outside the buffer)
-            sPw[i] = xw < lw ? KLT_LDG32(reinterpret_cast<const uint32_t*>(img + (size_t)(iy - 1 + r) * pitch + xw)) : 0u;
-        }
-        return (ix - 1) & 3;
+// Phase 1, interior path (aligned image, patch_interior()): the 12 rows as 4 aligned words each, off = (ix - 1) & 3.  Word i
+// of sP is staged by lane i & 31: lane l holds row l >> 2 and, for l < 16, row 8 + (l >> 2), both at word l & 3 of the row.
+// Offsets within one level image fit 32 bits (as in the search gathers), so the lane forms one 32-bit offset from the level's
+// base and reaches its second row 8 pitches further.
+KLT_HD void stage_interior(int lane, const uint8_t* img, int pitch, int lw, int ix, int iy, uint8_t* sP) {
+    const int xw = ((ix - 1) & ~3) + 4 * (lane & 3);   // the lane's word column (>= 0), word aligned
+    uint32_t* sPw = reinterpret_cast<uint32_t*>(sP);
+    // a word starting at or beyond lw holds no byte the patch needs (and may lie outside the buffer)
+    unsigned w0 = 0u, w1 = 0u;
+    if (xw < lw) {
+        const uint8_t* p = img + ((iy - 1 + (lane >> 2)) * pitch + xw);
+        w0 = KLT_LDG32(reinterpret_cast<const uint32_t*>(p));
+        if (lane < 16) w1 = KLT_LDG32(reinterpret_cast<const uint32_t*>(p + 8 * pitch));
     }
+    sPw[lane] = w0;
+    if (lane < 16) sPw[lane + 32] = w1;
+}
+
+// Phase 1, border path: the 12 x 12 neighbourhood byte by byte through reflect-101, off = 0.
+KLT_HD void stage_border(int lane, const uint8_t* img, int pitch, int lw, int lh, int ix, int iy, uint8_t* sP) {
     for (int i = lane; i < PW * PW; i += 32) {
         const int r = i / PW, c = i - r * PW;
         const int y = reflect101_any(iy - 1 + r, lh), x = reflect101_any(ix - 1 + c, lw);
         sP[r * SP_PITCH + c] = KLT_LDG8(img + (size_t)y * pitch + x);
     }
+}
+
+// Phase 1 (all lanes), either path.  Returns off.  `aligned`: image base and pitch are multiples of 4.
+KLT_HD int stage_patch(int lane, const uint8_t* img, int pitch, int lw, int lh, int ix, int iy, bool aligned, uint8_t* sP) {
+    if (aligned && patch_interior(ix, iy, lw, lh)) {
+        stage_interior(lane, img, pitch, lw, ix, iy, sP);
+        return (ix - 1) & 3;
+    }
+    stage_border(lane, img, pitch, lw, lh, ix, iy, sP);
     return 0;
 }
 
@@ -112,8 +131,10 @@ KLT_HD void scharr_rows(int lane, const uint8_t* sP, int off, int ix, int iy, in
 
 // Phase 3 (lanes 0..26; others get zeros): window pixels 3l .. 3l+2 = row l / 3, columns 3 (l % 3) .. +2.
 // OpenCV's fixed point: I = (bilinear(u8) * 2^14 + 2^8) >> 9, Ix / Iy = (bilinear(s16) + 2^13) >> 14.
+// OpenCV stores the results as int16; they fit it (0 <= I <= 8160, |Ix|, |Iy| <= 4081 even with iw11 = -1), so the int
+// outputs are the int16 values already sign-extended, as the iterations use them.
 KLT_HD void template_rows(int lane, const uint8_t* sP, int off, const int* sD, int iw00, int iw01, int iw10, int iw11,
-                          short* Iv, short* Ixv, short* Iyv, int& sA11, int& sA12, int& sA22) {
+                          int* Iv, int* Ixv, int* Iyv, int& sA11, int& sA12, int& sA22) {
     sA11 = 0; sA12 = 0; sA22 = 0;
     Iv[0] = Iv[1] = Iv[2] = 0; Ixv[0] = Ixv[1] = Ixv[2] = 0; Iyv[0] = Iyv[1] = Iyv[2] = 0;
     if (lane >= 27) return;
@@ -133,11 +154,17 @@ KLT_HD void template_rows(int lane, const uint8_t* sP, int off, const int* sD, i
         const int ival = (t[k] * iw00 + t[k + 1] * iw01 + b[k] * iw10 + b[k + 1] * iw11 + (1 << 8)) >> 9;
         const int ixval = (dxt[k] * iw00 + dxt[k + 1] * iw01 + dxb[k] * iw10 + dxb[k + 1] * iw11 + (1 << 13)) >> 14;
         const int iyval = (dyt[k] * iw00 + dyt[k + 1] * iw01 + dyb[k] * iw10 + dyb[k + 1] * iw11 + (1 << 13)) >> 14;
-        Iv[k] = (short)ival; Ixv[k] = (short)ixval; Iyv[k] = (short)iyval;
+        Iv[k] = ival; Ixv[k] = ixval; Iyv[k] = iyval;
         sA11 += ixval * ixval;
         sA12 += ixval * iyval;
         sA22 += iyval * iyval;
     }
+}
+KLT_HD void template_rows(int lane, const uint8_t* sP, int off, const int* sD, int iw00, int iw01, int iw10, int iw11,
+                          short* Iv, short* Ixv, short* Iyv, int& sA11, int& sA12, int& sA22) {
+    int v[3], x[3], y[3];
+    template_rows(lane, sP, off, sD, iw00, iw01, iw10, iw11, v, x, y, sA11, sA12, sA22);
+    for (int k = 0; k < 3; ++k) { Iv[k] = (short)v[k]; Ixv[k] = (short)x[k]; Iyv[k] = (short)y[k]; }
 }
 
 // dp2a: signed 16-bit halves of a (bilinear weights: iw11 = 16384 - others can round to -1) times UNSIGNED bytes of b
@@ -174,9 +201,9 @@ KLT_HD unsigned funnel_r(unsigned lo, unsigned hi, unsigned sh) {   // bytes of 
 // with W <= 255 * 16385 (22 bits) and the Scharr sums of W below 2^27: same integers as template_rows() produces from the
 // int16 derivative planes, then the same roundings (I: (W + 2^8) >> 9, Ix / Iy: (. + 2^13) >> 14).  A lane forms the 3 x 5 W
 // values around its three pixels straight from the staged bytes with dp2a; nothing is written to sD and no second
-// __syncwarp is needed.  Lane l < 27 owns window pixels (l / 3, 3 (l % 3) ..+2) as in template_rows().
+// __syncwarp is needed.  Lane l < 27 owns window pixels (l / 3, 3 (l % 3) ..+2) as in template_rows(), int outputs as there.
 KLT_HD void template_direct(int lane, const uint8_t* sP, int off, int iw00, int iw01, int iw10, int iw11,
-                            short* Iv, short* Ixv, short* Iyv, int& sA11, int& sA12, int& sA22) {
+                            int* Iv, int* Ixv, int* Iyv, int& sA11, int& sA12, int& sA22) {
     sA11 = 0; sA12 = 0; sA22 = 0;
     Iv[0] = Iv[1] = Iv[2] = 0; Ixv[0] = Ixv[1] = Ixv[2] = 0; Iyv[0] = Iyv[1] = Iyv[2] = 0;
     if (lane >= 27) return;
@@ -216,11 +243,17 @@ KLT_HD void template_direct(int lane, const uint8_t* sP, int off, int iw00, int 
         const int ival = (W[1][k + 1] + (1 << 8)) >> 9;
         const int ixval = (vs[k + 2] - vs[k] + (1 << 13)) >> 14;
         const int iyval = ((vd[k] + vd[k + 2]) * 3 + vd[k + 1] * 10 + (1 << 13)) >> 14;
-        Iv[k] = (short)ival; Ixv[k] = (short)ixval; Iyv[k] = (short)iyval;
+        Iv[k] = ival; Ixv[k] = ixval; Iyv[k] = iyval;
         sA11 += ixval * ixval;
         sA12 += ixval * iyval;
         sA22 += iyval * iyval;
     }
+}
+KLT_HD void template_direct(int lane, const uint8_t* sP, int off, int iw00, int iw01, int iw10, int iw11,
+                            short* Iv, short* Ixv, short* Iyv, int& sA11, int& sA12, int& sA22) {
+    int v[3], x[3], y[3];
+    template_direct(lane, sP, off, iw00, iw01, iw10, iw11, v, x, y, sA11, sA12, sA22);
+    for (int k = 0; k < 3; ++k) { Iv[k] = (short)v[k]; Ixv[k] = (short)x[k]; Iyv[k] = (short)y[k]; }
 }
 
 // ---- Any window from 3 to 31 (fb_klt_win_kernel): lane c owns window column c, every row of it.
@@ -316,6 +349,59 @@ KLT_HD void win_mismatch(int lane, const uint8_t* sN, const short* sI, const int
         sb2 += d * (g >> 16);
         t0 = b0; t1 = b1;
     }
+}
+
+// ---- Host-side thresholds that let the trackers skip a division or a square root whose result is only ever compared.
+//
+// The minimal eigenvalue is minEig = RN(q / (2 win^2)) with q = A22 + A11 - sqrt(...), and RN(q / d) for d > 0 is
+// monotone in q, so each test of minEig against a constant is a test of q against one float; likewise the forward-backward
+// test sqrt(s) > fb_dist on s = dx^2 + dy^2 (double).  The thresholds are found by bisection over bit patterns with the
+// host's IEEE division and square root, the same correctly rounded operations the device performs.
+
+// the non-NaN floats in increasing order: k in [-0x7f800000, 0x7f800000] <-> -inf .. -0 (skipped), +0 .. +inf
+inline float klt_key_float(long long k) {
+    const uint32_t u = k >= 0 ? (uint32_t)k : 0x80000000u | (uint32_t)(-k);
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+}
+
+// the smallest float key in [lo, hi] where the monotone (false .. true) predicate holds; hi + 1 if it holds nowhere
+template <class P> inline long long klt_first_true(long long lo, long long hi, P pred) {
+    ++hi;
+    while (lo < hi) {
+        const long long m = lo + (hi - lo) / 2;
+        if (pred(m)) hi = m; else lo = m + 1;
+    }
+    return lo;
+}
+
+// q < eig_q  <=>  RN(q / (2 win^2)) < min_eig, for every float q (NaN: both false)
+inline float klt_eig_q(int win, float min_eig) {
+    const float d = (float)(2 * win * win);
+    const long long K = 0x7f800000LL;
+    const long long k = klt_first_true(-K, K, [&](long long k) { return !(klt_key_float(k) / d < min_eig); });
+    return klt_key_float(k);                       // the predicate holds at +inf, so k <= K
+}
+
+// q > ferr_q  <=>  RN(q / (2 win^2)) > ferr, for every float q and every ferr (NaN, infinite, negative or zero included)
+inline float klt_ferr_q(int win, float ferr) {
+    const float d = (float)(2 * win * win);
+    const long long K = 0x7f800000LL;
+    const long long k = klt_first_true(-K, K, [&](long long k) { return klt_key_float(k) / d > ferr; });
+    if (k > K) return klt_key_float(K);            // never true (ferr NaN or +inf): q > +inf never holds either
+    return klt_key_float(k - 1);                   // k > -K: RN(-inf / d) = -inf exceeds no ferr
+}
+
+// s > fb_s  <=>  sqrt(s) > fb_dist, for every double s >= 0 or NaN (the squared distance) and every fb_dist
+inline double klt_fb_s(float fb_dist) {
+    const double f = (double)fb_dist;
+    const long long K = 0x7ff0000000000000LL;      // +0 .. +inf
+    auto dbl = [](long long k) { double x; const uint64_t u = (uint64_t)k; memcpy(&x, &u, 8); return x; };
+    const long long k = klt_first_true(0, K, [&](long long k) { return sqrt(dbl(k)) > f; });
+    if (k > K) return dbl(K);                      // never true: fb_dist NaN or +inf
+    if (k == 0) return -dbl(K);                    // true from 0 on (fb_dist < 0): every s >= 0 exceeds -inf
+    return dbl(k - 1);
 }
 
 }  // namespace kltsetup
