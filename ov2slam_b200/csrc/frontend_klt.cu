@@ -16,10 +16,11 @@
 // the image edge, constant 0 outside the image - exactly the planes buildOpticalFlowPyramid
 // would have materialised), so the tracker reads only the 8-bit pyramid.
 //
-// Two kernels: fb_klt_kernel for the 9 x 9 window of every shipped configuration (three window pixels per lane, search
-// taps packed in registers), and fb_klt_win_kernel for every other window from 3 x 3 to 31 x 31 (lane c owns window
-// column c; template and staged image bytes in shared memory).  ov2_fb_klt picks one from nwinsize.  Both share the
-// per-keypoint forward / backward logic and the float32 steps below.
+// One kernel, fb_klt_kernel, instantiated for two window layouts: Win9 for the 9 x 9 window of every shipped configuration
+// (three window pixels per lane, search taps packed in registers) and WinAny for every other window from 3 x 3 to 31 x 31
+// (lane c owns window column c; template and staged image bytes in shared memory), profiled as fb_klt_win_kernel.
+// ov2_fb_klt picks one from nwinsize.  Both run the same per-keypoint forward / backward logic, level and iteration
+// control flow and float32 steps.
 #include <climits>
 #include "ov2_common.cuh"
 #include "klt_setup.cuh"
@@ -27,7 +28,6 @@
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
-constexpr int WARPS_PER_CTA = 8;   // one keypoint per warp
 
 struct KltArgs {
     PyrView prev, cur;
@@ -57,7 +57,7 @@ __device__ __forceinline__ long long warp_sum64(int s) {
     return ((long long)shi << 16) + (long long)slo;
 }
 
-// ---- OpenCV's float32 steps of one LK level, shared by both trackers.  The weights, convergence and oscillation tests
+// ---- OpenCV's float32 steps of one LK level, shared by both window layouts.  The weights, convergence and oscillation tests
 // are macros rather than inline functions: as calls they change how fb_klt_kernel is scheduled.
 
 // 14-bit bilinear weights of the sub-pixel offsets (a, b)
@@ -135,57 +135,54 @@ __device__ __forceinline__ void gather_taps(const uint8_t* Jlane, int Jpitch, in
     }
 }
 
-// One calcOpticalFlowPyrLK track for one point (whole warp cooperates).
-// Ipyr = template pyramid, Jpyr = search pyramid.  nxt: in = initial guess, out = result.
-// COUNT (measurement instantiation): work gains 1 << 16 per level set-up that builds the template and 1 per iteration that
-// forms the mismatch sums (one register for both: the product instantiation has none to spare).
-// lk_track_win repeats this level / iteration control flow (bounds tests, nxt at each exit, convergence, oscillation,
-// max_iter) for the other window sizes: a change to it here belongs there too.
-template <bool COUNT>
-__device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
-                         int max_iter, double eps2, float eps_lo, float eps_hi, float eig_q, float& err_out, uint8_t* sP, int* sD,
-                         int lane, int& work) {
-    using kltsetup::WIN;
-    // lane l < 27 owns the three horizontally adjacent window pixels 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..),
-    // so the search-image taps of a lane are 4 consecutive bytes on two rows; the integer window sums are order independent.
-    constexpr int PER_LANE = 3;
-    const float half = (WIN - 1) * 0.5f;
-    const float FLT_SCALE = 1.f / (1 << 20);
-    const int lane_row = lane / 3, lane_col = 3 * (lane - 3 * (lane / 3));
-    bool status = true;
-    float err = 0.f;   // the numerator q of minEig (lk_eig_num)
+// ---- Window layouts.  lk_track runs the level / iteration control flow for both; its Win parameter does a level's window
+// work in the warp's shared memory (sN bytes, sD ints) and registers:
+//   Win(lane, sN, sD, win)                                 once per track
+//   level(Jimg, Jpitch, lw, lh)                            a level's search image
+//   setup(Iimg, Ipitch, ix, iy, iw.., A11, A12, A22)      template window and normal matrix (float32, scaled by 2^-20)
+//   search(jx, jy)                                         the search pixels of a new integer window origin
+//   mismatch(iw.., b1, b2)                                 one iteration's mismatch sums (float32, scaled by 2^-20)
+// and gives its kernel instantiation's warps per CTA, launch bounds and per-warp shared memory.
+constexpr float LK_SCALE = 1.f / (1 << 20);
 
-    for (int level = maxlevel; level >= 0; --level) {
-        const int lw = Ipyr.w[level], lh = Ipyr.h[level];
-        const uint8_t* Iimg = Ipyr.lvl[level] + Ipyr.fstride[level] * frame;
-        const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
-        const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
-        const bool packed_ok = ((reinterpret_cast<uintptr_t>(Jimg) | (uintptr_t)Jpitch) & 3) == 0;   // aliased level 0 may be unaligned
-        const uint8_t* Jlane = Jimg + lane_row * Jpitch;
-        const float sc = __int_as_float((127 - level) << 23);   // 2^-level, exactly 1.f / (1 << level)
-        float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
-        float2 nextPt;
-        if (level == maxlevel) nextPt = make_float2(nxt.x * sc, nxt.y * sc);
-        else nextPt = make_float2(nxt.x * 2.f, nxt.y * 2.f);
-        nxt = nextPt;
-        prevPt.x -= half;
-        prevPt.y -= half;
-        const int ix = __float2int_rd(prevPt.x), iy = __float2int_rd(prevPt.y);
-        if (ix < -WIN || ix >= lw || iy < -WIN || iy >= lh) {
-            if (level == 0) { status = false; err = 0.f; }
-            continue;
-        }
-        if (COUNT) work += 1 << 16;
-        float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
-        int iw00, iw01, iw10, iw11;
-        LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
+// 9 x 9, the window of every shipped configuration.  Lane l < 27 owns the three horizontally adjacent window pixels
+// 3l .. 3l+2 (row l / 3, columns 3 (l % 3) ..), so the search-image taps of a lane are 4 consecutive bytes on two rows,
+// packed in registers; the integer window sums are order independent.  Lanes 27..31 keep zero taps against a zero
+// template, so every lane runs the same straight-line arithmetic.
+struct Win9 {
+    static constexpr const char* NAME = "fb_klt_kernel";
+    static constexpr int WARPS = 8, MIN_CTAS = 32 / WARPS;
+    static constexpr int SN_BYTES = kltsetup::SP_BYTES, SD_INTS = kltsetup::SD_INTS;
+    __host__ __device__ static constexpr int size(int) { return kltsetup::WIN; }
 
-        // ---- level set-up (klt_setup.cuh): 12 x 12 neighbourhood -> shared memory (aligned words on the
-        //      interior path), Scharr at the 10 x 10 bilinear footprint, int16 template window (as sign-extended ints) +
-        //      exact integer normal-equation sums.  Lane l < 27 owns window pixels 3l .. 3l+2; lanes 27..31 get zeros.
-        __syncwarp();
+    const int lane, lane_row, lane_col;
+    uint8_t* const sP;
+    int* const sD;
+    int Jpitch, lw, lh;
+    bool packed_ok;   // aliased level 0 may be unaligned
+    const uint8_t* Jlane;
+    int I0, I1, I2, X0, X1, X2, Y0, Y1, Y2;   // the template values as the iterations use them
+    int gsum;                                 // sum |Ix| + |Iy| over the window
+    unsigned top, bot;                        // the lane's search taps
+
+    __device__ __forceinline__ Win9(int lane, uint8_t* sN, int* sD, int)
+        : lane(lane), lane_row(lane / 3), lane_col(3 * (lane - 3 * (lane / 3))), sP(sN), sD(sD) {}
+    __device__ __forceinline__ void level(const uint8_t* Jimg, int pitch, int w, int h) {
+        Jpitch = pitch;
+        lw = w;
+        lh = h;
+        packed_ok = ((reinterpret_cast<uintptr_t>(Jimg) | (uintptr_t)Jpitch) & 3) == 0;
+        Jlane = Jimg + lane_row * Jpitch;
+        top = 0;
+        bot = 0;
+    }
+
+    // klt_setup.cuh: 12 x 12 neighbourhood -> shared memory (aligned words on the interior path), Scharr at the 10 x 10
+    // bilinear footprint, int16 template window (as sign-extended ints) + exact integer normal-equation sums.
+    __device__ __forceinline__ void setup(const uint8_t* Iimg, int Ipitch, int ix, int iy, int iw00, int iw01, int iw10,
+                                          int iw11, float& A11, float& A12, float& A22) {
         const bool tmpl_aligned = ((reinterpret_cast<uintptr_t>(Iimg) | (uintptr_t)Ipitch) & 3) == 0;
-        int Iv[PER_LANE], Ixv[PER_LANE], Iyv[PER_LANE];
+        int Iv[3], Ixv[3], Iyv[3];
         int sA11, sA12, sA22;
         if (tmpl_aligned && kltsetup::patch_interior(ix, iy, lw, lh)) {
             // interior (warp-uniform): interpolate first, differentiate after - same integers, one pass, no derivative patch
@@ -199,106 +196,114 @@ __device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, fl
             __syncwarp();
             kltsetup::template_rows(lane, sP, 0, sD, iw00, iw01, iw10, iw11, Iv, Ixv, Iyv, sA11, sA12, sA22);
         }
-        // the template values as the iterations use them
-        const int I0 = Iv[0], I1 = Iv[1], I2 = Iv[2];
-        const int X0 = Ixv[0], X1 = Ixv[1], X2 = Ixv[2];
-        const int Y0 = Iyv[0], Y1 = Iyv[1], Y2 = Iyv[2];
-        // |b sums| <= max|J - I| * sum|Ix| with |J - I| <= 8160 (both are 8-bit intensities with 5 fractional bits): when
-        // 8160 * (sum|Ix| + sum|Iy|) < 2^31 the iterations' mismatch sums fit one exact 32-bit redux each (true for
-        // every window whose mean |gradient| is below ~3200 of the possible 8160, i.e. anything but a synthetic
-        // checkerboard; 8162 * 262000 < 2^31); otherwise the split 64-bit reduction is kept.  Same integers either way.
-        const int sabs = abs(X0) + abs(X1) + abs(X2) + abs(Y0) + abs(Y1) + abs(Y2);
-        const bool b32 = __reduce_add_sync(FULL, sabs) < 262000;
+        I0 = Iv[0], I1 = Iv[1], I2 = Iv[2];
+        X0 = Ixv[0], X1 = Ixv[1], X2 = Ixv[2];
+        Y0 = Iyv[0], Y1 = Iyv[1], Y2 = Iyv[2];
+        gsum = __reduce_add_sync(FULL, abs(X0) + abs(X1) + abs(X2) + abs(Y0) + abs(Y1) + abs(Y2));
         // |window sums| <= 81 * 4080^2 = 1.35e9 < 2^31 for the 9 x 9 window: one exact 32-bit redux each
         // (the b sums of the iterations can reach 2.7e9 and keep the split 64-bit reduction)
-        const float A11 = __int2float_rn(__reduce_add_sync(FULL, sA11)) * FLT_SCALE;
-        const float A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * FLT_SCALE;
-        const float A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * FLT_SCALE;
-        float D = A11 * A22 - A12 * A12;
-        err = lk_eig_num(A11, A12, A22);
-        if (err < eig_q || D < LK_MIN_DET) {
-            if (level == 0) status = false;
-            continue;
-        }
-        D = 1.f / D;
-        nextPt.x -= half;
-        nextPt.y -= half;
-        float2 prevDelta = make_float2(0.f, 0.f);
-        // The lane's taps are gathered when the integer origin (jx, jy) of the window moves and kept while it does not
-        // (sub-pixel steps only change the bilinear weights).  Lanes 27..31 keep zero taps against a zero template, so every
-        // lane runs the same straight-line arithmetic.  nxt is written where the loop ends, not every iteration: the
-        // values are those OpenCV leaves in nextPts at each exit.
-        int cjx = INT_MIN, cjy = INT_MIN;
-        unsigned top = 0, bot = 0;
-        int j = 0;
-        for (; j < max_iter; ++j) {
-            const int jx = __float2int_rd(nextPt.x), jy = __float2int_rd(nextPt.y);
-            if ((jx != cjx) | (jy != cjy)) {
-                if (jx < -WIN || jx >= lw || jy < -WIN || jy >= lh) {
-                    if (j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
-                    if (level == 0) status = false;
-                    break;
-                }
-                if (lane < 27) gather_taps(Jlane, Jpitch, lw, lh, jx, jy, lane_row, lane_col, packed_ok, top, bot);
-                cjx = jx;
-                cjy = jy;
-            }
-            if (COUNT) ++work;
-            a = nextPt.x - (float)jx;
-            b = nextPt.y - (float)jy;
-            LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
-            // the 14-bit bilinear weights as signed 16-bit pairs, applied to the packed taps with dp2a (u16 x u8 pairs):
-            // the same integers as (J00 iw00 + J01 iw01 + J10 iw10 + J11 iw11 + 2^8) >> 9, exact in int32
-            const unsigned W01 = __byte_perm((unsigned)iw00, (unsigned)iw01, 0x5410);
-            const unsigned W23 = __byte_perm((unsigned)iw10, (unsigned)iw11, 0x5410);
-            const int j0 = kltsetup::dp2a_lo_su16(W01, top, kltsetup::dp2a_lo_su16(W23, bot, 256)) >> 9;
-            const int j1 = kltsetup::dp2a_lo_su16(W01, top >> 8, kltsetup::dp2a_lo_su16(W23, bot >> 8, 256)) >> 9;
-            const int j2 = kltsetup::dp2a_hi_su16(W01, top, kltsetup::dp2a_hi_su16(W23, bot, 256)) >> 9;
-            const int d0 = j0 - I0, d1 = j1 - I1, d2 = j2 - I2;
-            const int sb1 = d0 * X0 + d1 * X1 + d2 * X2;
-            const int sb2 = d0 * Y0 + d1 * Y1 + d2 * Y2;
-            float b1, b2;
-            if (b32) {
-                b1 = __int2float_rn(__reduce_add_sync(FULL, sb1)) * FLT_SCALE;
-                b2 = __int2float_rn(__reduce_add_sync(FULL, sb2)) * FLT_SCALE;
-            } else {
-                b1 = __ll2float_rn(warp_sum64(sb1)) * FLT_SCALE;
-                b2 = __ll2float_rn(warp_sum64(sb2)) * FLT_SCALE;
-            }
-            const float2 delta = lk_step(A11, A12, A22, D, b1, b2);
-            nextPt.x += delta.x;
-            nextPt.y += delta.y;
-            LK_CONVERGED(conv, delta, eps2, eps_lo, eps_hi);
-            if (conv) {
-                nxt = make_float2(nextPt.x + half, nextPt.y + half);
-                break;
-            }
-            if (j > 0 && LK_OSCILLATES(delta, prevDelta)) {
-                nxt = make_float2((nextPt.x + half) - delta.x * 0.5f, (nextPt.y + half) - delta.y * 0.5f);
-                break;
-            }
-            prevDelta = delta;
-        }
-        if (j == max_iter && j > 0) nxt = make_float2(nextPt.x + half, nextPt.y + half);
+        A11 = __int2float_rn(__reduce_add_sync(FULL, sA11)) * LK_SCALE;
+        A12 = __int2float_rn(__reduce_add_sync(FULL, sA12)) * LK_SCALE;
+        A22 = __int2float_rn(__reduce_add_sync(FULL, sA22)) * LK_SCALE;
     }
-    err_out = err;
-    return status;
-}
 
-// One calcOpticalFlowPyrLK track with a win x win window, 3 <= win <= 31, any size but 9 (whole warp cooperates).  Lane c
-// owns window column c (klt_setup.cuh, win_*): the level set-up stages the (win + 3)^2 template neighbourhood, its Scharr
-// derivatives and the template into the warp's shared memory, and each move of the integer search origin stages the
-// (win + 1)^2 search bytes into the neighbourhood's buffer.  A lane's column sums are exact in int32, the window sums in
-// 64 bits.  Float32 steps and COUNT as in lk_track.  The level / iteration control flow repeats lk_track's (kept apart so that
-// fb_klt_kernel's code stays as it is): a change to it here belongs there too.
-template <bool COUNT>
-__device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel,
-                             int win, int max_iter, double eps2, float eps_lo, float eps_hi, float eig_q, float& err_out,
-                             uint8_t* sN, int* sD, int lane, int& work) {
-    int* sG = sD + kltsetup::WD_INTS;
-    short* sI = reinterpret_cast<short*>(sG + kltsetup::WT_ELEMS);
+    __device__ __forceinline__ void search(int jx, int jy) {
+        if (lane < 27) gather_taps(Jlane, Jpitch, lw, lh, jx, jy, lane_row, lane_col, packed_ok, top, bot);
+    }
+
+    __device__ __forceinline__ void mismatch(int iw00, int iw01, int iw10, int iw11, float& b1, float& b2) const {
+        // the 14-bit bilinear weights as signed 16-bit pairs, applied to the packed taps with dp2a (u16 x u8 pairs):
+        // the same integers as (J00 iw00 + J01 iw01 + J10 iw10 + J11 iw11 + 2^8) >> 9, exact in int32
+        const unsigned W01 = __byte_perm((unsigned)iw00, (unsigned)iw01, 0x5410);
+        const unsigned W23 = __byte_perm((unsigned)iw10, (unsigned)iw11, 0x5410);
+        const int j0 = kltsetup::dp2a_lo_su16(W01, top, kltsetup::dp2a_lo_su16(W23, bot, 256)) >> 9;
+        const int j1 = kltsetup::dp2a_lo_su16(W01, top >> 8, kltsetup::dp2a_lo_su16(W23, bot >> 8, 256)) >> 9;
+        const int j2 = kltsetup::dp2a_hi_su16(W01, top, kltsetup::dp2a_hi_su16(W23, bot, 256)) >> 9;
+        const int d0 = j0 - I0, d1 = j1 - I1, d2 = j2 - I2;
+        const int sb1 = d0 * X0 + d1 * X1 + d2 * X2;
+        const int sb2 = d0 * Y0 + d1 * Y1 + d2 * Y2;
+        // |b sums| <= max|J - I| * sum|Ix| with |J - I| <= 8160 (both are 8-bit intensities with 5 fractional bits): when
+        // 8160 * (sum|Ix| + sum|Iy|) < 2^31 the mismatch sums fit one exact 32-bit redux each (true for every window whose
+        // mean |gradient| is below ~3200 of the possible 8160, i.e. anything but a synthetic checkerboard;
+        // 8162 * 262000 < 2^31); otherwise the split 64-bit reduction is kept.  Same integers either way.
+        if (gsum < 262000) {
+            b1 = __int2float_rn(__reduce_add_sync(FULL, sb1)) * LK_SCALE;
+            b2 = __int2float_rn(__reduce_add_sync(FULL, sb2)) * LK_SCALE;
+        } else {
+            b1 = __ll2float_rn(warp_sum64(sb1)) * LK_SCALE;
+            b2 = __ll2float_rn(warp_sum64(sb2)) * LK_SCALE;
+        }
+    }
+};
+
+// Any window from 3 to 31 but 9.  Lane c owns window column c (klt_setup.cuh, win_*): the level set-up stages the
+// (win + 3)^2 template neighbourhood, its Scharr derivatives and the template into the warp's shared memory, and each
+// move of the integer search origin stages the (win + 1)^2 search bytes into the neighbourhood's buffer.  A lane's column
+// sums are exact in int32, the window sums in 64 bits.  Per warp: the staged bytes (WN_BYTES), then the derivative plane,
+// the template derivatives (ints) and the template intensities (shorts) in one int array; 11 272 bytes.
+struct WinAny {
+    static constexpr const char* NAME = "fb_klt_win_kernel";
+    static constexpr int WARPS = 4, MIN_CTAS = 0;
+    static constexpr int SN_BYTES = kltsetup::WN_BYTES;
+    static constexpr int SD_INTS = kltsetup::WD_INTS + kltsetup::WT_ELEMS + kltsetup::WT_ELEMS / 2;
+    __host__ __device__ static constexpr int size(int win) { return win; }
+
+    const int lane, win;
+    uint8_t* const sN;
+    int* const sD;
+    int* const sG;
+    short* const sI;
+    const uint8_t* Jimg;
+    int Jpitch, lw, lh;
+
+    __device__ __forceinline__ WinAny(int lane, uint8_t* sN, int* sD, int win)
+        : lane(lane), win(win), sN(sN), sD(sD), sG(sD + kltsetup::WD_INTS),
+          sI(reinterpret_cast<short*>(sD + kltsetup::WD_INTS + kltsetup::WT_ELEMS)) {}
+    __device__ __forceinline__ void level(const uint8_t* img, int pitch, int w, int h) {
+        Jimg = img;
+        Jpitch = pitch;
+        lw = w;
+        lh = h;
+    }
+
+    __device__ __forceinline__ void setup(const uint8_t* Iimg, int Ipitch, int ix, int iy, int iw00, int iw01, int iw10,
+                                          int iw11, float& A11, float& A12, float& A22) {
+        kltsetup::win_stage(lane, Iimg, Ipitch, lw, lh, ix - 1, iy - 1, win + 3, sN);
+        __syncwarp();
+        kltsetup::win_scharr(lane, sN, ix, iy, lw, lh, win, sD);
+        __syncwarp();
+        int sA11, sA12, sA22;
+        kltsetup::win_template(lane, sN, sD, win, iw00, iw01, iw10, iw11, sI, sG, sA11, sA12, sA22);
+        A11 = __ll2float_rn(warp_sum64(sA11)) * LK_SCALE;
+        A12 = __ll2float_rn(warp_sum64(sA12)) * LK_SCALE;
+        A22 = __ll2float_rn(warp_sum64(sA22)) * LK_SCALE;
+    }
+
+    __device__ __forceinline__ void search(int jx, int jy) {
+        __syncwarp();            // the template phase or the previous iteration is done with sN
+        kltsetup::win_stage(lane, Jimg, Jpitch, lw, lh, jx, jy, win + 1, sN);
+        __syncwarp();
+    }
+
+    __device__ __forceinline__ void mismatch(int iw00, int iw01, int iw10, int iw11, float& b1, float& b2) const {
+        int sb1, sb2;
+        kltsetup::win_mismatch(lane, sN, sI, sG, win, iw00, iw01, iw10, iw11, sb1, sb2);
+        b1 = __ll2float_rn(warp_sum64(sb1)) * LK_SCALE;
+        b2 = __ll2float_rn(warp_sum64(sb2)) * LK_SCALE;
+    }
+};
+
+// One calcOpticalFlowPyrLK track for one point with Win's window (whole warp cooperates).
+// Ipyr = template pyramid, Jpyr = search pyramid.  nxt: in = initial guess, out = result.
+// COUNT (measurement instantiation): work gains 1 << 16 per level set-up that builds the template and 1 per iteration that
+// forms the mismatch sums (one register for both: the product instantiation has none to spare).
+template <bool COUNT, class Win>
+__device__ bool lk_track(const PyrView& Ipyr, const PyrView& Jpyr, int frame, float2 pt, float2& nxt, int maxlevel, int win,
+                         int max_iter, double eps2, float eps_lo, float eps_hi, float eig_q, float& err_out, uint8_t* sN, int* sD,
+                         int lane, int& work) {
+    win = Win::size(win);
+    Win W(lane, sN, sD, win);
     const float half = (win - 1) * 0.5f;
-    const float FLT_SCALE = 1.f / (1 << 20);
     bool status = true;
     float err = 0.f;   // the numerator q of minEig (lk_eig_num)
 
@@ -307,6 +312,7 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
         const uint8_t* Iimg = Ipyr.lvl[level] + Ipyr.fstride[level] * frame;
         const uint8_t* Jimg = Jpyr.lvl[level] + Jpyr.fstride[level] * frame;
         const int Ipitch = Ipyr.pitch[level], Jpitch = Jpyr.pitch[level];
+        W.level(Jimg, Jpitch, lw, lh);
         const float sc = __int_as_float((127 - level) << 23);   // 2^-level, exactly 1.f / (1 << level)
         float2 prevPt = make_float2(pt.x * sc, pt.y * sc);
         float2 nextPt;
@@ -324,16 +330,9 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
         float a = prevPt.x - (float)ix, b = prevPt.y - (float)iy;
         int iw00, iw01, iw10, iw11;
         LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
-        __syncwarp();                    // the previous level's iterations are done with sN
-        kltsetup::win_stage(lane, Iimg, Ipitch, lw, lh, ix - 1, iy - 1, win + 3, sN);
-        __syncwarp();
-        kltsetup::win_scharr(lane, sN, ix, iy, lw, lh, win, sD);
-        __syncwarp();
-        int sA11, sA12, sA22;
-        kltsetup::win_template(lane, sN, sD, win, iw00, iw01, iw10, iw11, sI, sG, sA11, sA12, sA22);
-        const float A11 = __ll2float_rn(warp_sum64(sA11)) * FLT_SCALE;
-        const float A12 = __ll2float_rn(warp_sum64(sA12)) * FLT_SCALE;
-        const float A22 = __ll2float_rn(warp_sum64(sA22)) * FLT_SCALE;
+        __syncwarp();                    // the previous level's iterations are done with the warp's shared memory
+        float A11, A12, A22;
+        W.setup(Iimg, Ipitch, ix, iy, iw00, iw01, iw10, iw11, A11, A12, A22);
         float D = A11 * A22 - A12 * A12;
         err = lk_eig_num(A11, A12, A22);
         if (err < eig_q || D < LK_MIN_DET) {
@@ -344,7 +343,9 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
         nextPt.x -= half;
         nextPt.y -= half;
         float2 prevDelta = make_float2(0.f, 0.f);
-        // search bytes are staged when the integer origin (jx, jy) moves and kept while it does not
+        // The search pixels are fetched when the integer origin (jx, jy) of the window moves and kept while it does not
+        // (sub-pixel steps only change the bilinear weights).  nxt is written where the loop ends, not every iteration:
+        // the values are those OpenCV leaves in nextPts at each exit.
         int cjx = INT_MIN, cjy = INT_MIN;
         int j = 0;
         for (; j < max_iter; ++j) {
@@ -355,9 +356,7 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
                     if (level == 0) status = false;
                     break;
                 }
-                __syncwarp();            // the template phase or the previous iteration is done with sN
-                kltsetup::win_stage(lane, Jimg, Jpitch, lw, lh, jx, jy, win + 1, sN);
-                __syncwarp();
+                W.search(jx, jy);
                 cjx = jx;
                 cjy = jy;
             }
@@ -365,10 +364,8 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
             a = nextPt.x - (float)jx;
             b = nextPt.y - (float)jy;
             LK_WEIGHTS(a, b, iw00, iw01, iw10, iw11);
-            int sb1, sb2;
-            kltsetup::win_mismatch(lane, sN, sI, sG, win, iw00, iw01, iw10, iw11, sb1, sb2);
-            const float b1 = __ll2float_rn(warp_sum64(sb1)) * FLT_SCALE;
-            const float b2 = __ll2float_rn(warp_sum64(sb2)) * FLT_SCALE;
+            float b1, b2;
+            W.mismatch(iw00, iw01, iw10, iw11, b1, b2);
             const float2 delta = lk_step(A11, A12, A22, D, b1, b2);
             nextPt.x += delta.x;
             nextPt.y += delta.y;
@@ -391,9 +388,8 @@ __device__ bool lk_track_win(const PyrView& Ipyr, const PyrView& Jpyr, int frame
 
 // One keypoint, whole warp: forward track, checks, backward track, forward-backward test (feature_tracker.cpp:35-137).
 // counts (measurement instantiation): level set-ups and iterations of both tracks, at 2 i and 2 i + 1.
-// ANY_WIN: track with lk_track_win and a win x win window, else with lk_track (9 x 9).
-template <bool COUNT, bool ANY_WIN>
-__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, int* sDw, int lane, int32_t* counts, int win) {
+template <bool COUNT, class Win>
+__device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sNw, int* sDw, int lane, int32_t* counts, int win) {
     const int frame = A.frame_idx ? A.frame_idx[i] : A.first_frame + i / A.per_frame;
     int maxlevel = A.lvls ? (int)A.lvls[i] : A.lvl_all;
     if (maxlevel > A.prev.nlev - 1) maxlevel = A.prev.nlev - 1;  // feature_tracker.cpp:50-52
@@ -404,13 +400,8 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
     int work = 0;
     // x < 0 marks an empty slot of a fixed-stride batch (the detectors pad their output with (-1, -1),
     // ov2_describe uses the same rule): status 0, prior untouched, no work
-    bool ok;
-    if constexpr (ANY_WIN)
-        ok = kp.x >= 0.f && lk_track_win<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, win, A.max_iter, A.eps2, A.eps_lo,
-                                                A.eps_hi, A.eig_q, err, sPw, sDw, lane, work);
-    else
-        ok = kp.x >= 0.f && lk_track<COUNT>(A.prev, A.cur, frame, kp, fwd, maxlevel, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
-                                            A.eig_q, err, sPw, sDw, lane, work);
+    bool ok = kp.x >= 0.f && lk_track<COUNT, Win>(A.prev, A.cur, frame, kp, fwd, maxlevel, win, A.max_iter, A.eps2, A.eps_lo,
+                                                  A.eps_hi, A.eig_q, err, sNw, sDw, lane, work);
     // feature_tracker.cpp:79-101 (err > ferr and the distance test through the thresholds of KltArgs)
     if (ok && err > A.ferr_q) ok = false;
     if (ok) {
@@ -421,13 +412,8 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
         // backward: template from the current image at the forward result, search the previous image
         float2 back = kp;
         float err2 = 0.f;
-        bool ok2;
-        if constexpr (ANY_WIN)
-            ok2 = lk_track_win<COUNT>(A.cur, A.prev, frame, fwd, back, 0, win, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, A.eig_q,
-                                      err2, sPw, sDw, lane, work);
-        else
-            ok2 = lk_track<COUNT>(A.cur, A.prev, frame, fwd, back, 0, A.max_iter, A.eps2, A.eps_lo, A.eps_hi, A.eig_q, err2, sPw,
-                                  sDw, lane, work);
+        const bool ok2 = lk_track<COUNT, Win>(A.cur, A.prev, frame, fwd, back, 0, win, A.max_iter, A.eps2, A.eps_lo, A.eps_hi,
+                                              A.eig_q, err2, sNw, sDw, lane, work);
         if (!ok2) ok = false;
         else {
             float dx = kp.x - back.x, dy = kp.y - back.y;
@@ -448,10 +434,12 @@ __device__ __forceinline__ void klt_one(const KltArgs& A, int i, uint8_t* sPw, i
 // assignment leaves SM slots idle while the slowest warp of a CTA finishes.  When the grid exceeds the
 // resident CTAs, the launch fills the GPU once and every warp pulls the next keypoint from a global counter;
 // it asks for the next index before tracking the current one, so the atomic's round trip overlaps the track.
-// Both kernels run their warps through this loop: NW warps per CTA, sPw / sDw the warp's shared memory.
-template <int NW, bool COUNT, bool ANY_WIN>
-__device__ __forceinline__ void klt_warps(const KltArgs& A, int warp, int lane, uint8_t* sPw, int* sDw, int32_t* counts, int win) {
-    int i = blockIdx.x * NW + warp;
+template <bool COUNT, class Win>
+__global__ void __launch_bounds__(Win::WARPS * 32, Win::MIN_CTAS) fb_klt_kernel(KltArgs A, int32_t* counts, int win) {
+    __shared__ __align__(16) uint8_t sNall[Win::WARPS][Win::SN_BYTES];
+    __shared__ __align__(16) int sDall[Win::WARPS][Win::SD_INTS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int i = blockIdx.x * Win::WARPS + warp;
     if (A.work_counter) {
         int first = 0;
         if (lane == 0) first = atomicAdd(A.work_counter, 1);
@@ -460,31 +448,10 @@ __device__ __forceinline__ void klt_warps(const KltArgs& A, int warp, int lane, 
     while (i < A.n) {
         int nxt_i = 0;
         if (A.work_counter && lane == 0) nxt_i = atomicAdd(A.work_counter, 1);
-        klt_one<COUNT, ANY_WIN>(A, i, sPw, sDw, lane, counts, win);
+        klt_one<COUNT, Win>(A, i, sNall[warp], sDall[warp], lane, counts, win);
         if (!A.work_counter) return;
         i = __shfl_sync(FULL, nxt_i, 0);
     }
-}
-
-template <bool COUNT>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 32 / WARPS_PER_CTA) fb_klt_kernel(KltArgs A, int32_t* counts) {
-    __shared__ __align__(16) uint8_t sPall[WARPS_PER_CTA][kltsetup::SP_BYTES];
-    __shared__ __align__(16) int sDall[WARPS_PER_CTA][kltsetup::SD_INTS];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    klt_warps<WARPS_PER_CTA, COUNT, false>(A, warp, lane, sPall[warp], sDall[warp], counts, 9);
-}
-
-// Any window from 3 to 31 but 9.  Per warp: the staged bytes (WN_BYTES), then the derivative plane, the template
-// derivatives (ints) and the template intensities (shorts) in one int array; 11 272 bytes, 45 088 per CTA.
-constexpr int WIN_WARPS_PER_CTA = 4;
-constexpr int WIN_WARP_INTS = kltsetup::WD_INTS + kltsetup::WT_ELEMS + kltsetup::WT_ELEMS / 2;
-
-template <bool COUNT>
-__global__ void __launch_bounds__(WIN_WARPS_PER_CTA * 32) fb_klt_win_kernel(KltArgs A, int32_t* counts, int win) {
-    __shared__ __align__(16) uint8_t sNall[WIN_WARPS_PER_CTA][kltsetup::WN_BYTES];
-    __shared__ __align__(16) int sWall[WIN_WARPS_PER_CTA][WIN_WARP_INTS];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    klt_warps<WIN_WARPS_PER_CTA, COUNT, true>(A, warp, lane, sNall[warp], sWall[warp], counts, win);
 }
 
 // Depth cv::buildOpticalFlowPyramid(img, pyr, Size(win, win), maxlevel) reaches: it stops before a level whose width or
@@ -494,6 +461,30 @@ int optflow_levels(const ov2_pyr* p, int win, int maxlevel) {
     for (int l = 0; l < maxlevel; ++l)
         if (p->w[l + 1] <= win || p->h[l + 1] <= win) return l;
     return maxlevel;
+}
+
+// Launches fb_klt_kernel with Win's layout, the counting instantiation when d_counts is set: one warp per keypoint, or the
+// persistent launch over the work counter when the grid exceeds the resident CTAs.
+template <class Win>
+ov2_status klt_run(ov2_ctx* ctx, KltArgs& A, int n, int32_t* d_counts, int win) {
+    constexpr int threads = Win::WARPS * 32;
+    int grid = div_up(n, Win::WARPS), per_sm = 0;
+    A.work_counter = nullptr;
+    OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false, Win>, threads, 0));
+    const int resident = per_sm * ctx->sm_count;
+    if (grid > resident) {
+        void* o = nullptr;
+        const ov2_status st = ov2_scratch(ctx, sizeof(int), &o);
+        if (st != OV2_OK) return st;
+        A.work_counter = (int*)o;
+        OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
+        grid = resident;
+    }
+    if (d_counts)
+        OV2_LAUNCH(ctx, Win::NAME, (fb_klt_kernel<true, Win><<<grid, threads, 0, ctx->stream>>>(A, d_counts, win)));
+    else
+        OV2_LAUNCH(ctx, Win::NAME, (fb_klt_kernel<false, Win><<<grid, threads, 0, ctx->stream>>>(A, nullptr, win)));
+    return OV2_OK;
 }
 
 // ov2_fb_klt, and with counts_out the counting instantiation of the kernel behind ov2_debug_klt_counts
@@ -545,33 +536,9 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
         if ((st = ov2_stage_out(ctx, counts_out, sizeof(int32_t) * 2 * (size_t)n, &o)) != OV2_OK) return st;
         d_counts = (int32_t*)o;
     }
-    // 9 x 9 (every shipped configuration) keeps its own kernel; every other size runs fb_klt_win_kernel
-    const int win = prm->win;
-    const int nw = win == 9 ? WARPS_PER_CTA : WIN_WARPS_PER_CTA;
-    int grid = div_up(n, nw), per_sm = 0;
-    A.work_counter = nullptr;
-    if (win == 9)
-        OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false>, WARPS_PER_CTA * 32, 0));
-    else
-        OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_win_kernel<false>, WIN_WARPS_PER_CTA * 32, 0));
-    const int resident = per_sm * ctx->sm_count;
-    if (grid > resident) {
-        if ((st = ov2_scratch(ctx, sizeof(int), &o)) != OV2_OK) return st;
-        A.work_counter = (int*)o;
-        OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
-        grid = resident;
-    }
-    if (win != 9) {
-        if (d_counts)
-            OV2_LAUNCH(ctx, "fb_klt_win_kernel",
-                       (fb_klt_win_kernel<true><<<grid, WIN_WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, d_counts, win)));
-        else
-            OV2_LAUNCH(ctx, "fb_klt_win_kernel",
-                       (fb_klt_win_kernel<false><<<grid, WIN_WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, nullptr, win)));
-    } else if (d_counts)
-        OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<true><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, d_counts)));
-    else
-        OV2_LAUNCH(ctx, "fb_klt_kernel", (fb_klt_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, ctx->stream>>>(A, nullptr)));
+    // 9 x 9 (every shipped configuration) keeps its own layout; every other size runs the general one
+    st = prm->win == 9 ? klt_run<Win9>(ctx, A, n, d_counts, prm->win) : klt_run<WinAny>(ctx, A, n, d_counts, prm->win);
+    if (st != OV2_OK) return st;
     return ov2_end(ctx);
 }
 
