@@ -241,8 +241,18 @@ OV2_API ov2_status ov2_debug_subpix_iters(ov2_ctx* ctx, const ov2_pyr* pyr, int 
  * function tolerance 1e-3; blocks with chi2 > chi2th or non-positive depth after the first solve are flagged
  * in outlier_flags (and removed before an L2 re-solve when apply_l2_after_robust).  success_out[k] = the
  * reference's return value.  The 5 ms wall-clock cap of the reference (:538) is not modelled.
- * offsets must be a HOST pointer; iterations_out (optional) = LM iterations of the last solve of each problem.
- * Validated on the host against the oracle and on the GPU by tests/test_pnp_gpu.py. */
+ * offsets must be a HOST pointer, start at 0 and never decrease (else OV2_ERR_INVALID, nothing staged or
+ * written); the other arrays may be host or device memory.  An empty problem returns success 0 and its pose as
+ * given.  The start quaternion is normalised as Sophus' SE3d(q, t) would.  iterations_out (optional, NULL
+ * accepted) = LM iterations of the last solve of each problem: every iteration started, so a solve that a
+ * tolerance ends inside an iteration counts it, where Ceres' Summary::iterations.size() (which also counts
+ * iteration 0) does not.
+ * Known deviation: when a solve is unusable (five consecutive invalid steps, Ceres' FAILURE), Ceres restores the
+ * parameters it started from; this kernel writes its best iterate (success_out is 0 either way).
+ * Tested: the solve code compiled for the host against the oracle and against the real Ceres; the kernel by
+ * tests/test_pnp_gpu.py and tests/test_pnp_paths_gpu.py on 1 to 20 000 points per problem, per-problem K, levels
+ * 0-3 and NULL, every option the callers vary, points behind the camera, batches of > 1 000 problems, device
+ * buffers and refused offsets: success, outlier flags and iterations exact, pose to 1e-9 of the oracle. */
 OV2_API ov2_status ov2_pnp_solve(ov2_ctx* ctx, int nprob, const int32_t* offsets, const double* unpx, const double* wpts,
                          const int32_t* scales, const double* K, double* pose_inout, int nmaxiter, float chi2th,
                          int use_robust, int apply_l2_after_robust, uint8_t* outlier_flags, uint8_t* success_out,

@@ -25,7 +25,8 @@ makes the reference itself non-deterministic (Ceres checks it between iterations
 
 PINNING STATUS: pinned against the real Ceres 2.0 of the reference tree running the reference's own cost function with the calls
 ceresPnP makes (DENSE_QR, Huber wrapper, outlier scan, L2 refinement): same outliers, verdict and pose to 1e-9
-(tests/test_oracle_vs_reference_ceres.py::test_ceres_pnp_equals_real_ceres; that build uses a stand-in linear-algebra header instead
+(tests/test_oracle_vs_reference_ceres.py::test_ceres_pnp_equals_real_ceres), and on the edge cases also termination, costs and
+iteration count of every solve (::test_ceres_pnp_edges_and_iterations_equal_real_ceres; that build uses a stand-in linear-algebra header instead
 of Eigen, see oracle/ba_ref.py).  Also: the Jacobian against central differences, the whole solve against ground truth and against
 scipy.optimize.least_squares on the same cost (tests/test_oracle_pnp.py).
 """
@@ -67,13 +68,26 @@ def evaluate(pose, wpts, unpx, K, scales=None, need_jac=True):
 def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=None, function_tolerance=1e-3, log=None):
     """ceres::Solve on the residual blocks `active` with one SE3 block, DENSE_QR, Ceres 2.0 defaults
     (jacobi scaling, initial radius 1e4, eta irrelevant for a direct solver).  Returns
-    (pose, summary, last) with last = chi2 / depth_pos of the last Evaluate() of each active block."""
+    (pose, summary, last) with last = chi2 / depth_pos of the last Evaluate() of each active block.
+
+    summary["stop"] names the test that ended the solve: "max_iterations", "gradient" and "radius" are checked at the top of
+    the loop (Ceres' FinalizeIterationAndCheckIfMinimizerCanContinue, after it has recorded the iteration), "parameter",
+    "function" and "invalid" inside an iteration (Ceres returns before recording it).  So Ceres' Summary::iterations.size(),
+    which counts iteration 0, is summary["iterations"] + 1 for the first three and summary["iterations"] for the others.
+
+    log: when a list, one entry per decision the loop takes, with the values each decision compares:
+      {"gmax"}                                      gradient max-norm of an accepted point (against 1e-10)
+      {"it", "valid", "radius"}                     a step the linear solve could not use
+      {"it", "step_norm", "xnorm", "x_cost", "cand_cost", "mcc", "rho", "radius"}
+                                                    a valid step: step norm against 1e-8 (xnorm + 1e-8), |x_cost - cand_cost|
+                                                    against function_tolerance x_cost, rho against 1e-3 (rho is None when a
+                                                    tolerance ended the solve first)"""
     pose = np.asarray(pose, np.float64).copy()
     idx = np.nonzero(active)[0]
     last = dict(chi2=np.zeros(len(active)), depth_pos=np.ones(len(active), bool))
-    summ = dict(iterations=0, termination="NO_CONVERGENCE", initial_cost=0.0, final_cost=0.0, usable=True)
+    summ = dict(iterations=0, termination="NO_CONVERGENCE", stop="max_iterations", initial_cost=0.0, final_cost=0.0, usable=True)
     if len(idx) == 0:
-        summ["termination"] = "CONVERGENCE"
+        summ["termination"], summ["stop"] = "CONVERGENCE", "no_blocks"
         return pose, summ, last
     W, U = wpts[idx], unpx[idx]
     sc = None if scales is None else np.asarray(scales)[idx]
@@ -100,6 +114,8 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
     g = J.T @ r
     gmax = np.abs(np.concatenate([pose[:3], quat_normalize(pose[3:])]) - pose_plus(pose, -g)).max()
     J = J * scale
+    if log is not None:
+        log.append(dict(gmax=gmax))
     summ["initial_cost"] = x_cost
     minimum_cost, best = DBL_MAX, pose.copy()
     xnorm = -1.0
@@ -111,10 +127,10 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
         if iteration >= max_iters:
             break
         if step_successful and gmax <= 1e-10:
-            summ["termination"] = "CONVERGENCE"
+            summ["termination"], summ["stop"] = "CONVERGENCE", "gradient"
             break
         if radius <= 1e-32:
-            summ["termination"] = "CONVERGENCE"
+            summ["termination"], summ["stop"] = "CONVERGENCE", "radius"
             break
         iteration += 1
         if not reuse_diag:
@@ -127,9 +143,11 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
         Jstep = J @ step
         model_cost_change = -(Jstep * (r + Jstep / 2.0)).sum()
         if not (np.isfinite(step).all() and model_cost_change > 0.0):
+            if log is not None:
+                log.append(dict(it=iteration, valid=False, radius=radius))
             num_invalid += 1
             if num_invalid >= 5:
-                summ["termination"] = "FAILURE"
+                summ["termination"], summ["stop"] = "FAILURE", "invalid"
                 summ["usable"] = False
                 break
             radius, decrease_factor = lm_step_rejected(radius, decrease_factor)
@@ -142,15 +160,19 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
         cand_cost, _ = cost_and_w(ev)
         if not np.isfinite(cand_cost):
             cand_cost = DBL_MAX
-        if np.sqrt(((pose - cand) ** 2).sum()) <= 1e-8 * (xnorm + 1e-8):
-            summ["termination"] = "CONVERGENCE"
+        step_norm = np.sqrt(((pose - cand) ** 2).sum())
+        entry = dict(it=iteration, valid=True, step_norm=step_norm, xnorm=xnorm, x_cost=x_cost, cand_cost=cand_cost, mcc=model_cost_change,
+                     rho=None, radius=radius)
+        if log is not None:
+            log.append(entry)
+        if step_norm <= 1e-8 * (xnorm + 1e-8):
+            summ["termination"], summ["stop"] = "CONVERGENCE", "parameter"
             break
         if abs(x_cost - cand_cost) <= function_tolerance * x_cost:
-            summ["termination"] = "CONVERGENCE"
+            summ["termination"], summ["stop"] = "CONVERGENCE", "function"
             break
         rel = -DBL_MAX if cand_cost >= DBL_MAX else (x_cost - cand_cost) / model_cost_change
-        if log is not None:
-            log.append(dict(it=iteration, x_cost=x_cost, cand_cost=cand_cost, rho=rel, radius=radius))
+        entry["rho"] = rel
         if rel > 1e-3:
             pose = cand
             xnorm = np.sqrt((pose ** 2).sum())
@@ -158,6 +180,8 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
             g = J.T @ r
             gmax = np.abs(pose - pose_plus(pose, -g)).max()
             J = J * scale
+            if log is not None:
+                log.append(dict(gmax=gmax))
             step_successful = True
             radius = lm_step_accepted(radius, rel)
             decrease_factor, reuse_diag = 2.0, False
@@ -169,19 +193,31 @@ def ceres_solve_pose(pose, wpts, unpx, K, active, max_iters, huber_a, scales=Non
     return best, summ, last
 
 
-def ceres_pnp(unpx, wpts, Twc, K, nmaxiter=5, chi2th=5.9915, use_robust=True, apply_l2_after_robust=True, scales=None):
-    """MultiViewGeometry::ceresPnP.  Returns (success, Twc_out, outlier indices)."""
+def ceres_pnp(unpx, wpts, Twc, K, nmaxiter=5, chi2th=5.9915, use_robust=True, apply_l2_after_robust=True, scales=None, summary=False):
+    """MultiViewGeometry::ceresPnP.  Returns (success, Twc_out, outlier indices); with summary=True also a dict:
+    summary      the Solver::Summary of the last solve that ran (see ceres_solve_pose)
+    solves       the summaries of every solve that ran (1 or 2)
+    log          per solve, the decision log of ceres_solve_pose
+    chi2, depth_pos, chi2th
+                 what the outlier scan after the first solve compared: chi2 > chi2th or not depth_pos is an outlier."""
     unpx = np.asarray(unpx, np.float64).reshape(-1, 2)
     wpts = np.asarray(wpts, np.float64).reshape(-1, 3)
     n = len(unpx)
     active = np.ones(n, bool)
     a = float(np.sqrt(np.float32(chi2th))) if use_robust else None     # chi2th is a float argument (:496)
     chi2th = float(np.float32(chi2th))
-    pose, summ, last = ceres_solve_pose(np.asarray(Twc, np.float64), wpts, unpx, K, active, nmaxiter, a, scales)
+    logs = [[]]
+    pose, summ, last = ceres_solve_pose(np.asarray(Twc, np.float64), wpts, unpx, K, active, nmaxiter, a, scales, log=logs[0])
+    info = dict(summary=summ, solves=[summ], log=logs, chi2=last["chi2"].copy(), depth_pos=last["depth_pos"].copy(), chi2th=chi2th)
     bad = (last["chi2"] > chi2th) | ~last["depth_pos"]
     outliers = np.nonzero(bad)[0]
     if len(outliers) == n:
-        return False, np.asarray(Twc, np.float64).copy(), outliers     # Twc is not written back (:568-570)
+        ret = (False, np.asarray(Twc, np.float64).copy(), outliers)   # Twc is not written back (:568-570)
+        return ret + (info,) if summary else ret
     if apply_l2_after_robust and len(outliers):
-        pose, summ, last = ceres_solve_pose(pose, wpts, unpx, K, ~bad, nmaxiter, None, scales)
-    return bool(summ["usable"]), pose, outliers
+        logs.append([])
+        pose, summ, last = ceres_solve_pose(pose, wpts, unpx, K, ~bad, nmaxiter, None, scales, log=logs[1])
+        info["summary"] = summ
+        info["solves"].append(summ)
+    ret = (bool(summ["usable"]), pose, outliers)
+    return ret + (info,) if summary else ret

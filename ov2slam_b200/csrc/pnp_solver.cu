@@ -97,8 +97,11 @@ extern "C" ov2_status ov2_pnp_solve(ov2_ctx* ctx, int nprob, const int32_t* offs
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: bad arguments");
     if (nprob == 0) return OV2_OK;
     if (ov2_is_device_ptr(offsets)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must be a host pointer");
+    // every block reads offsets[pb] .. offsets[pb + 1] of buffers sized offsets[nprob]: a descending pair would read past them
+    if (offsets[0] != 0) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
+    for (int k = 0; k < nprob; ++k)
+        if (offsets[k + 1] < offsets[k]) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
     const int N = offsets[nprob];
-    if (N < 0 || offsets[0] != 0) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
     if (N > 0 && (!unpx || !wpts || !outlier_flags)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: null array");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;

@@ -4,8 +4,9 @@
 // MultiViewGeometry (P3P / 5-point RANSAC, triangulation) stays in the reference's own translation unit built with
 // -DOV2_EXTERNAL_CERESPNP (one #ifndef around the two bodies, INTEGRATION.md).
 //
-// Same arguments, same return value (false when more than half of the blocks were rejected / nothing left, Twc untouched
-// then), voutliersidx filled with the rejected residual blocks.  The 5 ms wall-clock cap of the reference (:545-546) is not
+// Same arguments, same return value (false when every block was rejected, Twc untouched then, or when the solve was not
+// usable; false for an empty input), voutliersidx filled with the rejected residual blocks.  voutliersidx is cleared first,
+// where the reference appends to it: both callers pass an empty vector, so the results are the same.  The 5 ms wall-clock cap of the reference (:545-546) is not
 // modelled (the device solve takes tens of microseconds).  No CPU fallback: without a device the call reports and
 // returns false (the caller then keeps the P3P / motion-model pose, exactly as after a failed Ceres solve).
 #include <cstdio>

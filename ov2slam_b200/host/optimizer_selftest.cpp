@@ -9,12 +9,21 @@
 //             i32 lm_anchor_cam[npts]; f64 lm_anchor_px[npts][2]; f64 lm_invdepth[npts]; i32 obs_cam[nobs]; i32 obs_lm[nobs];
 //             f64 obs_px[nobs][2]; u8 obs_type[nobs]
 // result.bin: f64 pose[ncam][7]; f64 invdepth[npts] (-1: map point removed); i32 n_removed_obs
+//
+//   optimizer_selftest pnp problem.bin result.bin
+// Calls both MultiViewGeometry::ceresPnP overloads (host/multi_view_geometry_pnp_gpu.cpp), the way VisualFrontEnd::computePose
+// and LoopCloser call them, on one pose problem.
+// problem.bin: i32 n, nmaxiter, use_robust, apply_l2; f32 chi2th, fx, fy, cx, cy; f64 Twc[7] (t, q xyzw); f64 unpx[n][2];
+//              f64 wpts[n][3]; i32 scales[n]
+// result.bin:  per overload (first with the scales, then the scale-less one): i32 return value; f64 Twc[7] as the call left it;
+//              i32 nout; i32 voutliersidx[nout]
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
 
+#include "multi_view_geometry.hpp"
 #include "optimizer.hpp"
 
 void Optimizer::signalStopLocalBA() { bstop_localba_ = true; }      // the reference's optimizer.cpp:2334-2343
@@ -22,8 +31,47 @@ bool Optimizer::stopLocalBA() { return bstop_localba_; }
 
 template <typename T> static bool rd(FILE* f, std::vector<T>& v, size_t n) { v.resize(n); return n == 0 || fread(v.data(), sizeof(T), n, f) == n; }
 
+static int pnp_main(const char* in, const char* outp) {
+    FILE* f = fopen(in, "rb");
+    if (!f) return 3;
+    int32_t hd[4];
+    float fl[5];
+    std::vector<double> T, px, wp;
+    std::vector<int32_t> sc;
+    if (fread(hd, 4, 4, f) != 4 || fread(fl, 4, 5, f) != 5) return 3;
+    const size_t n = (size_t)hd[0];
+    if (!rd(f, T, 7) || !rd(f, px, 2 * n) || !rd(f, wp, 3 * n) || !rd(f, sc, n)) return 3;
+    fclose(f);
+    std::vector<Eigen::Vector2d, Eigen::aligned_allocator<Eigen::Vector2d> > vunkps;
+    std::vector<Eigen::Vector3d, Eigen::aligned_allocator<Eigen::Vector3d> > vwpts;
+    for (size_t i = 0; i < n; ++i) {
+        vunkps.emplace_back(px[2 * i], px[2 * i + 1]);
+        vwpts.emplace_back(wp[3 * i], wp[3 * i + 1], wp[3 * i + 2]);
+    }
+    const std::vector<int> vscales(sc.begin(), sc.end());
+    f = fopen(outp, "wb");
+    if (!f) return 3;
+    for (int overload = 0; overload < 2; ++overload) {
+        Sophus::SE3d Twc(Eigen::Quaterniond(T[6], T[3], T[4], T[5]), Eigen::Vector3d(T[0], T[1], T[2]));
+        std::vector<int> vout;
+        const bool ok = overload == 0
+            ? MultiViewGeometry::ceresPnP(vunkps, vwpts, vscales, Twc, hd[1], fl[0], hd[2] != 0, hd[3] != 0, fl[1], fl[2], fl[3], fl[4], vout)
+            : MultiViewGeometry::ceresPnP(vunkps, vwpts, Twc, hd[1], fl[0], hd[2] != 0, hd[3] != 0, fl[1], fl[2], fl[3], fl[4], vout);
+        const int32_t r = ok ? 1 : 0, nout = (int32_t)vout.size();
+        const Eigen::Quaterniond& q = Twc.unit_quaternion();
+        const double p[7] = {Twc.translation().x(), Twc.translation().y(), Twc.translation().z(), q.x(), q.y(), q.z(), q.w()};
+        fwrite(&r, 4, 1, f);
+        fwrite(p, sizeof(double), 7, f);
+        fwrite(&nout, 4, 1, f);
+        for (int i : vout) { const int32_t v = i; fwrite(&v, 4, 1, f); }
+    }
+    fclose(f);
+    return 0;
+}
+
 int main(int argc, char** argv) {
-    if (argc < 3) { fprintf(stderr, "usage: optimizer_selftest window.bin result.bin [stop]\n"); return 2; }
+    if (argc == 4 && std::string(argv[1]) == "pnp") return pnp_main(argv[2], argv[3]);
+    if (argc < 3) { fprintf(stderr, "usage: optimizer_selftest window.bin result.bin [stop]\n       optimizer_selftest pnp problem.bin result.bin\n"); return 2; }
     FILE* f = fopen(argv[1], "rb");
     if (!f) return 3;
     int32_t hd[4];

@@ -279,7 +279,7 @@ extern "C" int pnp_host(int n, const double* unpx, const double* wpts, const dou
         px = np.ascontiguousarray(px)
         start = ba_ref.pose_plus(pose, np.concatenate([rng.standard_normal(3) * 0.05, rng.standard_normal(3) * 0.02]))
         for apply_l2 in (1, 0):
-            ok_r, est_r, out_r = pnp_ref.ceres_pnp(px, wpts, start, K, 5, 5.9915, True, bool(apply_l2))
+            ok_r, est_r, out_r, info = pnp_ref.ceres_pnp(px, wpts, start, K, 5, 5.9915, True, bool(apply_l2), summary=True)
             est = start.copy()
             flags = np.zeros(n, np.uint8)
             its = ctypes.c_int()
@@ -288,6 +288,7 @@ extern "C" int pnp_host(int n, const double* unpx, const double* wpts, const dou
             assert bool(ok) == ok_r, case
             assert np.array_equal(np.nonzero(flags)[0], out_r), case
             assert np.abs(est - est_r).max() <= 1e-9, (case, np.abs(est - est_r).max())
+            assert its.value == info["summary"]["iterations"], (case, its.value, info["summary"]["iterations"])
 
 
 def test_device_lm_controller_replays_the_oracle_decisions(tmp_path):

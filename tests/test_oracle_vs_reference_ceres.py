@@ -15,6 +15,7 @@ import pytest
 from oracle import ba_ref as B
 from oracle.ref_build import build_ceres_ref
 from ov2slam_b200 import synth
+import pnp_scenes as PS
 from reference_golden import ReferenceOutputs
 
 D, I, U = C.POINTER(C.c_double), C.POINTER(C.c_int32), C.POINTER(C.c_uint8)
@@ -292,3 +293,78 @@ extern "C" int pnp_host(int n, const double* unpx, const double* wpts, const int
             assert np.abs(Tc - Th).max() <= 1e-9
             nbad_total += int(oc.sum())
     assert nbad_total > 100
+
+
+# Ceres' Summary::iterations counts iteration 0 and every iteration that reached the check at the top of the loop; a solve that a
+# tolerance or invalid steps end inside an iteration returns before recording it (trust_region_minimizer.cc).  The oracle counts
+# every iteration it started, as the kernel's iterations_out does.
+_RECORDED = {"max_iterations": 1, "gradient": 1, "radius": 1, "parameter": 0, "function": 0, "invalid": 0}
+
+# (name, pnp_scenes.make arguments, ceresPnP options, what the case is about)
+PNP_EDGES = [
+    ("calm", dict(n=150), {}, None),
+    ("outliers", dict(n=300, nout=40, scales=True), {}, lambda r: len(r[2]) >= 20 and len(r[3]["solves"]) == 2),
+    ("n1", dict(n=1), {}, None),
+    ("n2", dict(n=2), {}, None),
+    ("n3", dict(n=3), {}, None),
+    ("n4", dict(n=4), {}, None),
+    ("n6", dict(n=6, nout=1), {}, None),
+    ("scales", dict(n=200, scales=True, nout=20), {}, lambda r: len(r[3]["solves"]) == 2),
+    ("level3", dict(n=120, scales=3), {}, None),
+    ("trivial_l2", dict(n=200, nout=20), dict(use_robust=False, apply_l2=True), lambda r: len(r[3]["solves"]) == 2),
+    ("trivial_no_l2", dict(n=200, nout=20), dict(use_robust=False, apply_l2=False), None),
+    ("iters0", dict(n=100), dict(nmaxiter=0, apply_l2=False), lambda r: r[3]["summary"]["iterations"] == 0),
+    ("iters1", dict(n=100), dict(nmaxiter=1, apply_l2=False), lambda r: r[3]["summary"]["stop"] == "max_iterations"),
+    ("iters10", dict(n=100, nout=10), dict(nmaxiter=10, apply_l2=False), None),
+    ("chi2_20", dict(n=200, nout=20), dict(chi2th=3.2189), None),
+    ("chi2_1", dict(n=200, nout=20), dict(chi2th=9.2103), None),
+    ("behind", dict(n=100, behind=12), {}, lambda r: len(r[2]) >= 12),
+    ("all_behind", dict(n=40, behind=40), {}, lambda r: not r[0] and len(r[2]) == 40),
+    ("optimum", dict(n=8, scales=3, start="optimum"), {}, lambda r: r[3]["summary"]["iterations"] == 0),
+    ("kitti", dict(n=200, calib="kitti_00-02", far=True, nout=20), {}, None),
+    ("wneg", dict(n=100, quat="wneg"), {}, None),
+]
+
+
+def _ceres_pnp_live(lib, sc, nmaxiter=5, chi2th=5.9915, use_robust=True, apply_l2=True):
+    T = PS.unit_start(sc)
+    out, summ = np.zeros(sc["n"], np.uint8), np.zeros((2, 8))
+    scales = sc["scales"]
+    rc = lib.ov2ref_ceres_pnp(sc["n"], sc["px"].ctypes.data_as(D), sc["w"].ctypes.data_as(D), None if scales is None else scales.ctypes.data_as(I),
+                              T.ctypes.data_as(D), int(nmaxiter), C.c_double(chi2th), int(use_robust), int(apply_l2), sc["K"].ctypes.data_as(D),
+                              out.ctypes.data_as(U), summ.ctypes.data_as(D))
+    return dict(rc=rc, T=T, out=out, summ=summ)
+
+
+@pytest.fixture(scope="module")
+def pnp_lib():
+    so = build_ceres_ref.build()
+    lib = None
+    if so is not None:
+        lib = C.CDLL(str(so))
+        lib.ov2ref_ceres_pnp.restype = C.c_int
+    rec = ReferenceOutputs("pnp", lib)
+    yield rec
+    rec.save()
+
+
+@pytest.mark.parametrize("case", [c[0] for c in PNP_EDGES])
+def test_ceres_pnp_edges_and_iterations_equal_real_ceres(pnp_lib, case):
+    """oracle/pnp_ref.py::ceres_pnp against the real Ceres on the edges of ceresPnP: 3 to 6 points, pyramid levels 0 to 3, the
+    trivial loss with and without the L2 pass, 0, 1 and 10 iterations (the loop closer's 10 without L2), the shipped 20 % and 1 %
+    chi2 thresholds, points behind the camera (some and all), a start at the optimum (0 iterations), KITTI-scale geometry and a
+    quaternion with w < 0.  Same verdict, outliers, pose to 1e-9, termination, costs and iteration count of every solve."""
+    _, kw, opts, keep = next(c for c in PNP_EDGES if c[0] == case)
+    sc, (ok, pose, outliers, info), _ = PS.draw(7000 + [c[0] for c in PNP_EDGES].index(case), keep=keep, opts=opts, **kw)
+    r = pnp_lib(f"pnp_{case}", lambda lib: _ceres_pnp_live(lib, sc, **opts))
+    rc, T, out, summ = int(r["rc"]), r["T"], r["out"], r["summ"]
+    assert np.array_equal(np.nonzero(out)[0], outliers)
+    if rc == -1:                                                   # every block rejected: false, Twc not written back
+        assert not ok and len(outliers) == sc["n"] and np.array_equal(T, PS.unit_start(sc))
+    else:
+        assert bool(rc) == ok and np.abs(T - pose).max() <= 1e-9, np.abs(T - pose).max()
+    assert len(info["solves"]) == (2 if summ[1][5] > 0 else 1)
+    for s, o in zip(summ, info["solves"]):
+        assert TERM[int(s[2])] == o["termination"]
+        assert int(s[5]) == o["iterations"] + _RECORDED[o["stop"]], (int(s[5]), o["iterations"], o["stop"])
+        assert rel(s[0], o["initial_cost"]) and rel(s[1], o["final_cost"])
