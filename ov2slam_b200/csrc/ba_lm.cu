@@ -112,6 +112,7 @@ __device__ __forceinline__ double warp_sum(double v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
     return v;
 }
+__device__ __forceinline__ int warp_sum(int v) { return __reduce_add_sync(FULL, v); }
 __device__ __forceinline__ double warp_max(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(FULL, v, o));
@@ -147,6 +148,16 @@ __device__ __forceinline__ unsigned long long global_ns() {
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
     return t;
 }
+// OV2_BA_TRACE phase timer, run by one thread: mark(trace, k) charges the time since the previous mark to trace slot k
+struct PhaseTimer {
+    bool on;
+    unsigned long long last;
+    __device__ __forceinline__ explicit PhaseTimer(bool on_) : on(on_), last(on_ ? global_ns() : 0) {}
+    __device__ __forceinline__ void mark(unsigned long long* trace, int k) {
+        if (on) { const unsigned long long t = global_ns(); trace[k] += t - last; last = t; }
+    }
+};
+
 constexpr unsigned long long BARRIER_TIMEOUT_NS = 30000000000ull;   // 30 s: a CTA that never arrives (includes waiting for CTA 0 inside a rank exchange)
 constexpr unsigned long long XSYNC_TIMEOUT_NS = 20000000000ull;     // 20 s: a peer rank that never arrives
 
@@ -179,15 +190,16 @@ struct GroupBar {
 // ------------------------------------------------------------------ keyframe staging
 // Rwc (9) + twc (3) of every keyframe of the window in the CTA's keyframe table: one normalisation + quaternion-to-rotation
 // per keyframe and CTA instead of two per residual block.
-__device__ __forceinline__ void stage_cams(const Prob& P, const double* __restrict__ pose, double* s_cam) {
-    for (int c = threadIdx.x; c < P.ncam; c += blockDim.x) {
-        double t[3], q[4], R[9];
-        load_pose(pose + 7 * c, t, q);
-        quat_to_rot(q, R);
+__device__ __forceinline__ void cam_entry(const double* pose, double* e) {
+    double t[3], q[4], R[9];
+    load_pose(pose, t, q);
+    quat_to_rot(q, R);
 #pragma unroll
-        for (int k = 0; k < 9; ++k) s_cam[12 * c + k] = R[k];
-        s_cam[12 * c + 9] = t[0]; s_cam[12 * c + 10] = t[1]; s_cam[12 * c + 11] = t[2];
-    }
+    for (int k = 0; k < 9; ++k) e[k] = R[k];
+    e[9] = t[0]; e[10] = t[1]; e[11] = t[2];
+}
+__device__ __forceinline__ void stage_cams(const Prob& P, const double* __restrict__ pose, double* s_cam) {
+    for (int c = threadIdx.x; c < P.ncam; c += blockDim.x) cam_entry(pose + 7 * c, s_cam + 12 * c);
 }
 
 // ------------------------------------------------------------------ residual blocks
@@ -287,6 +299,41 @@ __device__ __forceinline__ void red_add_f64(double* p, double v) {
     asm volatile("red.global.add.f64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "d"(v) : "memory");
 }
 
+// dst[j] += the CTA's sum of v[j], j < K: warp sums into the per-warp slots s_red, thread j adds the warps up in warp order
+// and sends one RED per CTA (the CTAs of a group all hit the same addresses), none for a zero sum
+template <int K, class T>
+__device__ __forceinline__ void cta_red_add(const T (&v)[K], double (*s_red)[4], double* dst) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    T s[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) s[j] = warp_sum(v[j]);
+    if (lane == 0)
+#pragma unroll
+        for (int j = 0; j < K; ++j) s_red[warp][j] = (double)s[j];
+    __syncthreads();
+    if (tid < K) {
+        double a = 0.0;
+        for (int w = 0; w < WARPS; ++w) a += s_red[w][tid];
+        if (a != 0.0) red_add_f64(dst + tid, a);
+    }
+}
+
+// LevenbergMarquardtStrategy (levenberg_marquardt_strategy.cc:66-160) with Jacobian scaling: column scale
+// sc = 1 / (1 + sqrt(column norm)), fixed at the first iteration of a solve (`writer` stores it), and the damping term
+// clamp(cn sc^2, 1e-6, 1e32) / (radius sc^2) added to the diagonal of the unscaled normal equations
+__device__ __forceinline__ double lm_scale(double* stored, double cn, int first_iter, bool writer) {
+    double sc = *stored;
+    if (first_iter) {
+        sc = 1.0 / (1.0 + sqrt(cn));
+        if (writer) *stored = sc;
+    }
+    return sc;
+}
+__device__ __forceinline__ double lm_damping(double cn, double sc, double radius) {
+    const double diag = fmin(fmax(cn * sc * sc, 1e-6), 1e32);
+    return diag / (radius * sc * sc);
+}
+
 // schur_eliminator_impl.h:179-308 for a scalar e-block: E'E, E'r, F'F, F'r, E'F per touching keyframe, then
 // S -= (E'F)' (E'E)^-1 (E'F), rhs -= (E'F)' (E'E)^-1 E'r.  The anchor keyframe's F'F / F'r / column norms are summed
 // over the landmark's observations in registers and leave the warp once.
@@ -321,13 +368,8 @@ __device__ __forceinline__ void schur_landmark(const Prob& P, const int* __restr
         if (lane == 0) { P.ete[l] = 0.0; P.ge[l] = 0.0; }
         return;
     }
-    double sc = P.sc_lm[l];
-    if (first_iter) {
-        sc = 1.0 / (1.0 + sqrt(cnl));
-        if (lane == 0) P.sc_lm[l] = sc;
-    }
-    const double diag = fmin(fmax(cnl * sc * sc, 1e-6), 1e32);
-    const double ete = cnl + diag / (radius * sc * sc);
+    const double sc = lm_scale(P.sc_lm + l, cnl, first_iter, lane == 0);
+    const double ete = cnl + lm_damping(cnl, sc, radius);
     const double inv_ete = 1.0 / ete;
     if (lane == 0) {
         P.ete[l] = ete;
@@ -545,13 +587,8 @@ __device__ __forceinline__ void owner_fill_row(const Prob& P, const int* __restr
         if (sl == 0) { P.ete[l] = 0.0; P.ge[l] = 0.0; }
         return;
     }
-    double sc = P.sc_lm[l];
-    if (first_iter) {
-        sc = 1.0 / (1.0 + sqrt(cnl));
-        if (sl == 0) P.sc_lm[l] = sc;
-    }
-    const double diag = fmin(fmax(cnl * sc * sc, 1e-6), 1e32);
-    const double ete = cnl + diag / (radius * sc * sc);
+    const double sc = lm_scale(P.sc_lm + l, cnl, first_iter, sl == 0);
+    const double ete = cnl + lm_damping(cnl, sc, radius);
     if (sl == 0) {
         P.ete[l] = ete;
         P.ge[l] = ge;
@@ -572,8 +609,7 @@ __device__ __noinline__ void schur_owner_phase(const Prob& P, const int* __restr
     const int gwarps = G * WARPS, gwarp = bid * WARPS + warp;
     double* const cRhs = P.acc; double* const cG = P.acc + n; double* const cCn = P.acc + 2 * n; double* const cS = P.acc + 3 * n;
     // ---------------- B1: camera part, one pair chunk per warp
-    const bool tracing = P.trace != nullptr && bid == 0 && tid == 0;
-    const unsigned long long t_b1 = tracing ? global_ns() : 0;
+    PhaseTimer tm(P.trace != nullptr && bid == 0 && tid == 0);
     {
         double* st = s_tile + (size_t)warp * (PCH * 26);
         int ia0[3], ja0[3], ja1[3], ei[3], ej[3];
@@ -671,7 +707,7 @@ __device__ __noinline__ void schur_owner_phase(const Prob& P, const int* __restr
         }
     }
     __syncthreads();
-    if (tracing) P.trace[15] += global_ns() - t_b1;                 // trace slot 15 = B1 share of B:schur in this mode
+    tm.mark(P.trace, 15);                                           // trace slot 15 = B1 share of B:schur in this mode
     // ---------------- B2: landmark part
     // S -= sum_rows w y y' is the one contraction of this phase: FP64 tensor cores (DMMA m8n8k4), a warp owns up to NT 8 x 8
     // tiles of the upper triangle and keeps their accumulators in registers over ALL rounds; per 4-row step and tile two
@@ -787,9 +823,7 @@ __device__ __forceinline__ void gj_pivots(double* sA, int n, int PIT, int* s_fai
 __device__ void reduced_solve_small(const Prob& P, double* T, int n, double radius, int first_iter, double* sA, double* scal) {
     const int tid = threadIdx.x, nt = blockDim.x;
     const int PIT = n + 2;
-    const bool tr = P.trace != nullptr && tid == 0;          // (CTA 0 only runs this) trace slots 12: load + damping, 13: pivots, 14: solution
-    unsigned long long tr_t = tr ? global_ns() : 0;
-#define TRS(k) do { if (tr) { const unsigned long long t_ = global_ns(); P.trace[k] += t_ - tr_t; tr_t = t_; } } while (0)
+    PhaseTimer tm(P.trace != nullptr && tid == 0);              // (CTA 0 only runs this) trace slots 12: load + damping, 13: pivots, 14: solution
     double* cRhs = T; double* cG = T + n; double* cCn = T + 2 * n; double* cS = T + 3 * n;
     __shared__ int s_fail;
     if (tid == 0) s_fail = 0;
@@ -800,35 +834,27 @@ __device__ void reduced_solve_small(const Prob& P, double* T, int n, double radi
     __syncthreads();
     for (int i = tid; i < n; i += nt) {
         const double cn = cCn[i];
-        double sc = P.sc_cam[i];
-        if (first_iter) {
-            sc = 1.0 / (1.0 + sqrt(cn));
-            P.sc_cam[i] = sc;
-        }
-        const double diag = fmin(fmax(cn * sc * sc, 1e-6), 1e32);
-        sA[i * PIT + i] += diag / (radius * sc * sc);
+        const double sc = lm_scale(P.sc_cam + i, cn, first_iter, true);
+        sA[i * PIT + i] += lm_damping(cn, sc, radius);
         sA[i * PIT + n] = cG[i] + cRhs[i];
     }
     __syncthreads();
-    TRS(12);
+    tm.mark(P.trace, 12);
     if (n <= 48) gj_pivots<13>(sA, n, PIT, &s_fail);         // (n + 1 + 3) / 4 columns per thread
     else if (n <= 64) gj_pivots<17>(sA, n, PIT, &s_fail);
     else gj_pivots<25>(sA, n, PIT, &s_fail);
     __syncthreads();
-    TRS(13);
+    tm.mark(P.trace, 13);
     if (s_fail) {
         if (tid == 0) scal[SC_CHOL_FAIL] = 1.0;
         return;
     }
     for (int i = tid; i < n; i += nt) P.z[i] = sA[i * PIT + n] / sA[i * PIT + i];
-    TRS(14);
-#undef TRS
+    tm.mark(P.trace, 14);
 }
 
-// ------------------------------------------------------------------ reduced camera system, n > 96: blocked Cholesky (one CTA)
-
 // ------------------------------------------------------------------ reduced camera system, n > 96: blocked Cholesky across the group
-// Same factorisation as reduced_solve_blocked, but only the sequential part of a block step stays on CTA 0 (diagonal
+// Right-looking blocked Cholesky in blocks of CH_NB.  Only the sequential part of a block step stays on CTA 0 (diagonal
 // block, row panel, forward substitution); the trailing update A22 -= U12' U12 - the one real contraction, (n - c1)^2 x 32
 // flops - is spread over every warp of the group (FP64 tensor cores, operands read from the row panel in L2).  Two group
 // barriers per block step; 9 steps for the 288 x 288 system of a 48-keyframe window.
@@ -846,20 +872,13 @@ __device__ void reduced_solve_blocked_group(const Prob& P, double* T, int n, dou
     double* Pan = P.panel;                               // [CH_NB][PW] in global memory: what the other CTAs read
     const int warp = tid >> 5, lane = tid & 31, nwarp = nt >> 5;
     const int gwarps = G * nwarp, gwarp = bid * nwarp + warp;
-    const bool tr = P.trace != nullptr && bid == 0 && tid == 0;
-    unsigned long long tr_t = tr ? global_ns() : 0;
-#define TRS(k) do { if (tr) { const unsigned long long t_ = global_ns(); P.trace[k] += t_ - tr_t; tr_t = t_; } } while (0)
+    PhaseTimer tm(P.trace != nullptr && bid == 0 && tid == 0);
     if (bid == 0) {
         if (tid == 0) s_bad = 0;
         for (int i = tid; i < n; i += nt) {
             const double cn = cCn[i];
-            double sc = P.sc_cam[i];
-            if (first_iter) {
-                sc = 1.0 / (1.0 + sqrt(cn));
-                P.sc_cam[i] = sc;
-            }
-            const double diag = fmin(fmax(cn * sc * sc, 1e-6), 1e32);
-            A[(size_t)i * n + i] += diag / (radius * sc * sc);
+            const double sc = lm_scale(P.sc_cam + i, cn, first_iter, true);
+            A[(size_t)i * n + i] += lm_damping(cn, sc, radius);
             w[i] = cG[i] + cRhs[i];
         }
         __syncthreads();
@@ -942,9 +961,9 @@ __device__ void reduced_solve_blocked_group(const Prob& P, double* T, int n, dou
                 }
             }
         }
-        TRS(12);
+        tm.mark(P.trace, 12);
         bar.sync();
-        TRS(13);
+        tm.mark(P.trace, 13);
         if (scal[SC_CHOL_FAIL] != 0.0) return;                           // uniform across the group (written before the barrier)
         if (bid == 0) {
             for (int r = tid; r < m; r += nt) {
@@ -982,9 +1001,9 @@ __device__ void reduced_solve_blocked_group(const Prob& P, double* T, int n, dou
                         }
             }
         }
-        TRS(14);
+        tm.mark(P.trace, 14);
         bar.sync();
-        TRS(13);
+        tm.mark(P.trace, 13);
     }
     if (bid != 0) return;
     // ---- backward substitution U z = y, last block first (CTA 0)
@@ -1014,68 +1033,17 @@ __device__ void reduced_solve_blocked_group(const Prob& P, double* T, int n, dou
         __syncthreads();
     }
     for (int i = tid; i < n; i += nt) P.z[i] = w[i];
-    TRS(15);
-#undef TRS
+    tm.mark(P.trace, 15);
 }
 
-// ------------------------------------------------------------------ back-substitution + candidate cost (warp / landmark)
+// ------------------------------------------------------------------ back-substitution + candidate cost (SG lanes / landmark)
 // schur_eliminator_impl.h:311-377: y_e = (E'E)^-1 (E'r - sum_k (E'F_k) z_k); model cost change
 // -(J delta)'(r + J delta / 2) (trust_region_minimizer.cc:424-427); candidate inverse depth; then the residual blocks of
 // the landmark at the candidate point (cost only).
-__device__ __forceinline__ void backsub_landmark(const Prob& P, const int* __restrict__ s_slot, const double* __restrict__ s_cam,
-                                                 int l, int lane, const double* __restrict__ invd, double* __restrict__ cand_invd,
-                                                 int use_huber, double& mcc_out, double& st2_out, double& cx2_out, double& cost_out) {
-    const double ete = P.ete[l];
-    if (ete == 0.0) return;   // landmark not in the program: candidate stays equal
-    const int p0 = P.lm_ptr[l], p1 = P.lm_ptr[l + 1];
-    const int sa = s_slot[P.lm_anchor_cam[l]];
-    double za[6] = {0, 0, 0, 0, 0, 0};
-    if (sa >= 0)
-        for (int k = 0; k < 6; ++k) za[k] = P.z[6 * sa + k];
-    double acc = 0.0;
-    for (int p = p0 + lane; p < p1; p += 32) {
-        if (!P.active[p]) continue;
-        const int so = (P.obs_type && P.obs_type[p] == 2) ? -1 : s_slot[P.obs_cam[p]];
-        const double* Ja = P.Ja + 12 * (size_t)p;
-        const double* Jo = P.Jo + 12 * (size_t)p;
-        double f0 = 0.0, f1 = 0.0;
-        if (sa >= 0)
-            for (int k = 0; k < 6; ++k) { f0 += Ja[k] * za[k]; f1 += Ja[6 + k] * za[k]; }
-        if (so >= 0)
-            for (int k = 0; k < 6; ++k) { const double zk = P.z[6 * so + k]; f0 += Jo[k] * zk; f1 += Jo[6 + k] * zk; }
-        acc += P.Jl[2 * (size_t)p] * f0 + P.Jl[2 * (size_t)p + 1] * f1;
-    }
-    acc = warp_sum(acc);
-    const double y = (P.ge[l] - acc) / ete;
-    const double dl = -y;
-    const double cl = invd[l] + dl;
-    double mcc = 0.0, cost = 0.0;
-    for (int p = p0 + lane; p < p1; p += 32) {
-        if (!P.active[p]) continue;
-        const int so = (P.obs_type && P.obs_type[p] == 2) ? -1 : s_slot[P.obs_cam[p]];
-        const double* Ja = P.Ja + 12 * (size_t)p;
-        const double* Jo = P.Jo + 12 * (size_t)p;
-        double f0 = P.Jl[2 * (size_t)p] * dl, f1 = P.Jl[2 * (size_t)p + 1] * dl;
-        if (sa >= 0)
-            for (int k = 0; k < 6; ++k) { f0 -= Ja[k] * za[k]; f1 -= Ja[6 + k] * za[k]; }
-        if (so >= 0)
-            for (int k = 0; k < 6; ++k) { const double zk = P.z[6 * so + k]; f0 -= Jo[k] * zk; f1 -= Jo[6 + k] * zk; }
-        mcc -= f0 * (P.Jr[2 * (size_t)p] + 0.5 * f0) + f1 * (P.Jr[2 * (size_t)p + 1] + 0.5 * f1);
-        cost += eval_block<false>(P, p, l, s_cam, cl, use_huber);
-    }
-    if (lane == 0) {
-        cand_invd[l] = cl;
-        st2_out += dl * dl;
-        cx2_out += cl * cl;
-    }
-    mcc_out += mcc;
-    cost_out += cost;
-}
-
-// Sub-group variant: SG lanes per landmark, 32 / SG landmarks per warp in flight.  A landmark has ~4 (C3) to ~8 (C5)
-// observations, so one warp per landmark leaves most lanes idle and - worse - strings the landmarks' dependent load chains
-// (CSR pointers -> Jacobian rows -> reduction -> second pass) one after the other: measured 3.9 ms of a 11.9 ms batched C3
-// solve.  Same arithmetic per observation; the per-landmark sums are formed inside the sub-group.
+// SG lanes per landmark, 32 / SG landmarks per warp in flight (SG = 4 / 8 for windows with few observations per landmark).
+// A landmark has ~4 (C3) to ~8 (C5) observations, so one warp per landmark leaves most lanes idle and - worse - strings the
+// landmarks' dependent load chains (CSR pointers -> Jacobian rows -> reduction -> second pass) one after the other:
+// measured 3.9 ms of a 11.9 ms batched C3 solve.  The per-landmark sums are formed inside the sub-group.
 template <int SG>
 __device__ __forceinline__ void backsub_landmarks_sg(const Prob& P, const int* __restrict__ s_slot, const double* __restrict__ s_cam,
                                                      int l0, int lane, const double* __restrict__ invd, double* __restrict__ cand_invd,
@@ -1163,6 +1131,22 @@ __device__ __forceinline__ double ld_peer(const double* p) {
     return v;
 }
 
+// rank r's part of the exchange buffer from byte offset `off` (an XB_* offset) on, as mapped in this process
+template <class T>
+__device__ __forceinline__ T* xslice(const Peers& X, int r, size_t off) {
+    return reinterpret_cast<T*>(static_cast<unsigned char*>(X.base[r]) + off);
+}
+
+// One exchange between the ranks: `publish` writes this rank's slice, then group barrier, xsync on CTA 0 / thread 0, group
+// barrier.  Afterwards every rank's slice is readable.  Every rank's kernel runs the same sequence of exchanges.
+template <class F>
+__device__ __forceinline__ void rank_exchange(const Peers& X, GroupBar& bar, int bid, unsigned long long& xepoch, F publish) {
+    publish();
+    bar.sync();
+    if (bid == 0 && threadIdx.x == 0) xsync(X, xepoch, bar.abort);
+    bar.sync();
+}
+
 // ------------------------------------------------------------------ the persistent solve kernel
 struct SolveOut { int iterations; double initial_cost, final_cost; int termination; };
 
@@ -1183,11 +1167,10 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
         __syncthreads();
         const Prob& P = sProb;
         GroupBar bar{P.bar, P.bar + 1, (unsigned)G, 0u};
-        // optional phase trace (CTA 0 / thread 0): time since the previous mark is charged to phase k
-        unsigned long long tr_last = 0, tr_acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-        const bool tracing = P.trace != nullptr && bid == 0 && tid == 0;
-        if (tracing) tr_last = global_ns();
-#define TR(k) do { if (tracing) { const unsigned long long t_ = global_ns(); tr_acc[k] += t_ - tr_last; tr_last = t_; } } while (0)
+        // trace slots 0-11 (the kernel's phases) add up in tr_acc and are stored at the end: a read-modify-write of the global
+        // trace per mark costs the kernel registers
+        unsigned long long tr_acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        PhaseTimer tm(P.trace != nullptr && bid == 0 && tid == 0);
         // keyframe table [ncam][12] + [ncam] slots: in shared memory, or (windows too large for it) this CTA's copy in
         // global memory; either way only this CTA reads and writes it
         double* s_cam = P.cam_tab ? P.cam_tab + (size_t)bid * P.cam_tab_stride : reinterpret_cast<double*>(smem_raw);
@@ -1231,20 +1214,19 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
             for (int i = gtid; i < P.npts; i += gthreads) c_invd[i] = x_invd[i];
             for (size_t i = gtid; i < blk; i += gthreads) P.acc[i] = 0.0;
             for (int i = gtid; i < 2 * SC_COUNT; i += gthreads) P.scal[i] = 0.0;
-            TR(stage == 0 ? 0 : 10);
+            tm.mark(tr_acc, stage == 0 ? 0 : 10);
             bar.sync();
-            TR(stage == 0 ? 11 : 10);
+            tm.mark(tr_acc, stage == 0 ? 11 : 10);
             if (X.world > 1) {
                 // a keyframe is in the program if ANY rank has an active residual touching it
-                uint8_t* mine = reinterpret_cast<uint8_t*>(X.base[X.rank]) + XB_CAMUSED + (size_t)stage * MAX_CAMS;
-                for (int i = gtid; i < P.ncam; i += gthreads) mine[i] = cam_used[i];
-                bar.sync();
-                if (bid == 0 && tid == 0) xsync(X, xepoch, P.bar + 1);
-                bar.sync();
+                const size_t xb = XB_CAMUSED + (size_t)stage * MAX_CAMS;
+                rank_exchange(X, bar, bid, xepoch, [&] {
+                    uint8_t* mine = xslice<uint8_t>(X, X.rank, xb);
+                    for (int i = gtid; i < P.ncam; i += gthreads) mine[i] = cam_used[i];
+                });
                 for (int c = tid; c < P.ncam; c += THREADS) {
                     int u = 0;
-                    for (int r = 0; r < X.world; ++r)
-                        u |= *reinterpret_cast<volatile const uint8_t*>(reinterpret_cast<const uint8_t*>(X.base[r]) + XB_CAMUSED + (size_t)stage * MAX_CAMS + c);
+                    for (int r = 0; r < X.world; ++r) u |= xslice<volatile const uint8_t>(X, r, xb)[c];
                     s_slot[c] = (u ? 1 : 0) | (P.pose_const[c] ? 2 : 0);          // temporarily: used / constant flags
                 }
             } else {
@@ -1267,7 +1249,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
             if (bid == 0)
                 for (int c = tid; c < P.ncam; c += THREADS) P.cam_slot[c] = s_slot[c];
             double* T = X.world > 1 ? P.total : P.acc;                       // the system the solve reads
-            TR(0);
+            tm.mark(tr_acc, 0);
             // ---- LM iterations
             for (;;) {
                 if (tid == 0) s_action = lmctl::begin_iteration(S, max_iters) ? 1 : 0;
@@ -1280,20 +1262,13 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                 if (x_is_new) {
                     stage_cams(P, x_pose, s_cam);
                     __syncthreads();
-                    double cost = 0.0;
+                    double cost[1] = {0.0};
                     for (int i = gtid; i < P.nobs; i += gthreads)
-                        if (P.active[i]) cost += eval_block<true>(P, i, P.obs_lm[i], s_cam, x_invd[P.obs_lm[i]], use_huber);
-                    cost = warp_sum(cost);
-                    if (lane == 0) s_red[warp][0] = cost;
-                    __syncthreads();
-                    if (tid == 0) {                               // one atomic per CTA: they all hit one address
-                        double a = 0.0;
-                        for (int w_ = 0; w_ < WARPS; ++w_) a += s_red[w_][0];
-                        if (a != 0.0) red_add_f64(scal + SC_COST, a);
-                    }
+                        if (P.active[i]) cost[0] += eval_block<true>(P, i, P.obs_lm[i], s_cam, x_invd[P.obs_lm[i]], use_huber);
+                    cta_red_add(cost, s_red, scal + SC_COST);
                 }
                 bar.sync();
-                TR(1);
+                tm.mark(tr_acc, 1);
                 // ---- B: Schur elimination into the accumulation block
                 if (P.schur_smem == 3) {
                     // owner mode (n <= 96): pair-sorted Gram blocks + dense landmark rows, no per-observation reductions
@@ -1328,26 +1303,25 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     if (lane == 0 && gmax_lm > 0.0) atomic_max_pos(scal + SC_GMAX_LM, gmax_lm);
                 }
                 bar.sync();
-                TR(2);
+                tm.mark(tr_acc, 2);
                 // ---- B2: multi-GPU: sum the ranks' partial systems out of peer memory
                 const int live = 3 * n + n * n;
                 if (X.world > 1) {
-                    double* mine = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(X.base[X.rank]) + XB_PARTIAL) + (size_t)par * (SC_COUNT + blk);
-                    for (int e = gtid; e < live; e += gthreads) mine[SC_COUNT + e] = P.acc[e];
-                    if (gtid < SC_COUNT) mine[gtid] = scal[gtid];
-                    bar.sync();
-                    if (bid == 0 && tid == 0) xsync(X, xepoch, P.bar + 1);
-                    bar.sync();
+                    const size_t slot = (size_t)par * (SC_COUNT + blk);   // [scalars | partial system] of this parity
+                    rank_exchange(X, bar, bid, xepoch, [&] {
+                        double* mine = xslice<double>(X, X.rank, XB_PARTIAL) + slot;
+                        for (int e = gtid; e < live; e += gthreads) mine[SC_COUNT + e] = P.acc[e];
+                        if (gtid < SC_COUNT) mine[gtid] = scal[gtid];
+                    });
                     for (int e = gtid; e < live; e += gthreads) {
                         double a = 0.0;
-                        for (int r = 0; r < X.world; ++r)
-                            a += ld_peer(reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(X.base[r]) + XB_PARTIAL) + (size_t)par * (SC_COUNT + blk) + SC_COUNT + e);
+                        for (int r = 0; r < X.world; ++r) a += ld_peer(xslice<const double>(X, r, XB_PARTIAL) + slot + SC_COUNT + e);
                         T[e] = a;
                     }
                     if (gtid == 0) {
                         double c = 0.0, g = 0.0;
                         for (int r = 0; r < X.world; ++r) {
-                            const double* pr = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(X.base[r]) + XB_PARTIAL) + (size_t)par * (SC_COUNT + blk);
+                            const double* pr = xslice<const double>(X, r, XB_PARTIAL) + slot;
                             c += ld_peer(pr + SC_COST);
                             g = fmax(g, ld_peer(pr + SC_GMAX_LM));
                         }
@@ -1356,7 +1330,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     }
                     bar.sync();
                 }
-                TR(3);
+                tm.mark(tr_acc, 3);
                 // ---- C: reduced camera system (CTA 0); gradient projection |x - Plus(x, -g)|_inf (last CTA); the other
                 //      CTAs clear the accumulation block for the next iteration once the solve has read it
                 const bool group_solve = P.solve_blocked && n > 0;
@@ -1376,9 +1350,9 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     if (lane == 0) atomic_max_pos(scal + SC_GMAX_CAM, gm);
                 }
                 if (group_solve) reduced_solve_blocked_group(P, T, n, radius, first_iter, s_work, scal, bar, bid, G);
-                TR(4);
+                tm.mark(tr_acc, 4);
                 bar.sync();
-                TR(5);
+                tm.mark(tr_acc, 5);
                 // ---- D: candidate keyframe poses (every CTA, into shared memory), back-substitution, candidate cost
                 {
                     double st2 = 0.0, cx2 = 0.0;
@@ -1398,48 +1372,32 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                         } else {
                             for (int k = 0; k < 7; ++k) out[k] = x_pose[7 * c + k];
                         }
-                        double t[3], q[4], R[9];
-                        load_pose(out, t, q);
-                        quat_to_rot(q, R);
-                        for (int k = 0; k < 9; ++k) s_cam[12 * c + k] = R[k];
-                        s_cam[12 * c + 9] = t[0]; s_cam[12 * c + 10] = t[1]; s_cam[12 * c + 11] = t[2];
+                        cam_entry(out, s_cam + 12 * c);
                     }
                     __syncthreads();
                     double mcc = 0.0, cost = 0.0, lst2 = 0.0, lcx2 = 0.0;
-                    if (P.sg == 4) {
-                        for (int l0 = gwarp * 8; l0 < P.npts; l0 += gwarps * 8)
-                            backsub_landmarks_sg<4>(P, s_slot, s_cam, l0, lane, x_invd, c_invd, use_huber, mcc, lst2, lcx2, cost);
-                    } else if (P.sg == 8) {
-                        for (int l0 = gwarp * 4; l0 < P.npts; l0 += gwarps * 4)
-                            backsub_landmarks_sg<8>(P, s_slot, s_cam, l0, lane, x_invd, c_invd, use_huber, mcc, lst2, lcx2, cost);
-                    } else {
-                        for (int l = gwarp; l < P.npts; l += gwarps)
-                            backsub_landmark(P, s_slot, s_cam, l, lane, x_invd, c_invd, use_huber, mcc, lst2, lcx2, cost);
-                    }
+#define OV2_BACKSUB(SG_) for (int l0 = gwarp * (32 / SG_); l0 < P.npts; l0 += gwarps * (32 / SG_)) \
+                             backsub_landmarks_sg<SG_>(P, s_slot, s_cam, l0, lane, x_invd, c_invd, use_huber, mcc, lst2, lcx2, cost)
+                    if (P.sg == 4) OV2_BACKSUB(4);
+                    else if (P.sg == 8) OV2_BACKSUB(8);
+                    else OV2_BACKSUB(32);
+#undef OV2_BACKSUB
                     // the keyframe part of the norms counts once per window (rank 0, CTA 0)
                     if (bid == 0 && X.rank == 0) { lst2 += st2; lcx2 += cx2; }
-                    mcc = warp_sum(mcc); cost = warp_sum(cost); lst2 = warp_sum(lst2); lcx2 = warp_sum(lcx2);
-                    if (lane == 0) { s_red[warp][0] = cost; s_red[warp][1] = mcc; s_red[warp][2] = lst2; s_red[warp][3] = lcx2; }
-                    __syncthreads();
-                    if (tid < 4) {
-                        double a = 0.0;
-                        for (int w_ = 0; w_ < WARPS; ++w_) a += s_red[w_][tid];
-                        if (a != 0.0) red_add_f64(scal + SC_CAND_COST + tid, a);
-                    }
+                    const double sums[4] = {cost, mcc, lst2, lcx2};   // SC_CAND_COST, SC_MCC, SC_STEP2, SC_CANDX2
+                    cta_red_add(sums, s_red, scal + SC_CAND_COST);
                     // clear for the next iteration: accumulation block and the other parity's scalars
                     for (size_t i = gtid; i < blk; i += gthreads) P.acc[i] = 0.0;
                     double* oscal = P.scal + (par ^ 1) * SC_COUNT;
                     if (gtid < SC_COUNT) oscal[gtid] = 0.0;
                 }
                 bar.sync();
-                TR(6);
+                tm.mark(tr_acc, 6);
                 if (X.world > 1) {
                     // second, tiny exchange: candidate cost, model cost change, step / candidate norms (rank order sum)
-                    double* mine = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(X.base[X.rank]) + XB_SC4) + par * 8;
-                    if (gtid < 4) mine[gtid] = scal[SC_CAND_COST + gtid];
-                    bar.sync();
-                    if (bid == 0 && tid == 0) xsync(X, xepoch, P.bar + 1);
-                    bar.sync();
+                    rank_exchange(X, bar, bid, xepoch, [&] {
+                        if (gtid < 4) xslice<double>(X, X.rank, XB_SC4)[par * 8 + gtid] = scal[SC_CAND_COST + gtid];
+                    });
                 }
                 // ---- E: trust-region controller, replayed by every CTA
                 if (tid == 0) {
@@ -1447,8 +1405,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     if (X.world > 1) {
                         for (int k = 0; k < 4; ++k) {
                             double a = 0.0;
-                            for (int r = 0; r < X.world; ++r)
-                                a += ld_peer(reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(X.base[r]) + XB_SC4) + par * 8 + k);
+                            for (int r = 0; r < X.world; ++r) a += ld_peer(xslice<const double>(X, r, XB_SC4) + par * 8 + k);
                             v[k] = a;
                         }
                     } else {
@@ -1459,7 +1416,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                 }
                 __syncthreads();
                 const int action = s_action;
-                TR(7);
+                tm.mark(tr_acc, 7);
                 if (action == lmctl::ACT_CONTINUE_ACCEPTED) {
                     xi ^= 1;
                     x_pose = P.pose[xi]; c_pose = P.pose[xi ^ 1];
@@ -1480,28 +1437,21 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                 double* cnt = P.counts + 4 * stage;
                 const int bit = stage == 0 ? 1 : 2;
                 const int deact = stage == 0 && P.apply_l2;
-                int bad_t = 0, left_t = 0, right_t = 0;
+                int nt[3] = {0, 0, 0};                           // outliers, left-camera and right-camera inliers
                 for (int i = gtid; i < P.nobs; i += gthreads) {
                     if (!P.active[i]) continue;
                     const bool bad = (P.chi2[i] > (double)P.th_f) || !P.dpos[i];
                     if (bad) {
                         P.flags[i] |= (uint8_t)bit;
                         if (deact) P.active[i] = 0;   // problem.RemoveResidualBlock
-                        bad_t++;
+                        nt[0]++;
                     } else {
                         const int typ = P.obs_type ? (int)P.obs_type[i] : 0;
-                        left_t += typ == 0;
-                        right_t += typ == 1;
+                        nt[1] += typ == 0;
+                        nt[2] += typ == 1;
                     }
                 }
-                bad_t = __reduce_add_sync(FULL, bad_t); left_t = __reduce_add_sync(FULL, left_t); right_t = __reduce_add_sync(FULL, right_t);
-                if (lane == 0) { s_red[warp][0] = (double)bad_t; s_red[warp][1] = (double)left_t; s_red[warp][2] = (double)right_t; }
-                __syncthreads();
-                if (tid < 3) {                                   // one atomic per CTA and counter
-                    double a = 0.0;
-                    for (int w_ = 0; w_ < WARPS; ++w_) a += s_red[w_][tid];
-                    if (a != 0.0) red_add_f64(cnt + tid, a);
-                }
+                cta_red_add(nt, s_red, cnt);
                 // the stop request lives in mapped HOST memory: ONE thread of the group reads it (every thread of every CTA
                 // polling it over PCIe cost 7 us per CTA of the group) and publishes it next to the counters
                 if (stage == 0 && bid == 0 && tid == 0)
@@ -1512,14 +1462,12 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
                     n_out1 = (int)nbad;
                     if (X.world > 1) {
                         // every rank must take the same branch: counts summed over the ranks
-                        double* mine = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(X.base[X.rank]) + XB_SC4) + 16;
-                        if (gtid < 3) mine[gtid] = cnt[gtid];
-                        bar.sync();
-                        if (bid == 0 && tid == 0) xsync(X, xepoch, P.bar + 1);
-                        bar.sync();
+                        rank_exchange(X, bar, bid, xepoch, [&] {
+                            if (gtid < 3) xslice<double>(X, X.rank, XB_SC4)[16 + gtid] = cnt[gtid];
+                        });
                         nbad = nleft = nright = 0.0;
                         for (int r = 0; r < X.world; ++r) {
-                            const double* pr = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(X.base[r]) + XB_SC4) + 16;
+                            const double* pr = xslice<const double>(X, r, XB_SC4) + 16;
                             nbad += ld_peer(pr); nleft += ld_peer(pr + 1); nright += ld_peer(pr + 2);
                         }
                     }
@@ -1540,7 +1488,7 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
             }
         }
         // ---- write-back: x into buffer 0, result record
-        TR(8);
+        tm.mark(tr_acc, 8);
         bar.sync();
         if (xi == 1) {
             for (int i = gtid; i < 7 * P.ncam; i += gthreads) P.pose[0][i] = P.pose[1][i];
@@ -1558,10 +1506,9 @@ __global__ void __launch_bounds__(THREADS, 2) ba_lm_kernel(const Prob* __restric
             R->n_outliers_second = n_out2;
             R->aborted = (int)ld_acquire_gpu(P.bar + 1);
         }
-        TR(9);
-        if (tracing)
+        tm.mark(tr_acc, 9);
+        if (tm.on)
             for (int k = 0; k < 12; ++k) P.trace[k] = tr_acc[k];
-#undef TR
     }
 }
 
@@ -1572,30 +1519,77 @@ using namespace balm;
 
 namespace {
 
+// The memory of one batch in regions, every window's arrays side by side in each.  Device blocks:
+//   upload block [state | input]: one H2D; state first, so one D2H brings the poses and inverse depths of every window back
+//   work block   [work | zero | output | active]: one memset each for zero + output and for active, one D2H of output
+// The pinned host block mirrors [state | input | output].  A window's arrays are taken while it is planned, as offsets
+// inside their region; place() fixes the regions once every window is planned, and d() / h() give the addresses.
+enum Region { RG_STATE, RG_INPUT, RG_WORK, RG_ZERO, RG_OUT, RG_ACT, RG_COUNT };
+
+struct Span { Region rg; size_t off; };
+
+struct Layout {
+    size_t used[RG_COUNT] = {};
+    char* dev[RG_COUNT] = {};
+    char* host[RG_COUNT] = {};   // state, input and output regions only
+
+    Span take(Region rg, size_t bytes, size_t align = 256) {
+        size_t& u = used[rg];
+        u = (u + align - 1) & ~(align - 1);
+        const Span sp{rg, u};
+        u += bytes;
+        return sp;
+    }
+    size_t bytes(Region rg) const { return (used[rg] + 255) & ~(size_t)255; }
+    size_t upload_bytes() const { return bytes(RG_STATE) + bytes(RG_INPUT); }
+    size_t work_bytes() const { return bytes(RG_WORK) + bytes(RG_ZERO) + bytes(RG_OUT) + bytes(RG_ACT); }
+    void place(char* upload, char* work, char* pinned) {
+        dev[RG_STATE] = upload;
+        dev[RG_INPUT] = upload + bytes(RG_STATE);
+        dev[RG_WORK] = work;
+        for (int r = RG_ZERO; r < RG_COUNT; ++r) dev[r] = dev[r - 1] + bytes((Region)(r - 1));
+        host[RG_STATE] = pinned;
+        host[RG_INPUT] = pinned + bytes(RG_STATE);
+        host[RG_OUT] = pinned + upload_bytes();
+    }
+    char* d(Span sp) const { return dev[sp.rg] + sp.off; }
+    char* h(Span sp) const { return host[sp.rg] + sp.off; }
+};
+
 struct HostPlan {
-    size_t off_prob, off_pose, off_invd, off_apx, off_opx, off_lac, off_oc, off_ol, off_lp, off_pc, off_ty, in_bytes;   // uploaded block
-    size_t off_pp, off_pch; int pch_cap, sg;   // owner mode: pair-sorted permutation, chunk table (capacity), lanes per landmark
-    // device-only work areas (offsets into the work block)
-    size_t w_pose1, w_invd1, w_active, w_flags, w_camused, w_camslot, w_Jr, w_Ja, w_Jo, w_Jl, w_chi2, w_dpos, w_sclm, w_ete, w_ge,
-           w_acc, w_total, w_scal, w_z, w_panel, w_sccam, w_counts, w_bar, w_result, w_trace, w_camtab, work_bytes, zero_off, zero_bytes;
-    size_t out_result, out_flags, act_rel;   // offsets inside the batch's output region / 'active' region (set up by balm_solve)
+    Span pose, invd;                                                               // state
+    Span prob, apx, opx, lac, oc, ol, lp, pc, ty, pp, pch;                        // input
+    Span pose1, invd1, camslot, Jr, Ja, Jo, Jl, chi2, dpos, ete, ge, acc, total, scal, z, panel, camtab;   // work
+    Span camused, counts, bar, trace, sclm, sccam;                                // zero
+    Span result, flags;                                                            // output
+    Span active;                                                                   // active
+    int pch_cap, sg;   // owner mode: chunk table capacity (pp: pair-sorted permutation, pch: chunk table); lanes per landmark
     int ncv_max, n_max, solve_blocked, schur_smem;
     bool cam_tab_global;                     // keyframe table in the work block (one copy per CTA), not in shared memory
     size_t blk, tab_bytes, smem_work_off, smem_bytes, smem_sacc_off;
 };
 
-size_t take(size_t& off, size_t bytes, size_t align = 256) {
-    off = (off + align - 1) & ~(align - 1);
-    const size_t o = off;
-    off += bytes;
-    return o;
+// Where a window's arrays live.  A window whose `pose` array is host memory is taken to be host memory throughout (the
+// reference's flow, optimizer.cpp:43-430): cudaPointerGetAttributes costs ~1.5 us on a plain host pointer, and 15 queries
+// per window were 6 ms of a 296-window batch.  Only windows whose poses live on the device are inspected array by array.
+struct Residence {
+    bool window = false;            // `pose` is device memory
+    bool invd = false, flags = false;
+    bool on_device(const void* p) const { return window && p && ov2_is_device_ptr(p); }
+};
+
+// a state array between the caller's memory and the pinned block
+cudaError_t copy_state(void* dst, const void* src, size_t bytes, bool device, cudaMemcpyKind kind) {
+    if (bytes == 0) return cudaSuccess;
+    if (device) return cudaMemcpy(dst, src, bytes, kind);
+    memcpy(dst, src, bytes);
+    return cudaSuccess;
 }
 
 }  // namespace
 
-// Plans one window: offsets of its inputs inside the upload block and of its work areas inside the work block.
-static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world, size_t& st_off, size_t& in_off, size_t& work_off,
-                              size_t& zero_off, size_t& out_off, size_t& act_off, HostPlan& H, bool single_window) {
+// Plans one window: its arrays in the batch's regions, its Schur mode, reduced solver and shared-memory layout.
+static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world, Layout& L, HostPlan& H, bool single_window) {
     const int ncam = pb->ncam, npts = pb->npts, nobs = pb->nobs;
     int ncv = 0;
     for (int c = 0; c < ncam; ++c) ncv += pb->pose_const[c] ? 0 : 1;
@@ -1622,56 +1616,52 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     if (H.blk == 0) H.blk = 1;
     H.solve_blocked = H.n_max > 96 ? 1 : 0;
     // states (pose, inverse depth) of all windows sit together at the head of the block: they are what comes back
-    H.off_pose = take(st_off, sizeof(double) * 7 * ncam, 16);
-    H.off_invd = take(st_off, sizeof(double) * (size_t)(npts > 0 ? npts : 1), 16);
-    H.off_prob = take(in_off, sizeof(Prob));
-    H.off_apx = take(in_off, sizeof(double) * 2 * (size_t)(npts > 0 ? npts : 1));
-    H.off_opx = take(in_off, sizeof(double) * 2 * (size_t)(nobs > 0 ? nobs : 1));
-    H.off_lac = take(in_off, sizeof(int32_t) * (size_t)(npts > 0 ? npts : 1));
-    H.off_oc = take(in_off, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
-    H.off_ol = take(in_off, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
-    H.off_lp = take(in_off, sizeof(int32_t) * (size_t)(npts + 1));
-    H.off_pc = take(in_off, (size_t)ncam);
-    H.off_ty = take(in_off, pb->obs_type ? (size_t)(nobs > 0 ? nobs : 1) : 0);
+    H.pose = L.take(RG_STATE, sizeof(double) * 7 * ncam, 16);
+    H.invd = L.take(RG_STATE, sizeof(double) * (size_t)(npts > 0 ? npts : 1), 16);
+    H.prob = L.take(RG_INPUT, sizeof(Prob));
+    H.apx = L.take(RG_INPUT, sizeof(double) * 2 * (size_t)(npts > 0 ? npts : 1));
+    H.opx = L.take(RG_INPUT, sizeof(double) * 2 * (size_t)(nobs > 0 ? nobs : 1));
+    H.lac = L.take(RG_INPUT, sizeof(int32_t) * (size_t)(npts > 0 ? npts : 1));
+    H.oc = L.take(RG_INPUT, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
+    H.ol = L.take(RG_INPUT, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
+    H.lp = L.take(RG_INPUT, sizeof(int32_t) * (size_t)(npts + 1));
+    H.pc = L.take(RG_INPUT, (size_t)ncam);
+    H.ty = L.take(RG_INPUT, pb->obs_type ? (size_t)(nobs > 0 ? nobs : 1) : 0);
     {
         // owner-mode Schur (n <= 96): observations sorted by (anchor keyframe, observing keyframe) + chunk table
         const size_t ngmax = (size_t)ncam * ncam < (size_t)(nobs > 0 ? nobs : 1) ? (size_t)ncam * ncam : (size_t)(nobs > 0 ? nobs : 1);
         H.pch_cap = (int)((size_t)(nobs > 0 ? nobs : 1) / PCH + ngmax + 1);
-        H.off_pp = take(in_off, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
-        H.off_pch = take(in_off, sizeof(int2) * (size_t)H.pch_cap);
+        H.pp = L.take(RG_INPUT, sizeof(int32_t) * (size_t)(nobs > 0 ? nobs : 1));
+        H.pch = L.take(RG_INPUT, sizeof(int2) * (size_t)H.pch_cap);
         const double avg = npts > 0 ? (double)nobs / (double)npts : 0.0;
         H.sg = avg <= 5.0 ? 4 : (avg <= 12.0 ? 8 : 32);
     }
     const size_t no = nobs > 0 ? nobs : 1, np = npts > 0 ? npts : 1;
-    // results (Result record + outlier flags) of all windows sit together in the output region, the 'active' bytes of all
-    // windows in another: one memset each and ONE D2H for a whole batch (w_flags / w_result / w_active are made absolute
-    // offsets by balm_solve once every window is planned)
-    H.out_result = take(out_off, sizeof(Result), 64);
-    H.out_flags = take(out_off, no, 64);
-    H.act_rel = take(act_off, no, 64);
-    // zero-initialised small arrays of all windows: a region of their own (relative offsets until balm_solve places it)
-    H.w_camused = take(zero_off, 2 * (size_t)ncam);
-    H.w_counts = take(zero_off, sizeof(double) * 8);
-    H.w_bar = take(zero_off, sizeof(unsigned) * 4);
-    H.w_trace = take(zero_off, sizeof(unsigned long long) * 16);
-    H.w_sclm = take(zero_off, sizeof(double) * np);
-    H.w_sccam = take(zero_off, sizeof(double) * MAX_N);
-    H.w_pose1 = take(work_off, sizeof(double) * 7 * ncam);
-    H.w_invd1 = take(work_off, sizeof(double) * np);
-    H.w_camslot = take(work_off, sizeof(int32_t) * ncam);
-    H.w_Jr = take(work_off, sizeof(double) * 2 * no);
-    H.w_Ja = take(work_off, sizeof(double) * 12 * no);
-    H.w_Jo = take(work_off, sizeof(double) * 12 * no);
-    H.w_Jl = take(work_off, sizeof(double) * 2 * no);
-    H.w_chi2 = take(work_off, sizeof(double) * no);
-    H.w_dpos = take(work_off, no);
-    H.w_ete = take(work_off, sizeof(double) * np);
-    H.w_ge = take(work_off, sizeof(double) * np);
-    H.w_acc = take(work_off, sizeof(double) * H.blk);
-    H.w_total = take(work_off, sizeof(double) * H.blk);
-    H.w_scal = take(work_off, sizeof(double) * 2 * SC_COUNT);
-    H.w_z = take(work_off, sizeof(double) * MAX_N);
-    H.w_panel = take(work_off, sizeof(double) * CH_NB * (size_t)(MAX_N + 24));
+    H.result = L.take(RG_OUT, sizeof(Result), 64);
+    H.flags = L.take(RG_OUT, no, 64);
+    H.active = L.take(RG_ACT, no, 64);
+    H.camused = L.take(RG_ZERO, 2 * (size_t)ncam);
+    H.counts = L.take(RG_ZERO, sizeof(double) * 8);
+    H.bar = L.take(RG_ZERO, sizeof(unsigned) * 4);
+    H.trace = L.take(RG_ZERO, sizeof(unsigned long long) * 16);
+    H.sclm = L.take(RG_ZERO, sizeof(double) * np);
+    H.sccam = L.take(RG_ZERO, sizeof(double) * MAX_N);
+    H.pose1 = L.take(RG_WORK, sizeof(double) * 7 * ncam);
+    H.invd1 = L.take(RG_WORK, sizeof(double) * np);
+    H.camslot = L.take(RG_WORK, sizeof(int32_t) * ncam);
+    H.Jr = L.take(RG_WORK, sizeof(double) * 2 * no);
+    H.Ja = L.take(RG_WORK, sizeof(double) * 12 * no);
+    H.Jo = L.take(RG_WORK, sizeof(double) * 12 * no);
+    H.Jl = L.take(RG_WORK, sizeof(double) * 2 * no);
+    H.chi2 = L.take(RG_WORK, sizeof(double) * no);
+    H.dpos = L.take(RG_WORK, no);
+    H.ete = L.take(RG_WORK, sizeof(double) * np);
+    H.ge = L.take(RG_WORK, sizeof(double) * np);
+    H.acc = L.take(RG_WORK, sizeof(double) * H.blk);
+    H.total = L.take(RG_WORK, sizeof(double) * H.blk);
+    H.scal = L.take(RG_WORK, sizeof(double) * 2 * SC_COUNT);
+    H.z = L.take(RG_WORK, sizeof(double) * MAX_N);
+    H.panel = L.take(RG_WORK, sizeof(double) * CH_NB * (size_t)(MAX_N + 24));
     // dynamic shared memory: [keyframe table: 12 doubles + 1 slot each][union: Schur scratch | solve area]
     size_t s = sizeof(double) * 12 * (size_t)ncam + sizeof(int) * (size_t)ncam;
     s = (s + 15) & ~(size_t)15;
@@ -1714,7 +1704,7 @@ static ov2_status plan_window(ov2_ctx* ctx, const ov2_ba_problem* pb, int world,
     return OV2_OK;
 }
 
-static void fill_prob(const ov2_ba_problem* pb, const ov2_ba_opts* opts, const HostPlan& H, char* din, char* dwork, Prob& P,
+static void fill_prob(const ov2_ba_problem* pb, const ov2_ba_opts* opts, const HostPlan& H, const Layout& L, Prob& P,
                       const double* Kh, const double* krh, const double* trlh, const int* stop_flag_dev) {
     memset(&P, 0, sizeof(P));
     P.ncam = pb->ncam; P.npts = pb->npts; P.nobs = pb->nobs;
@@ -1740,40 +1730,33 @@ static void fill_prob(const ov2_ba_problem* pb, const ov2_ba_opts* opts, const H
     P.max_it1 = opts->max_iters_robust; P.max_it2 = opts->max_iters_refine;
     P.ftol = opts->function_tolerance;
     P.stop_flag = stop_flag_dev;
-    P.pose_const = (const uint8_t*)(din + H.off_pc);
-    P.lm_anchor_cam = (const int32_t*)(din + H.off_lac);
-    P.lm_anchor_px = (const double*)(din + H.off_apx);
-    P.obs_cam = (const int32_t*)(din + H.off_oc);
-    P.obs_lm = (const int32_t*)(din + H.off_ol);
-    P.obs_px = (const double*)(din + H.off_opx);
-    P.obs_type = pb->obs_type ? (const uint8_t*)(din + H.off_ty) : nullptr;
-    P.lm_ptr = (const int32_t*)(din + H.off_lp);
-    P.pose[0] = (double*)(din + H.off_pose); P.pose[1] = (double*)(dwork + H.w_pose1);
-    P.invd[0] = (double*)(din + H.off_invd); P.invd[1] = (double*)(dwork + H.w_invd1);
-    P.active = (uint8_t*)(dwork + H.w_active); P.flags = (uint8_t*)(dwork + H.w_flags);
-    P.cam_used = (uint8_t*)(dwork + H.w_camused); P.cam_slot = (int32_t*)(dwork + H.w_camslot);
-    P.Jr = (double*)(dwork + H.w_Jr); P.Ja = (double*)(dwork + H.w_Ja); P.Jo = (double*)(dwork + H.w_Jo); P.Jl = (double*)(dwork + H.w_Jl);
-    P.chi2 = (double*)(dwork + H.w_chi2); P.dpos = (uint8_t*)(dwork + H.w_dpos);
-    P.sc_lm = (double*)(dwork + H.w_sclm); P.ete = (double*)(dwork + H.w_ete); P.ge = (double*)(dwork + H.w_ge);
-    P.acc = (double*)(dwork + H.w_acc); P.total = (double*)(dwork + H.w_total); P.scal = (double*)(dwork + H.w_scal);
-    P.z = (double*)(dwork + H.w_z); P.sc_cam = (double*)(dwork + H.w_sccam); P.panel = (double*)(dwork + H.w_panel);
-    P.counts = (double*)(dwork + H.w_counts); P.bar = (unsigned*)(dwork + H.w_bar); P.result = (Result*)(dwork + H.w_result);
+    P.pose_const = (const uint8_t*)L.d(H.pc);
+    P.lm_anchor_cam = (const int32_t*)L.d(H.lac);
+    P.lm_anchor_px = (const double*)L.d(H.apx);
+    P.obs_cam = (const int32_t*)L.d(H.oc);
+    P.obs_lm = (const int32_t*)L.d(H.ol);
+    P.obs_px = (const double*)L.d(H.opx);
+    P.obs_type = pb->obs_type ? (const uint8_t*)L.d(H.ty) : nullptr;
+    P.lm_ptr = (const int32_t*)L.d(H.lp);
+    P.pose[0] = (double*)L.d(H.pose); P.pose[1] = (double*)L.d(H.pose1);
+    P.invd[0] = (double*)L.d(H.invd); P.invd[1] = (double*)L.d(H.invd1);
+    P.active = (uint8_t*)L.d(H.active); P.flags = (uint8_t*)L.d(H.flags);
+    P.cam_used = (uint8_t*)L.d(H.camused); P.cam_slot = (int32_t*)L.d(H.camslot);
+    P.Jr = (double*)L.d(H.Jr); P.Ja = (double*)L.d(H.Ja); P.Jo = (double*)L.d(H.Jo); P.Jl = (double*)L.d(H.Jl);
+    P.chi2 = (double*)L.d(H.chi2); P.dpos = (uint8_t*)L.d(H.dpos);
+    P.sc_lm = (double*)L.d(H.sclm); P.ete = (double*)L.d(H.ete); P.ge = (double*)L.d(H.ge);
+    P.acc = (double*)L.d(H.acc); P.total = (double*)L.d(H.total); P.scal = (double*)L.d(H.scal);
+    P.z = (double*)L.d(H.z); P.sc_cam = (double*)L.d(H.sccam); P.panel = (double*)L.d(H.panel);
+    P.counts = (double*)L.d(H.counts); P.bar = (unsigned*)L.d(H.bar); P.result = (Result*)L.d(H.result);
     // OV2_BA_TRACE selects no path: it records per-phase times and prints the window's plan (read back by the plan tests)
-    P.trace = getenv("OV2_BA_TRACE") ? (unsigned long long*)(dwork + H.w_trace) : nullptr;
+    P.trace = getenv("OV2_BA_TRACE") ? (unsigned long long*)L.d(H.trace) : nullptr;
     P.ncv_max = H.ncv_max; P.blk = H.blk; P.solve_blocked = H.solve_blocked;
     P.sg = H.sg;   // lanes per landmark in the per-landmark phases
-    P.cam_tab = H.cam_tab_global ? (double*)(dwork + H.w_camtab) : nullptr;
+    P.cam_tab = H.cam_tab_global ? (double*)L.d(H.camtab) : nullptr;
     P.cam_tab_stride = H.tab_bytes / sizeof(double);
     P.schur_smem = H.schur_smem; P.smem_sacc_off = (int)H.smem_sacc_off;
-    P.pair_perm = (const int32_t*)(din + H.off_pp); P.pair_chunk = (const int2*)(din + H.off_pch); P.npchunk = 0;
+    P.pair_perm = (const int32_t*)L.d(H.pp); P.pair_chunk = (const int2*)L.d(H.pch); P.npchunk = 0;
     P.smem_work_off = (int)H.smem_work_off;
-}
-
-static ov2_status host_copy(ov2_ctx* ctx, void* dst, const void* src, size_t bytes, bool maybe_device = true) {
-    if (bytes == 0) return OV2_OK;
-    if (maybe_device && ov2_is_device_ptr(src)) OV2_CUDA(ctx, cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
-    else memcpy(dst, src, bytes);
-    return OV2_OK;
 }
 
 // Solves `nprob` windows with one launch.  peers: multi-GPU exchange description (world 1 = none).
@@ -1786,8 +1769,8 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     std::vector<HostPlan> plans(nprob);
     std::vector<ov2_ba_problem> hp(nprob);           // host-resident views of every window (device inputs are copied down)
     std::vector<std::vector<char>> hold;              // storage for inputs that came as device pointers
-    std::vector<char> win_on_device(nprob, 0);
-    size_t st_off = 0, in_off = 0, work_off = 0, zero_off = 0, out_off = 0, act_off = 0;
+    std::vector<Residence> where(nprob);
+    Layout L;
     size_t smem_max = 0;
     int gmax_work = 1;
     for (int k = 0; k < nprob; ++k) {
@@ -1797,14 +1780,13 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         hp[k] = pb;
         // the flattened window is host data in the reference's flow (optimizer.cpp:43-430); device-resident inputs are
         // accepted and staged through the host once (the solve itself never leaves the device)
-        // cudaPointerGetAttributes costs ~1.5 us on a plain host pointer: 15 queries per window were 6 ms of a 296-window batch.
-        // One query per window: a window whose `pose` array is host memory is taken to be host memory throughout (the
-        // reference's flow, optimizer.cpp:43-430); only windows whose poses live on the device are inspected array by array.
-        const bool win_dev = ov2_is_device_ptr(pb.pose);
-        win_on_device[k] = win_dev ? 1 : 0;
+        Residence& R = where[k];
+        R.window = ov2_is_device_ptr(pb.pose);
+        R.invd = R.on_device(pb.lm_invdepth);
+        R.flags = R.on_device(outlier_outs ? outlier_outs[k] : nullptr);
         cudaError_t pull_err = cudaSuccess;
         auto pull = [&](const void* p, size_t bytes) -> const void* {
-            if (!p || bytes == 0 || !win_dev || !ov2_is_device_ptr(p)) return p;
+            if (!p || bytes == 0 || !R.on_device(p)) return p;
             hold.emplace_back(bytes);
             const cudaError_t ce = cudaMemcpy(hold.back().data(), p, bytes, cudaMemcpyDeviceToHost);
             if (ce != cudaSuccess) pull_err = ce;
@@ -1822,7 +1804,7 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         hp[k].Trl = (const double*)pull(pb.Trl, 56);
         if (pull_err != cudaSuccess) return ov2_fail(ctx, OV2_ERR_CUDA, "ov2_localba_solve: staging a device-resident window", pull_err);
         if (pb.obs_type && (!pb.Kr || !pb.Trl)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_localba_solve: obs_type given without Kr / Trl");
-        if ((st = plan_window(ctx, &hp[k], world, st_off, in_off, work_off, zero_off, out_off, act_off, plans[k], nprob == 1)) != OV2_OK) return st;
+        if ((st = plan_window(ctx, &hp[k], world, L, plans[k], nprob == 1)) != OV2_OK) return st;
         if (plans[k].smem_bytes > smem_max) smem_max = plans[k].smem_bytes;
         const int wk = (pb.nobs + THREADS - 1) / THREADS;
         const int wl = (pb.npts + WARPS - 1) / WARPS;                  // a landmark per warp and phase (single window: every SM helps)
@@ -1862,40 +1844,20 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     int grid = ngroups * G;
     // keyframe tables that live in the work block: one per CTA of the window's group
     for (int k = 0; k < nprob; ++k)
-        if (plans[k].cam_tab_global) plans[k].w_camtab = take(work_off, (size_t)G * plans[k].tab_bytes);
-    // ---- pack the inputs into one pinned block: ONE H2D copy for the whole batch.  Layout: [states | everything else]
-    const size_t st_bytes = (st_off + 255) & ~(size_t)255;
-    for (int k = 0; k < nprob; ++k) {
-        HostPlan& H = plans[k];
-        for (size_t* f : {&H.off_prob, &H.off_apx, &H.off_opx, &H.off_lac, &H.off_oc, &H.off_ol, &H.off_lp, &H.off_pc, &H.off_ty, &H.off_pp, &H.off_pch}) *f += st_bytes;
-    }
-    const size_t in_bytes = st_bytes + ((in_off + 255) & ~(size_t)255);
-    // work block layout: [per-window work areas | zero region | output region (Result + flags) | 'active' region]
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t zbase = al(work_off), zbytes = al(zero_off);
-    const size_t obase = zbase + zbytes, obytes = al(out_off);
-    const size_t abase = obase + obytes, abytes = al(act_off);
-    for (int k = 0; k < nprob; ++k) {
-        HostPlan& H = plans[k];
-        for (size_t* f : {&H.w_camused, &H.w_counts, &H.w_bar, &H.w_trace, &H.w_sclm, &H.w_sccam}) *f += zbase;
-        H.w_result = obase + H.out_result;
-        H.w_flags = obase + H.out_flags;
-        H.w_active = abase + H.act_rel;
-    }
-    const size_t host_need = in_bytes + obytes;      // pinned: [packed inputs / returned states | returned output region]
+        if (plans[k].cam_tab_global) plans[k].camtab = L.take(RG_WORK, (size_t)G * plans[k].tab_bytes);
+    // ---- pack the inputs into one pinned block: ONE H2D copy for the whole batch
+    const size_t in_bytes = L.upload_bytes();
+    const size_t host_need = in_bytes + L.bytes(RG_OUT);      // pinned: [packed inputs / returned states | returned output region]
     if (ctx->ba_ws_cap < host_need) {
         if (ctx->ba_ws) cudaFreeHost(ctx->ba_ws);
         ctx->ba_ws = nullptr; ctx->ba_ws_cap = 0;
         OV2_CUDA(ctx, cudaHostAlloc(&ctx->ba_ws, host_need * 2, cudaHostAllocDefault));
         ctx->ba_ws_cap = host_need * 2;
     }
-    char* hpk = (char*)ctx->ba_ws;
-    char* hout = hpk + in_bytes;
-    void* o = nullptr;
-    if ((st = ov2_scratch(ctx, in_bytes, &o)) != OV2_OK) return st;
-    char* din = (char*)o;
-    if ((st = ov2_scratch(ctx, abase + abytes + 256, &o)) != OV2_OK) return st;
-    char* dwork = (char*)o;
+    void *dup = nullptr, *dwork = nullptr, *o = nullptr;
+    if ((st = ov2_scratch(ctx, in_bytes, &dup)) != OV2_OK) return st;
+    if ((st = ov2_scratch(ctx, L.work_bytes() + 256, &dwork)) != OV2_OK) return st;
+    L.place((char*)dup, (char*)dwork, (char*)ctx->ba_ws);
     // one window's share of the packing: validation, CSR by landmark, copies into the pinned block, the Prob record.
     // Windows write disjoint parts of the block, so a batch is packed by a few host threads.  Returns an error text.
     auto pack_window = [&](int k) -> const char* {
@@ -1903,7 +1865,7 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         const HostPlan& H = plans[k];
         const int ncam = pb.ncam, npts = pb.npts, nobs = pb.nobs;
         // CSR by landmark (observations must be sorted by landmark)
-        int32_t* lp = (int32_t*)(hpk + H.off_lp);
+        int32_t* lp = (int32_t*)L.h(H.lp);
         memset(lp, 0, sizeof(int32_t) * (size_t)(npts + 1));
         for (int i = 0; i < nobs; ++i) {
             const int l = pb.obs_lm[i];
@@ -1915,21 +1877,23 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
             if (pb.obs_cam[i] < 0 || pb.obs_cam[i] >= ncam) return "ov2_localba_solve: obs_cam out of range";
         for (int l = 0; l < npts; ++l)
             if (pb.lm_anchor_cam[l] < 0 || pb.lm_anchor_cam[l] >= ncam) return "ov2_localba_solve: lm_anchor_cam out of range";
-        if (host_copy(ctx, hpk + H.off_pose, pbs[k].pose, sizeof(double) * 7 * ncam, win_on_device[k] != 0) != OV2_OK) return "ov2_localba_solve: copying the poses failed";
-        if (host_copy(ctx, hpk + H.off_invd, pbs[k].lm_invdepth, sizeof(double) * (size_t)npts, win_on_device[k] != 0) != OV2_OK) return "ov2_localba_solve: copying the inverse depths failed";
-        memcpy(hpk + H.off_apx, pb.lm_anchor_px, sizeof(double) * 2 * (size_t)npts);
-        memcpy(hpk + H.off_opx, pb.obs_px, sizeof(double) * 2 * (size_t)nobs);
-        memcpy(hpk + H.off_lac, pb.lm_anchor_cam, sizeof(int32_t) * (size_t)npts);
-        memcpy(hpk + H.off_oc, pb.obs_cam, sizeof(int32_t) * (size_t)nobs);
-        memcpy(hpk + H.off_ol, pb.obs_lm, sizeof(int32_t) * (size_t)nobs);
-        memcpy(hpk + H.off_pc, pb.pose_const, (size_t)ncam);
-        if (pb.obs_type) memcpy(hpk + H.off_ty, pb.obs_type, (size_t)nobs);
+        if (copy_state(L.h(H.pose), pbs[k].pose, sizeof(double) * 7 * ncam, where[k].window, cudaMemcpyDeviceToHost) != cudaSuccess)
+            return "ov2_localba_solve: copying the poses failed";
+        if (copy_state(L.h(H.invd), pbs[k].lm_invdepth, sizeof(double) * (size_t)npts, where[k].invd, cudaMemcpyDeviceToHost) != cudaSuccess)
+            return "ov2_localba_solve: copying the inverse depths failed";
+        memcpy(L.h(H.apx), pb.lm_anchor_px, sizeof(double) * 2 * (size_t)npts);
+        memcpy(L.h(H.opx), pb.obs_px, sizeof(double) * 2 * (size_t)nobs);
+        memcpy(L.h(H.lac), pb.lm_anchor_cam, sizeof(int32_t) * (size_t)npts);
+        memcpy(L.h(H.oc), pb.obs_cam, sizeof(int32_t) * (size_t)nobs);
+        memcpy(L.h(H.ol), pb.obs_lm, sizeof(int32_t) * (size_t)nobs);
+        memcpy(L.h(H.pc), pb.pose_const, (size_t)ncam);
+        if (pb.obs_type) memcpy(L.h(H.ty), pb.obs_type, (size_t)nobs);
         Prob P;
-        fill_prob(&pb, opts, H, din, dwork, P, pb.K, pb.Kr, pb.Trl, stop_flag_dev);
+        fill_prob(&pb, opts, H, L, P, pb.K, pb.Kr, pb.Trl, stop_flag_dev);
         if (H.schur_smem == 3) {
             // stable counting sort of the observations by (anchor keyframe, observing keyframe), cut into chunks of <= PCH
-            int32_t* perm = (int32_t*)(hpk + H.off_pp);
-            int2* chunks = (int2*)(hpk + H.off_pch);
+            int32_t* perm = (int32_t*)L.h(H.pp);
+            int2* chunks = (int2*)L.h(H.pch);
             std::vector<int32_t> head((size_t)ncam * ncam + 1, 0);
             for (int i = 0; i < nobs; ++i) head[(size_t)pb.lm_anchor_cam[pb.obs_lm[i]] * ncam + pb.obs_cam[i] + 1]++;
             for (size_t g = 0; g < (size_t)ncam * ncam; ++g) head[g + 1] += head[g];
@@ -1945,7 +1909,7 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
                 }
             P.npchunk = nch;
         }
-        memcpy(hpk + H.off_prob, &P, sizeof(P));
+        memcpy(L.h(H.prob), &P, sizeof(P));
         return nullptr;
     };
     {
@@ -1971,15 +1935,15 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     }
     // the Prob records must be contiguous for the kernel: they are the first thing of each window's block, so gather them
     std::vector<Prob> parr(nprob);
-    for (int k = 0; k < nprob; ++k) memcpy(&parr[k], hpk + plans[k].off_prob, sizeof(Prob));
+    for (int k = 0; k < nprob; ++k) memcpy(&parr[k], L.h(plans[k].prob), sizeof(Prob));
     if ((st = ov2_scratch(ctx, sizeof(Prob) * (size_t)nprob, &o)) != OV2_OK) return st;
     Prob* dprobs = (Prob*)o;
     cudaStream_t s = ctx->stream;
-    OV2_CUDA(ctx, cudaMemcpyAsync(din, hpk, in_bytes, cudaMemcpyHostToDevice, s));
-    if (nprob == 1) dprobs = (Prob*)(din + plans[0].off_prob);
+    OV2_CUDA(ctx, cudaMemcpyAsync(L.dev[RG_STATE], L.host[RG_STATE], in_bytes, cudaMemcpyHostToDevice, s));
+    if (nprob == 1) dprobs = (Prob*)L.d(plans[0].prob);
     else OV2_CUDA(ctx, cudaMemcpyAsync(dprobs, parr.data(), sizeof(Prob) * (size_t)nprob, cudaMemcpyHostToDevice, s));   // parr outlives the sync below
-    OV2_CUDA(ctx, cudaMemsetAsync(dwork + zbase, 0, zbytes + obytes, s));   // zero region + output region of every window
-    OV2_CUDA(ctx, cudaMemsetAsync(dwork + abase, 1, abytes, s));            // every observation starts active
+    OV2_CUDA(ctx, cudaMemsetAsync(L.dev[RG_ZERO], 0, L.bytes(RG_ZERO) + L.bytes(RG_OUT), s));   // zero + output regions of every window
+    OV2_CUDA(ctx, cudaMemsetAsync(L.dev[RG_ACT], 1, L.bytes(RG_ACT), s));                      // every observation starts active
     Peers X;
     memset(&X, 0, sizeof(X));
     X.world = 1;
@@ -1996,24 +1960,18 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     if (le != cudaSuccess) return ov2_fail(ctx, OV2_ERR_CUDA, "ba_lm_kernel launch", le);
     if (ctx->profiling) ov2_prof_end(ctx, "ba_lm_kernel");
     // ---- results: [pose | invd] live in the input block (buffer 0), flags + result record in the work block
-    OV2_CUDA(ctx, cudaMemcpyAsync(hpk, din, st_bytes, cudaMemcpyDeviceToHost, s));   // poses and inverse depths of every window: one copy
-    OV2_CUDA(ctx, cudaMemcpyAsync(hout, dwork + obase, obytes, cudaMemcpyDeviceToHost, s));   // Result records + outlier flags: one copy
-    std::vector<Result> hres(nprob);
-    std::vector<char> flags_to_host(nprob, 0);
-    for (int k = 0; k < nprob; ++k) {
-        if (outlier_outs && outlier_outs[k] && pbs[k].nobs > 0) {
-            if (win_on_device[k] && ov2_is_device_ptr(outlier_outs[k])) {
-                OV2_CUDA(ctx, cudaMemcpyAsync(outlier_outs[k], dwork + plans[k].w_flags, (size_t)pbs[k].nobs, cudaMemcpyDeviceToDevice, s));
-            } else {
-                flags_to_host[k] = 1;
-            }
-        }
-    }
+    OV2_CUDA(ctx, cudaMemcpyAsync(L.host[RG_STATE], L.dev[RG_STATE], L.bytes(RG_STATE), cudaMemcpyDeviceToHost, s));   // poses and inverse depths of every window: one copy
+    OV2_CUDA(ctx, cudaMemcpyAsync(L.host[RG_OUT], L.dev[RG_OUT], L.bytes(RG_OUT), cudaMemcpyDeviceToHost, s));         // Result records + outlier flags: one copy
+    auto wants_flags = [&](int k) { return outlier_outs && outlier_outs[k] && pbs[k].nobs > 0; };
+    for (int k = 0; k < nprob; ++k)
+        if (wants_flags(k) && where[k].flags)
+            OV2_CUDA(ctx, cudaMemcpyAsync(outlier_outs[k], L.d(plans[k].flags), (size_t)pbs[k].nobs, cudaMemcpyDeviceToDevice, s));
     OV2_CUDA(ctx, cudaStreamSynchronize(s));
-    for (int k = 0; k < nprob; ++k) memcpy(&hres[k], hout + plans[k].out_result, sizeof(Result));
+    std::vector<Result> hres(nprob);
+    for (int k = 0; k < nprob; ++k) memcpy(&hres[k], L.h(plans[k].result), sizeof(Result));
     if (getenv("OV2_BA_TRACE")) {
         unsigned long long tr[16];
-        cudaMemcpy(tr, dwork + plans[0].w_trace, sizeof(tr), cudaMemcpyDeviceToHost);
+        cudaMemcpy(tr, L.d(plans[0].trace), sizeof(tr), cudaMemcpyDeviceToHost);
         static const char* names[16] = {"setup0", "A:eval", "B:schur", "B2:fold", "C:solve", "C:wait", "D:backsub", "E:ctl", "scan", "wb", "setup1", "bar0",
                                         "chol:P1", "chol:bar", "chol:P2", "chol:back|ownerB1"};
         fprintf(stderr, "[ba trace] G=%d grid=%d smem=%zu smemS=%d camtab=%s blocked=%d sg=%d |", G, grid, smem_max,
@@ -2025,13 +1983,9 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     for (int k = 0; k < nprob; ++k) {
         const HostPlan& H = plans[k];
         const size_t pb_bytes = sizeof(double) * 7 * pbs[k].ncam, ib = sizeof(double) * (size_t)pbs[k].npts;
-        if (win_on_device[k]) cudaMemcpy(pbs[k].pose, hpk + H.off_pose, pb_bytes, cudaMemcpyHostToDevice);
-        else memcpy(pbs[k].pose, hpk + H.off_pose, pb_bytes);
-        if (ib) {
-            if (win_on_device[k] && ov2_is_device_ptr(pbs[k].lm_invdepth)) cudaMemcpy(pbs[k].lm_invdepth, hpk + H.off_invd, ib, cudaMemcpyHostToDevice);
-            else memcpy(pbs[k].lm_invdepth, hpk + H.off_invd, ib);
-        }
-        if (flags_to_host[k]) memcpy(outlier_outs[k], hout + plans[k].out_flags, (size_t)pbs[k].nobs);
+        copy_state(pbs[k].pose, L.h(H.pose), pb_bytes, where[k].window, cudaMemcpyHostToDevice);
+        copy_state(pbs[k].lm_invdepth, L.h(H.invd), ib, where[k].invd, cudaMemcpyHostToDevice);
+        if (wants_flags(k) && !where[k].flags) memcpy(outlier_outs[k], L.h(H.flags), (size_t)pbs[k].nobs);
         ov2_ba_result& r = results[k];
         memset(&r, 0, sizeof(r));
         r.iters_robust = hres[k].iters_robust; r.iters_refine = hres[k].iters_refine;
