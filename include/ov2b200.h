@@ -179,6 +179,36 @@ OV2_API ov2_status ov2_debug_klt_counts(ov2_ctx* ctx, const ov2_pyr* prev, const
                       const uint8_t* nbpyrlvl, int nbpyrlvl_all,
                       const float* kps, float* priors_inout, uint8_t* status_out, int32_t* counts_out);
 
+/* ------------------------------------------------------------------ K2: the front-end's frame tracking
+ * Replaces VisualFrontEnd::kltTracking() (/root/reference/src/visual_front_end.cpp:132-275) for frames [first, first+count)
+ * of two pyramids.  Frame k owns keypoints [offsets[k], offsets[k+1]) of px ([n][2] float, kp.px_), wpt ([n][3] double, the
+ * keypoint's map point; read only where is3d) and is3d ([n] bytes, kp.is3d_); n = offsets[count].  Per frame: Tcw[k] = 12
+ * doubles (row-major rotation, then translation, as ov2_match_problem), K[k] = fx, fy, cx, cy, dist[k] = k1, k2, p1, p2, k3 of
+ * the radial-tangential model (dist NULL: no distortion in any frame), img_wh[k] = the calibration's image width, height.
+ *   prior    Frame::projWorldToImageDist (src/frame.cpp:825-828, src/camera_calibration.cpp:254-281): Tcw * X in double,
+ *            invz = 1 / z, x * invz, y * invz; without distortion fx * x + cx in double rounded to float, with it
+ *            cv::projectPoints on Point3f(x, y, 1) as ov2_match_to_map evaluates it.  z is not tested (the reference does not):
+ *            a point behind the camera whose projection lands in the image gets a prior.
+ *   in image Frame::isInImage (src/frame.cpp:840-843): x >= 0 && y >= 0 && x < img_w && y < img_h, float against int.
+ *   pass 1   the 3-D keypoints whose prior is in the image, tracked from the prior at depth 1 (fbKltTracking, nbpyrlvl 1).
+ *            Skipped when use_prior == 0 or the frame has no such keypoint.
+ *   rule     p3p_req = nbgood < 0.33 * nbkps in double, on the frame's pass-1 counts (0 when pass 1 is skipped).
+ *   pass 2   the 2-D keypoints, the 3-D keypoints without an in-image prior (prior = px) and the failed pass-1 keypoints,
+ *            at depth nklt_pyr_lvl; a failed pass-1 keypoint starts from its pass-1 forward result, or from px when p3p_req.
+ * Outputs: tracked_out ([n][2]: the pass-1 result of a pass-1 track, else the pass-2 forward result, the position the
+ * reference's updateKeypoint receives for a tracked keypoint), status_out ([n] 0/1), pass_out ([n]: 0 none, 1 pass 1,
+ * 2 pass 2); per frame p3p_req_out, nbgood_out and nbkps_out (pass-1 counts).  A keypoint with px.x < 0 is an empty slot:
+ * pass 0, status 0, tracked = px, not counted.
+ * Both passes are ov2_fb_klt over all n slots (non-members are empty slots): status and positions equal to fbKltTracking
+ * on each pass's keypoints.  offsets must be a HOST pointer that starts at 0 and never decreases (OV2_ERR_INVALID
+ * otherwise, nothing staged or written); every other array may be host or device memory.  There is no host
+ * synchronisation between the passes; with device arrays the call only enqueues. */
+OV2_API ov2_status ov2_klt_tracking(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, const ov2_klt_params* prm, int first,
+                                    int count, const int32_t* offsets, const double* Tcw, const double* K, const double* dist,
+                                    const int32_t* img_wh, const float* px, const double* wpt, const uint8_t* is3d,
+                                    int nklt_pyr_lvl, int use_prior, float* tracked_out, uint8_t* status_out, uint8_t* pass_out,
+                                    uint8_t* p3p_req_out, int32_t* nbgood_out, int32_t* nbkps_out);
+
 /* ------------------------------------------------------------------ F + S: grid FAST + cornerSubPix
  * Replaces FeatureExtractor::detectGridFAST(im, ncellsize, vcurkps, roi)
  * (/root/reference/src/feature_extractor.cpp:443-570; include/feature_extractor.hpp:41-42) with

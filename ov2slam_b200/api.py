@@ -3,6 +3,7 @@
 This is the Python-side mirror of the reference's operator interface for the hot paths:
 
     FeatureTracker.fb_klt_tracking   <- FeatureTracker::fbKltTracking   (feature_tracker.cpp:35-137)
+    FeatureTracker.klt_tracking      <- VisualFrontEnd::kltTracking     (visual_front_end.cpp:132-275)
     FeatureExtractor.detect_grid_fast<- FeatureExtractor::detectGridFAST(feature_extractor.cpp:443-570)
     FeatureExtractor.describe_brief  <- FeatureExtractor::describeBRIEF (feature_extractor.cpp:224-285)
     Optimizer.local_ba               <- Optimizer::localBA solve part   (optimizer.cpp:436-735)
@@ -31,7 +32,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_debug_klt_counts", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_klt_tracking", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_debug_klt_counts", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -128,6 +129,8 @@ def load():
     lib.ov2_remap.argtypes = [vp, vp, vp, sz, sz, vp, sz, sz, i32]
     lib.ov2_pyr_build_remap.argtypes = [vp, vp, vp, vp, sz, sz, i32, i32]
     lib.ov2_fb_klt.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp]
+    lib.ov2_klt_tracking.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32,
+                                     vp, vp, vp, vp, vp, vp]
     lib.ov2_debug_klt_counts.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp, vp]
     lib.ov2_grid_fast.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_detect_single_scale.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, i32]
@@ -392,6 +395,38 @@ class FeatureTracker:
             self.ctx.check(self.ctx.lib.ov2_fb_klt(*args))
         else:
             self.ctx.check(self.ctx.lib.ov2_debug_klt_counts(*args, _ptr(counts_out)))
+
+    def klt_tracking(self, prev: Pyramid, cur: Pyramid, nwinsize, nklt_pyr_lvl, ferr, fmax_fbklt_dist, offsets, Tcw, K, img_wh,
+                     px, wpt, is3d, dist=None, use_prior=True, first=0, out=None):
+        """VisualFrontEnd::kltTracking for frames [first, first + count) (ov2_klt_tracking).  offsets: int32[count + 1] (host);
+        per frame Tcw float64[count, 12] (row-major R, then t), K float64[count, 4], img_wh int32[count, 2], dist
+        float64[count, 5] or None; per keypoint px float32[n, 2], wpt float64[n, 3], is3d uint8[n].  Inputs may be numpy
+        (host) or CUDA tensors (device).  Returns dict(tracked, status, passes, p3p_req, nbgood, nbkps) as numpy arrays, or
+        fills `out` (a dict with those keys, host or device arrays) and returns it."""
+        offsets = np.ascontiguousarray(offsets, np.int32)
+        count = len(offsets) - 1
+        n = int(offsets[-1]) if count >= 0 else 0
+        if out is None:
+            out = dict(tracked=np.zeros((n, 2), np.float32), status=np.zeros(n, np.uint8), passes=np.zeros(n, np.uint8),
+                       p3p_req=np.zeros(count, np.uint8), nbgood=np.zeros(count, np.int32), nbkps=np.zeros(count, np.int32))
+        prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
+
+        def typed(a, dt, name):
+            # numpy inputs are converted to the ABI's types; a tensor of another type is refused (its bytes would be misread)
+            if a is None or isinstance(a, int):
+                return a
+            if isinstance(a, np.ndarray) or not hasattr(a, "data_ptr"):
+                return np.ascontiguousarray(a, dt)
+            if str(a.dtype) != "torch." + np.dtype(dt).name:
+                raise Ov2Error(f"klt_tracking: {name} must be {np.dtype(dt).name}, got {a.dtype}")
+            return a
+        Tcw, K, dist, wpt = (typed(a, np.float64, nm) for a, nm in ((Tcw, "Tcw"), (K, "K"), (dist, "dist"), (wpt, "wpt")))
+        img_wh, px, is3d = typed(img_wh, np.int32, "img_wh"), typed(px, np.float32, "px"), typed(is3d, np.uint8, "is3d")
+        self.ctx.check(self.ctx.lib.ov2_klt_tracking(
+            self.ctx.h, prev.h_, cur.h_, C.byref(prm), int(first), count, offsets.ctypes.data, _ptr(Tcw), _ptr(K), _ptr(dist),
+            _ptr(img_wh), _ptr(px), _ptr(wpt), _ptr(is3d), int(nklt_pyr_lvl), 1 if use_prior else 0, _ptr(out["tracked"]),
+            _ptr(out["status"]), _ptr(out["passes"]), _ptr(out["p3p_req"]), _ptr(out["nbgood"]), _ptr(out["nbkps"])))
+        return out
 
     def line_min_sad(self, left: Pyramid, right: Pyramid, level: int, pts, nwinsize, goleft, xprior_out, l1err_out,
                      n=None, frame_idx=None, first_frame=0, per_frame=None):

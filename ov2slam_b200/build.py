@@ -24,6 +24,7 @@ SOURCES = {
     "ctx.cu": [],
     "frontend_pyr.cu": ["-fmad=false"],
     "frontend_klt.cu": ["-fmad=false"],
+    "frontend_klt_tracking.cu": ["-fmad=false"],
     "frontend_fast.cu": ["-fmad=false"],
     "frontend_desc.cu": ["-fmad=false"],
     "frontend_clahe.cu": ["-fmad=false"],
@@ -125,6 +126,7 @@ def build_optimizer_shim(verbose: bool = False) -> Path:
     subprocess.check_call(["g++", "-o", str(exe), *objs, "-L", str(LIB), "-lov2b200", "-lpthread", "-Wl,-rpath,$ORIGIN"])
     build_mapper_shim(verbose)
     build_stereo_shim(verbose)
+    build_klt_tracking_shim(verbose)
     return exe
 
 
@@ -168,6 +170,28 @@ def build_stereo_shim(verbose: bool = False) -> Path:
             subprocess.check_call(cmd)
         objs.append(str(obj))
     exe = LIB / "stereo_selftest"
+    subprocess.check_call(["g++", "-o", str(exe), *objs, "-L", str(LIB), "-lov2b200", "-lpthread", "-Wl,-rpath,$ORIGIN"])
+    return exe
+
+
+def build_klt_tracking_shim(verbose: bool = False) -> Path:
+    """Compile the drop-in VisualFrontEnd::kltTracking (host/visual_front_end_klt_gpu.cpp) with the drop-in FeatureTracker against the
+    stand-in front-end / map / OpenCV headers and link its self-test driver."""
+    host = ROOT / "host"
+    build()
+    objs = []
+    deps = list(host.glob("*.hpp")) + list((host / "standin").rglob("*"))
+    for name in ("feature_tracker.cpp", "visual_front_end_klt_gpu.cpp", "klt_tracking_selftest.cpp"):
+        obj = LIB / "obj" / (name + ".klt.o")
+        src = host / name
+        if _newer(src, obj) or any(d.is_file() and _newer(d, obj) for d in deps):
+            cmd = ["g++", "-std=c++17", "-O2", "-Wall", "-fPIC", "-I", str(host / "standin" / "ref"), "-I", str(host / "standin"), "-I", str(host),
+                   "-c", str(src), "-o", str(obj)]
+            if verbose:
+                print(" ".join(cmd), flush=True)
+            subprocess.check_call(cmd)
+        objs.append(str(obj))
+    exe = LIB / "klt_tracking_selftest"
     subprocess.check_call(["g++", "-o", str(exe), *objs, "-L", str(LIB), "-lov2b200", "-lpthread", "-Wl,-rpath,$ORIGIN"])
     return exe
 

@@ -16,6 +16,7 @@
 // best / second scan replayed in keypoint order from the lanes' results.  match_kp_kernel: one thread per keypoint.
 // double arithmetic without FMA contraction (-fmad=false) in OpenCV's / the reference's operation order.
 #include "ov2_common.cuh"
+#include "cam_project.cuh"
 
 namespace {
 
@@ -24,8 +25,8 @@ constexpr int WARPS = 4;
 
 struct MatchDev {
     double Tcw[12];
-    double fx, fy, cx, cy, k1, k2, p1, p2, k3;
-    int has_dist, img_w, img_h, ncellsize, nbwcells, ncells;
+    CamModel cam;
+    int img_w, img_h, ncellsize, nbwcells, ncells;
     const int32_t* cell_ptr; const int32_t* cell_kp;
     int nkps; const float2* kp_px; const int32_t* kp_lm;
     int nmps; const double* mp_xyz; const int32_t* mp_desc_ptr; const uint8_t* desc; const unsigned long long* mp_kfmask;
@@ -36,27 +37,6 @@ struct MatchDev {
     int32_t* best_kp; float* best_dist;
     int32_t* kp_match; float* kp_dist;
 };
-
-// CameraCalibration::projectCamToImageDist (camera_calibration.cpp:254-281), pinhole model
-__device__ __forceinline__ float2 project_dist(const MatchDev& A, double X, double Y, double Z) {
-    const double invz = 1.0 / Z;
-    double x = X * invz, y = Y * invz;
-    if (!A.has_dist) return make_float2((float)(A.fx * x + A.cx), (float)(A.fy * y + A.cy));
-    x = (double)(float)x;                  // cv::Point3f(x, y, 1.)
-    y = (double)(float)y;
-    const double r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
-    const double a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
-    const double cdist = 1 + A.k1 * r2 + A.k2 * r4 + A.k3 * r6;
-    const double xd = x * cdist + A.p1 * a1 + A.p2 * a2;
-    const double yd = y * cdist + A.p1 * a3 + A.p2 * a1;
-    return make_float2((float)(xd * A.fx + A.cx), (float)(yd * A.fy + A.cy));
-}
-
-__device__ __forceinline__ void transform(const double* T, const double* w, double& X, double& Y, double& Z) {
-    X = T[0] * w[0] + T[1] * w[1] + T[2] * w[2] + T[9];
-    Y = T[3] * w[0] + T[4] * w[1] + T[5] * w[2] + T[10];
-    Z = T[6] * w[0] + T[7] * w[1] + T[8] * w[2] + T[11];
-}
 
 __device__ __forceinline__ int hamming256(const uint8_t* a, const uint8_t* b) {
     const uint32_t* pa = reinterpret_cast<const uint32_t*>(a);
@@ -84,8 +64,8 @@ __global__ void __launch_bounds__(WARPS * 32) match_mp_kernel(MatchDev A) {
         if (fabsf(view_angle) < A.view_th) alive = false;
     }
     if (alive) {
-        proj = project_dist(A, X, Y, Z);
-        if (!(proj.x >= 0.f && proj.y >= 0.f && proj.x < (float)A.img_w && proj.y < (float)A.img_h)) alive = false;
+        proj = project_dist(A.cam, X, Y, Z);
+        if (!in_image(proj, A.img_w, A.img_h)) alive = false;
     }
     if (alive) {
         const int rkp = (int)floor((double)(proj.y / (float)A.ncellsize)), ckp = (int)floor((double)(proj.x / (float)A.ncellsize));
@@ -126,7 +106,7 @@ __global__ void __launch_bounds__(WARPS * 32) match_mp_kernel(MatchDev A) {
                         for (int o = A.mp_obs_ptr[lm]; o < A.mp_obs_ptr[lm + 1]; ++o) {
                             double cx_, cy_, cz_;
                             transform(A.kf_Tcw + 12 * (size_t)A.obs_kf[o], wpt, cx_, cy_, cz_);
-                            const float2 pq = project_dist(A, cx_, cy_, cz_);
+                            const float2 pq = project_dist(A.cam, cx_, cy_, cz_);
                             const float2 op = A.obs_px[o];
                             const float ex = op.x - pq.x, ey = op.y - pq.y;
                             coproj = (float)((double)coproj + sqrt((double)ex * (double)ex + (double)ey * (double)ey));
@@ -188,10 +168,7 @@ extern "C" ov2_status ov2_match_to_map(ov2_ctx* ctx, const ov2_match_problem* p,
     if (st != OV2_OK) return st;
     MatchDev A;
     memcpy(A.Tcw, p->Tcw, sizeof(A.Tcw));
-    A.fx = p->K[0]; A.fy = p->K[1]; A.cx = p->K[2]; A.cy = p->K[3];
-    A.has_dist = p->dist ? 1 : 0;
-    A.k1 = A.k2 = A.p1 = A.p2 = A.k3 = 0.0;
-    if (p->dist) { A.k1 = p->dist[0]; A.k2 = p->dist[1]; A.p1 = p->dist[2]; A.p2 = p->dist[3]; A.k3 = p->dist[4]; }
+    A.cam = make_cam(p->K, p->dist);
     A.img_w = p->img_w; A.img_h = p->img_h; A.ncellsize = p->ncellsize; A.nbwcells = p->nbwcells; A.ncells = p->ncells;
     A.nkps = p->nkps; A.nmps = p->nmps; A.ncand = p->ncand;
     A.dmaxpxdist = p->dmaxpxdist; A.view_th = p->view_th;

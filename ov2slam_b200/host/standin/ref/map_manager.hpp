@@ -22,7 +22,7 @@ struct SlamParams {
     int nmin_covscore_ = 25;
     int nklt_pyr_lvl_ = 3, nklt_win_size_ = 9, nklt_err_ = 30;
     float fmax_fbklt_dist_ = 0.5f;
-    bool bdo_stereo_rect_ = false, debug_ = false, log_timings_ = false;
+    bool bdo_stereo_rect_ = false, debug_ = false, log_timings_ = false, klt_use_prior_ = true;
     bool stereo_ = false, buse_inv_depth_ = true, apply_l2_after_robust_ = true;
     float robust_mono_th_ = 5.9915f;
 };
@@ -118,6 +118,9 @@ public:
         it->second.runpx_ = pcalib_rightcam_->undistortImagePoint(pt);
         if (!it->second.is_stereo_) { it->second.is_stereo_ = true; nb_stereo_kps_++; }
     }
+    // Frame::updateKeypoint(lmid, pt) (frame.cpp:334-370): the stand-in moves the pixel only (the reference also refreshes the
+    // undistorted pixel, the bearing and the grid cell)
+    void updateKeypoint(const int lmid, const cv::Point2f& pt) { auto it = mapkps_.find(lmid); if (it != mapkps_.end()) it->second.px_ = pt; }
     Sophus::SE3d getTwc() const { return Twc_; }
     void setTwc(const Sophus::SE3d& Twc) { Twc_ = Twc; }
     std::map<int, int> getCovisibleKfMap() const { return covkfs_; }

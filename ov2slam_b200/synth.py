@@ -112,6 +112,46 @@ def make_priors(seed: int, kps: np.ndarray, flow: np.ndarray, frac3d: float = 0.
     return is3d, pri
 
 
+def make_klt_tracking_scene(seed: int, counts, w: int = 640, h: int = 480, frac3d: float = 0.6, bad_frac: float = 0.2,
+                            distorted: bool = False, images=None):
+    """Frames for VisualFrontEnd::kltTracking (ov2_klt_tracking): frame k has counts[k] keypoints, a `frac3d` share of them
+    3-D.  A 3-D keypoint's map point is placed (at a random depth, through a random pose Tcw) so that it projects near
+    px + the pair's flow, N(0, 0.7) px off; a `bad_frac` share of them projects 12 - 30 px off, so that pass 1 loses some
+    tracks and pass 2 retries them.  The placement inverts the pinhole model only, so with `distorted` the priors move by
+    the distortion too (a few px).  images = (prevs, curs, flows) to reuse pairs, else make_batch(seed, len(counts)).
+    Returns a dict of the ov2_klt_tracking arrays plus prevs, curs."""
+    counts = [int(c) for c in counts]
+    nf = len(counts)
+    prevs, curs, flows = images if images is not None else make_batch(seed, nf, w, h)
+    rng = np.random.default_rng(seed + 9_000_011)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    n = int(offsets[-1])
+    K = np.tile(np.array([458.654, 457.296, w / 2 + 7.215, h / 2 + 8.375]), (nf, 1))
+    dist = np.tile(np.array([-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05, 0.0]) * 0.2, (nf, 1)) if distorted else None
+    Tcw = np.zeros((nf, 12))
+    px = np.zeros((n, 2), np.float32)
+    wpt = np.zeros((n, 3))
+    is3d = np.zeros(n, np.uint8)
+    for f in range(nf):
+        Rm = _so3_exp(rng.normal(0, 0.3, 3))
+        t = rng.normal(0, 1.0, 3)
+        Tcw[f, :9] = Rm.reshape(-1)
+        Tcw[f, 9:] = t
+        sl = slice(offsets[f], offsets[f + 1])
+        m = counts[f]
+        px[sl] = np.stack([rng.uniform(8, w - 8, m), rng.uniform(8, h - 8, m)], 1)
+        is3d[sl] = rng.random(m) < frac3d
+        off = rng.normal(0, 0.7, (m, 2))
+        bad = rng.random(m) < bad_frac
+        off[bad] = rng.uniform(12, 30, (int(bad.sum()), 2)) * rng.choice([-1, 1], (int(bad.sum()), 2))
+        q = px[sl].astype(np.float64) + flows[f][None, :] + off
+        depth = rng.uniform(2.0, 20.0, m)
+        pc = np.stack([(q[:, 0] - K[f, 2]) / K[f, 0] * depth, (q[:, 1] - K[f, 3]) / K[f, 1] * depth, depth], 1)
+        wpt[sl] = (pc - t[None, :]) @ Rm          # R^T (pc - t), row by row
+    return dict(prevs=prevs, curs=curs, offsets=offsets, Tcw=Tcw, K=K, dist=dist,
+                img_wh=np.tile(np.array([w, h], np.int32), (nf, 1)), px=px, wpt=wpt, is3d=is3d)
+
+
 # ----------------------------------------------------------------------------- local BA
 def _so3_exp(w: np.ndarray) -> np.ndarray:
     th = np.linalg.norm(w)
