@@ -323,6 +323,49 @@ OV2_API ov2_status ov2_line_min_sad(ov2_ctx* ctx, const ov2_pyr* left, const ov2
                             const int32_t* frame_idx, int first_frame, int per_frame, const float* pts, int nwinsize,
                             int goleft, float* xprior_out, float* l1err_out);
 
+/* ------------------------------------------------------------------ 8f-3: stereo matching of keyframes
+ * Replaces MapManager::stereoMatching(frame, vleftpyr, vrightpyr) (/root/reference/src/map_manager.cpp:367-611) for
+ * keyframes [first, first+count) of a left and a right pyramid.  Keyframe k owns keypoints [offsets[k], offsets[k+1]), in
+ * the order of frame.getKeypoints(); n = offsets[count].  Per keypoint: px, unpx ([n][2] float, kp.px_, kp.unpx_), bv ([n][3]
+ * double, kp.bv_), is3d (kp.is3d_), has_mp (0 when getMapPoint(kp.lmid_) is null) and wpt ([n][3] double, the map point;
+ * read only where is3d && has_mp).  Per keyframe: Tcw[k] (12 doubles, row-major rotation then translation), the right
+ * camera's K[k] = fx, fy, cx, cy and dist[k] = k1, k2, p1, p2, k3 (dist NULL: no distortion in any keyframe), Trl[k] (the
+ * right calibration's Tcic0_, 12 doubles), Frl[k] (9 doubles, row-major) and img_wh[k] (the right image's width, height).
+ * Other rigs also pass the grid (Frame::vgridkps_): keyframe k's cells are [cell_offsets[k], cell_offsets[k+1]), row-major
+ * with grid[k] = (ncellsize, nbwcells); cell c lists the keypoints cell_kps[cell_ptr[c] .. cell_ptr[c+1]) in vgridkps_
+ * order, as keypoint indices (into px) of the keyframe, and those lists lie in cell_kps[offsets[k] .. offsets[k+1]).
+ *   prior    a 3-D keypoint with a map point: Frame::projWorldToRightImageDist (Tcw, then Trl, then the right camera as
+ *            ov2_klt_tracking projects) tested by Frame::isInRightImage.  Without a map point it is dropped (pass 0, no
+ *            stereo; the caller removes the observation).
+ *   rectified (rectified != 0) the remaining keypoints' row search: ov2_line_min_sad at level nklt_pyr_lvl, window 7,
+ *            leftwards, on px * downpyrcoef; x = xprior * uppyrcoef (floats, :380-381) replaces the prior's x iff
+ *            0 <= x <= px.x.
+ *   other    the remaining keypoints' depth prior (:438-483): Frame::getSurroundingKeypoints (the 2 x 2 cells up and to the
+ *            left, the keypoint itself excluded), 3-D neighbours with a map point weighted by 1 / cv::norm(unpx_j - unpx),
+ *            the weighted mean of their z in Tcw, in double and in cell then list order; mean_z * bv / bv.z projected
+ *            through Trl into the right image.  Equal unpx give a NaN prior, which no image contains.
+ *   pass 1   keypoints with an in-image prior, tracked from it at depth 1 (fbKltTracking, clamped as :503-505).
+ *   pass 2   the other kept keypoints and the failed pass-1 keypoints at depth nklt_pyr_lvl; the latter start from their
+ *            pass-1 forward result.
+ *   gate     the right pixel undistorted (cv::undistortPoints(pt, K, D, K), or the pixel itself without distortion);
+ *            rectified: |lun.y - run.y| and y := lun.y; other rigs: MultiViewGeometry::computeSampsonDistance(Frl, lun,
+ *            run) with its float roundings.  A track is a stereo match iff the error is <= 2.
+ * Outputs: right_out ([n][2]: what updateKeypointStereo receives for a stereo match; otherwise the track's forward result,
+ * or px for a keypoint that was not tracked), stereo_out ([n] 0/1), pass_out ([n]: 0 not tracked, 1 pass 1, 2 pass 2) and
+ * nstereo_out ([count]).  A keypoint with px.x < 0 is an empty slot: pass 0, no stereo, right = px.
+ * offsets and (other rigs) cell_offsets must be HOST pointers that start at 0 and never decrease; every other array may be
+ * host or device memory.  OV2_ERR_INVALID, with nothing staged or written, for those tables, a window outside 3 .. 31,
+ * mismatched or unbuilt pyramids, and a rectified call whose pyramids lack level nklt_pyr_lvl (or nklt_pyr_lvl > 3).
+ * There is no host synchronisation between the steps; with device arrays the call only enqueues. */
+OV2_API ov2_status ov2_stereo_matching(ov2_ctx* ctx, const ov2_pyr* left, const ov2_pyr* right, const ov2_klt_params* prm,
+                                       int first, int count, const int32_t* offsets, const double* Tcw, const double* K,
+                                       const double* dist, const double* Trl, const double* Frl, const int32_t* img_wh,
+                                       const int32_t* cell_offsets, const int32_t* grid, const int32_t* cell_ptr,
+                                       const int32_t* cell_kps, const float* px, const float* unpx, const double* bv,
+                                       const uint8_t* is3d, const uint8_t* has_mp, const double* wpt, int rectified,
+                                       int nklt_pyr_lvl, float* right_out, uint8_t* stereo_out, uint8_t* pass_out,
+                                       int32_t* nstereo_out);
+
 /* ------------------------------------------------------------------ 8f-4: local-map matching
  * The data-parallel core of Mapper::matchToMap(frame, fmaxprojerr, fdistratio, set_local_lmids)
  * (/root/reference/src/mapper.cpp:576-774): for every candidate map point of the local map (cand_mp, in the caller's

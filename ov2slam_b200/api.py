@@ -4,6 +4,7 @@ This is the Python-side mirror of the reference's operator interface for the hot
 
     FeatureTracker.fb_klt_tracking   <- FeatureTracker::fbKltTracking   (feature_tracker.cpp:35-137)
     FeatureTracker.klt_tracking      <- VisualFrontEnd::kltTracking     (visual_front_end.cpp:132-275)
+    FeatureTracker.stereo_matching   <- MapManager::stereoMatching      (map_manager.cpp:367-611)
     FeatureExtractor.detect_grid_fast<- FeatureExtractor::detectGridFAST(feature_extractor.cpp:443-570)
     FeatureExtractor.describe_brief  <- FeatureExtractor::describeBRIEF (feature_extractor.cpp:224-285)
     Optimizer.local_ba               <- Optimizer::localBA solve part   (optimizer.cpp:436-735)
@@ -32,7 +33,7 @@ ABI_SYMBOLS = [
     "ov2_host_alloc", "ov2_host_free", "ov2_launch_count", "ov2_profile_enable", "ov2_profile_query",
     "ov2_pyr_create", "ov2_pyr_destroy", "ov2_pyr_build", "ov2_pyr_download", "ov2_clahe", "ov2_preprocess",
     "ov2_remap_create", "ov2_remap_destroy", "ov2_remap", "ov2_pyr_build_remap",
-    "ov2_fb_klt", "ov2_klt_tracking", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_debug_klt_counts", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
+    "ov2_fb_klt", "ov2_klt_tracking", "ov2_stereo_matching", "ov2_grid_fast", "ov2_detect_single_scale", "ov2_pnp_solve", "ov2_fast_cell_capacity", "ov2_debug_fast_cells", "ov2_debug_subpix_iters", "ov2_debug_klt_counts", "ov2_describe", "ov2_describe_config", "ov2_line_min_sad", "ov2_match_to_map", "ov2_frontend_step", "ov2_localba_solve", "ov2_localba_solve_batch", "ov2_localba_request_stop",
     "ov2_ba_comm_create", "ov2_ba_comm_handle", "ov2_ba_comm_connect", "ov2_ba_comm_connect_local", "ov2_ba_comm_destroy", "ov2_localba_solve_p2p",
 ]
 
@@ -131,6 +132,7 @@ def load():
     lib.ov2_fb_klt.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp]
     lib.ov2_klt_tracking.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32,
                                      vp, vp, vp, vp, vp, vp]
+    lib.ov2_stereo_matching.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, i32] + [vp] * 17 + [i32, i32, vp, vp, vp, vp]
     lib.ov2_debug_klt_counts.argtypes = [vp, vp, vp, C.POINTER(KltParams), i32, vp, i32, i32, vp, i32, vp, vp, vp, vp]
     lib.ov2_grid_fast.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, i32]
     lib.ov2_detect_single_scale.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, i32]
@@ -426,6 +428,49 @@ class FeatureTracker:
             self.ctx.h, prev.h_, cur.h_, C.byref(prm), int(first), count, offsets.ctypes.data, _ptr(Tcw), _ptr(K), _ptr(dist),
             _ptr(img_wh), _ptr(px), _ptr(wpt), _ptr(is3d), int(nklt_pyr_lvl), 1 if use_prior else 0, _ptr(out["tracked"]),
             _ptr(out["status"]), _ptr(out["passes"]), _ptr(out["p3p_req"]), _ptr(out["nbgood"]), _ptr(out["nbkps"])))
+        return out
+
+    def stereo_matching(self, left: Pyramid, right: Pyramid, nwinsize, nklt_pyr_lvl, ferr, fmax_fbklt_dist, rectified, offsets, Tcw,
+                        K, Trl, img_wh, px, unpx, bv, is3d, has_mp, wpt, dist=None, Frl=None, cell_offsets=None, grid=None,
+                        cell_ptr=None, cell_kps=None, first=0, out=None):
+        """MapManager::stereoMatching for keyframes [first, first + count) (ov2_stereo_matching).  offsets: int32[count + 1]
+        (host); per keyframe Tcw and Trl float64[count, 12] (row-major R, then t), the right camera's K float64[count, 4] and
+        dist float64[count, 5] or None, img_wh int32[count, 2] (right image), Frl float64[count, 9]; per keypoint px and unpx
+        float32[n, 2], bv and wpt float64[n, 3], is3d and has_mp uint8[n].  Other rigs pass the grid: cell_offsets int32[count
+        + 1] (host), grid int32[count, 2] (ncellsize, nbwcells), cell_ptr int32[cells + 1], cell_kps int32[n].  Inputs may be
+        numpy (host) or CUDA tensors (device).  Returns dict(right, stereo, passes, nstereo) as numpy arrays, or fills `out` (a
+        dict with those keys, host or device arrays) and returns it."""
+        offsets = np.ascontiguousarray(offsets, np.int32)
+        count = len(offsets) - 1
+        n = int(offsets[-1]) if count >= 0 else 0
+        if cell_offsets is not None:
+            cell_offsets = np.ascontiguousarray(cell_offsets, np.int32)
+        if out is None:
+            out = dict(right=np.zeros((n, 2), np.float32), stereo=np.zeros(n, np.uint8), passes=np.zeros(n, np.uint8),
+                       nstereo=np.zeros(count, np.int32))
+        prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
+
+        def typed(a, dt, name):
+            # numpy inputs are converted to the ABI's types; a tensor of another type is refused (its bytes would be misread)
+            if a is None:
+                return a
+            if isinstance(a, np.ndarray) or not hasattr(a, "data_ptr"):
+                return np.ascontiguousarray(a, dt)
+            if str(a.dtype) != "torch." + np.dtype(dt).name:
+                raise Ov2Error(f"stereo_matching: {name} must be {np.dtype(dt).name}, got {a.dtype}")
+            return a
+        f64 = [typed(a, np.float64, nm) for a, nm in ((Tcw, "Tcw"), (K, "K"), (dist, "dist"), (Trl, "Trl"), (Frl, "Frl"),
+                                                       (bv, "bv"), (wpt, "wpt"))]
+        Tcw, K, dist, Trl, Frl, bv, wpt = f64
+        img_wh, grid, cell_ptr, cell_kps = (typed(a, np.int32, nm) for a, nm in ((img_wh, "img_wh"), (grid, "grid"),
+                                                                                 (cell_ptr, "cell_ptr"), (cell_kps, "cell_kps")))
+        px, unpx = typed(px, np.float32, "px"), typed(unpx, np.float32, "unpx")
+        is3d, has_mp = typed(is3d, np.uint8, "is3d"), typed(has_mp, np.uint8, "has_mp")
+        self.ctx.check(self.ctx.lib.ov2_stereo_matching(
+            self.ctx.h, left.h_, right.h_, C.byref(prm), int(first), count, offsets.ctypes.data, _ptr(Tcw), _ptr(K), _ptr(dist),
+            _ptr(Trl), _ptr(Frl), _ptr(img_wh), _ptr(cell_offsets), _ptr(grid), _ptr(cell_ptr), _ptr(cell_kps), _ptr(px),
+            _ptr(unpx), _ptr(bv), _ptr(is3d), _ptr(has_mp), _ptr(wpt), 1 if rectified else 0, int(nklt_pyr_lvl),
+            _ptr(out["right"]), _ptr(out["stereo"]), _ptr(out["passes"]), _ptr(out["nstereo"])))
         return out
 
     def line_min_sad(self, left: Pyramid, right: Pyramid, level: int, pts, nwinsize, goleft, xprior_out, l1err_out,

@@ -25,6 +25,7 @@ SOURCES = {
     "frontend_pyr.cu": ["-fmad=false"],
     "frontend_klt.cu": ["-fmad=false"],
     "frontend_klt_tracking.cu": ["-fmad=false"],
+    "frontend_stereo_matching.cu": ["-fmad=false"],
     "frontend_fast.cu": ["-fmad=false"],
     "frontend_desc.cu": ["-fmad=false"],
     "frontend_clahe.cu": ["-fmad=false"],

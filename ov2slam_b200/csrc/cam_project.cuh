@@ -1,4 +1,5 @@
-// Projection of a world point into a frame, shared by match_map.cu and frontend_klt_tracking.cu.
+// Projection of a world point into a frame, shared by match_map.cu, frontend_klt_tracking.cu and frontend_stereo_matching.cu,
+// and the undistortion of a pixel.
 //
 // Frame::projWorldToCam (src/frame.cpp:811-828) with the pose as 12 doubles (row-major rotation, then the translation), and
 // CameraCalibration::projectCamToImageDist (src/camera_calibration.cpp:254-281) for the pinhole model, with or without
@@ -44,7 +45,34 @@ __device__ __forceinline__ float2 project_dist(const CamModel& C, double X, doub
     return make_float2((float)(xd * C.fx + C.cx), (float)(yd * C.fy + C.cy));
 }
 
-// Frame::isInImage (src/frame.cpp:840-843): float coordinates against the int image size
+// Frame::isInImage / isInRightImage (src/frame.cpp:840-848): float coordinates against the int image size
 __device__ __forceinline__ bool in_image(float2 p, int img_w, int img_h) {
     return p.x >= 0.f && p.y >= 0.f && p.x < (float)img_w && p.y < (float)img_h;
+}
+
+// CameraCalibration::undistortImagePoint (src/camera_calibration.cpp:313-332), pinhole model: the pixel itself without
+// distortion, else cv::undistortPoints(pt, K, D, K) as OpenCV evaluates it with its default criteria (5 iterations, no
+// tolerance test) and D = (k1, k2, p1, p2, k3): the rational and thin-prism coefficients are zero, the tilt matrix and
+// R are identities and P = K, so those terms add or multiply exact zeros and ones and are left out.  When the inverse
+// radial factor turns negative the point keeps its normalised pixel coordinates (OpenCV's icdist < 0 exit).
+// oracle/stereo_matching_ref.py::undistort_points_ref restates it; it equals cv2.undistortPoints bit for bit.
+__host__ __device__ inline float2 undistort_point(const CamModel& C, float u, float v) {
+    if (!C.has_dist) return make_float2(u, v);
+    const double ifx = 1. / C.fx, ify = 1. / C.fy;
+    const double x0 = ((double)u - C.cx) * ifx, y0 = ((double)v - C.cy) * ify;
+    double x = x0, y = y0;
+    for (int j = 0; j < 5; ++j) {
+        const double r2 = x * x + y * y;
+        const double icdist = 1. / (1 + ((C.k3 * r2 + C.k2) * r2 + C.k1) * r2);
+        if (icdist < 0) {
+            x = x0;
+            y = y0;
+            break;
+        }
+        const double dx = 2 * C.p1 * x * y + C.p2 * (r2 + 2 * x * x);
+        const double dy = C.p1 * (r2 + 2 * y * y) + 2 * C.p2 * x * y;
+        x = (x0 - dx) * icdist;
+        y = (y0 - dy) * icdist;
+    }
+    return make_float2((float)(C.fx * x + C.cx), (float)(C.fy * y + C.cy));
 }

@@ -152,6 +152,73 @@ def make_klt_tracking_scene(seed: int, counts, w: int = 640, h: int = 480, frac3
                 img_wh=np.tile(np.array([w, h], np.int32), (nf, 1)), px=px, wpt=wpt, is3d=is3d)
 
 
+def make_stereo_matching_scene(seed: int, counts, w: int = 320, h: int = 240, rectified: bool = True, distorted: bool = False,
+                               frac3d: float = 0.5, cs: int = 35, shifts=None):
+    """Keyframes for MapManager::stereoMatching (ov2_stereo_matching): keyframe k has counts[k] keypoints, a `frac3d` share of
+    them 3-D and 10 % of those without a map point.  The right image is the left one moved by shifts[k] = (dx, dy) px
+    (default: dx in [-8, 0], dy in [-2.5, 2.5], so the row search and the epipolar test both keep and reject), plus noise.
+    A 3-D keypoint's map point is placed so that it projects into the right image near px + shift, N(0, 0.7) px off, 20 %
+    of them 12 - 30 px off (pass 1 fails and pass 2 retries).  The rig: Trl = a small rotation (none when rectified) and a
+    0.11 m baseline; Frl = K^-T [t]x R K^-1 with the right camera's K for both.  The grid lists each keyframe's keypoints
+    by cell (ncellsize cs) in index order.  Returns a dict of the ov2_stereo_matching arrays plus lefts, rights."""
+    counts = [int(c) for c in counts]
+    nf = len(counts)
+    rng = np.random.default_rng(seed + 5_000_017)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    n = int(offsets[-1])
+    lefts, rights = np.empty((nf, h, w), np.uint8), np.empty((nf, h, w), np.uint8)
+    K = np.tile(np.array([458.654, 457.296, w / 2 + 7.215, h / 2 + 8.375]), (nf, 1))
+    dist = np.tile(np.array([-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05, 0.0]), (nf, 1)) if distorted else None
+    Tcw, Trl, Frl = np.zeros((nf, 12)), np.zeros((nf, 12)), np.zeros((nf, 9))
+    nbw, nbh = -(-w // cs), -(-h // cs)
+    cell_offsets = (np.arange(nf + 1) * nbw * nbh).astype(np.int32)
+    cell_ptr, cell_kps = [0], []
+    px = np.zeros((n, 2), np.float32)
+    wpt = np.zeros((n, 3))
+    bv = np.zeros((n, 3))
+    is3d = np.zeros(n, np.uint8)
+    has_mp = np.zeros(n, np.uint8)
+    for f in range(nf):
+        dx, dy = shifts[f] if shifts is not None else (rng.uniform(-8, 0), rng.uniform(-2.5, 2.5))
+        lefts[f] = make_frame(seed * 7 + f, w, h)
+        r = shift_image(lefts[f], dx, dy) + rng.normal(0.0, 2.0, (h, w))
+        rights[f] = np.clip(np.rint(r), 0, 255).astype(np.uint8)
+        Rm, t = _so3_exp(rng.normal(0, 0.3, 3)), rng.normal(0, 1.0, 3)
+        Tcw[f, :9], Tcw[f, 9:] = Rm.reshape(-1), t
+        Rrl = np.eye(3) if rectified else _so3_exp(rng.normal(0, 0.004, 3))
+        trl = np.array([-0.11, 0.0, 0.0]) if rectified else np.array([-0.11, 0.002, -0.001])
+        Trl[f, :9], Trl[f, 9:] = Rrl.reshape(-1), trl
+        Km = np.array([[K[f, 0], 0, K[f, 2]], [0, K[f, 1], K[f, 3]], [0, 0, 1.0]])
+        tx = np.array([[0, -trl[2], trl[1]], [trl[2], 0, -trl[0]], [-trl[1], trl[0], 0]])
+        Frl[f] = (np.linalg.inv(Km).T @ tx @ Rrl @ np.linalg.inv(Km)).reshape(-1)
+        sl = slice(offsets[f], offsets[f + 1])
+        m = counts[f]
+        px[sl] = np.stack([rng.uniform(4, w - 4, m), rng.uniform(4, h - 4, m)], 1)
+        b = np.stack([(px[sl, 0] - K[f, 2]) / K[f, 0], (px[sl, 1] - K[f, 3]) / K[f, 1], np.ones(m)], 1)
+        bv[sl] = b / np.linalg.norm(b, axis=1, keepdims=True)
+        is3d[sl] = rng.random(m) < frac3d
+        has_mp[sl] = is3d[sl] & (rng.random(m) > 0.1)
+        off = rng.normal(0, 0.7, (m, 2))
+        bad = rng.random(m) < 0.2
+        off[bad] = rng.uniform(12, 30, (int(bad.sum()), 2)) * rng.choice([-1, 1], (int(bad.sum()), 2))
+        q = px[sl].astype(np.float64) + np.array([dx, dy]) + off
+        zr = rng.uniform(2.0, 8.0, m)
+        cr = np.stack([(q[:, 0] - K[f, 2]) / K[f, 0] * zr, (q[:, 1] - K[f, 3]) / K[f, 1] * zr, zr], 1)
+        cl = (cr - trl) @ Rrl                                  # Rrl^T (c_right - t), row by row
+        wpt[sl] = (cl - t) @ Rm
+        cells = [[] for _ in range(nbw * nbh)]
+        for i in range(offsets[f], offsets[f + 1]):
+            cells[int(np.floor(px[i, 1] / np.float32(cs))) * nbw + int(np.floor(px[i, 0] / np.float32(cs)))].append(i)
+        for c in cells:
+            cell_kps += c
+            cell_ptr.append(len(cell_kps))
+    return dict(lefts=lefts, rights=rights, offsets=offsets, Tcw=Tcw, K=K, dist=dist, Trl=Trl, Frl=Frl,
+                img_wh=np.tile(np.array([w, h], np.int32), (nf, 1)), cell_offsets=cell_offsets,
+                grid=np.tile(np.array([cs, nbw], np.int32), (nf, 1)), cell_ptr=np.array(cell_ptr, np.int32),
+                cell_kps=np.array(cell_kps, np.int32), px=px, unpx=px.copy(), bv=bv, is3d=is3d, has_mp=has_mp, wpt=wpt,
+                rectified=int(rectified))
+
+
 # ----------------------------------------------------------------------------- local BA
 def _so3_exp(w: np.ndarray) -> np.ndarray:
     th = np.linalg.norm(w)
