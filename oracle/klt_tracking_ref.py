@@ -21,6 +21,8 @@ reference's own VisualFrontEnd::kltTracking is not compiled in place (DESIGN.md 
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 
 from oracle import image_ref as R
@@ -29,15 +31,15 @@ from oracle import match_ref as M
 f32 = np.float32
 
 
-def prior(T, K, dist, img_w: int, img_h: int, wpt):
-    """(x, y, in_image) of the world point's projection into the frame (float32 pixel)."""
-    X, Y, Z = M.camera_point(T, wpt)
-    if Z == 0.0:
-        return f32(np.nan), f32(np.nan), False
-    with np.errstate(over="ignore", invalid="ignore"):
+def prior(T, K, dist, img_w: int, img_h: int, pt):
+    """(x, y, in_image): the point through T into the camera K / dist (float32 pixel), and Frame::isInImage against the
+    img_w x img_h image.  stereo_matching_ref's right prior is the same with Trl and a camera point."""
+    X, Y, Z = M.camera_point(T, pt)
+    if Z == 0.0 or not all(math.isfinite(c) for c in (X, Y, Z)):
+        return f32(np.nan), f32(np.nan), False      # inf / nan in IEEE arithmetic, which no image contains
+    with np.errstate(all="ignore"):
         x, y = M.project_dist((X, Y, Z), K, dist)
-    inside = bool(x >= 0 and y >= 0 and x < f32(img_w) and y < f32(img_h))
-    return x, y, inside
+    return x, y, bool(x >= 0 and y >= 0 and x < f32(img_w) and y < f32(img_h))
 
 
 def klt_tracking_ref(prevs, curs, offsets, Tcw, K, img_wh, px, wpt, is3d, dist=None, win=9, nklt_pyr_lvl=3, use_prior=True,

@@ -2,10 +2,10 @@
 
 /root/reference/src/map_manager.cpp:367-611 restated per keyframe of a ragged batch, composed from the fbKltTracking oracle
 (image_ref.fb_klt_ref, or the same flow around cv2.calcOpticalFlowPyrLK), the getLineMinSAD oracle (image_ref.line_min_sad_ref),
-match_ref's projection and the two restatements below, every double formed in the kernel's order:
+klt_tracking_ref's projection and the two restatements below, every double formed in the kernel's order:
 
-  prior    a 3-D keypoint with a map point: Frame::projWorldToRightImageDist (src/frame.cpp:835-838), Tcw then Trl (each row
-           summed left to right) then match_ref.project_dist with the right camera; Frame::isInRightImage (:845-848).  A 3-D
+  prior    a 3-D keypoint with a map point: Frame::projWorldToRightImageDist (src/frame.cpp:835-838), Tcw then
+           right_prior (klt_tracking_ref.prior) through Trl with the right camera and Frame::isInRightImage (:845-848).  A 3-D
            keypoint without a map point is dropped: pass 0, no stereo.
   rect     the remaining keypoints' row search on level nklt_pyr_lvl (window 7, leftwards) at px * downpyrcoef; the column
            times uppyrcoef (float) replaces the prior's x iff 0 <= x <= px.x (:421-436).
@@ -29,15 +29,18 @@ branches (golden tests/golden/reference_map.npz, calls stereo_matching0 / stereo
 """
 from __future__ import annotations
 
-import math
-
 import numpy as np
 
 from oracle import image_ref as R
+from oracle import klt_tracking_ref as KT
 from oracle import match_ref as M
 
 f32 = np.float32
 SAD_WIN = 7
+
+# Frame::projCamToRightImageDist and isInRightImage: the camera point through Trl into the right camera, the projection and
+# in-image test of klt_tracking_ref.prior.
+right_prior = KT.prior
 
 
 def undistort_points_ref(u, v, K, dist):
@@ -77,16 +80,6 @@ def sampson_ref(F, l, r):
     x2, y2 = f32(F[0] * lx + F[1] * ly + F[2]), f32(F[3] * lx + F[4] * ly + F[5])
     den = x1 * x1 + y1 * y1 + x2 * x2 + y2 * y2
     return np.sqrt(num / den)
-
-
-def right_prior(Trl, K, dist, img_w, img_h, campt):
-    """(x, y, inside): the camera point through Trl into the right image (Frame::projCamToRightImageDist), isInRightImage."""
-    X, Y, Z = M.camera_point(Trl, campt)
-    if Z == 0.0 or not all(math.isfinite(c) for c in (X, Y, Z)):
-        return f32(np.nan), f32(np.nan), False      # inf / nan in IEEE arithmetic, which no image contains
-    with np.errstate(all="ignore"):
-        x, y = M.project_dist((X, Y, Z), K, dist)
-    return x, y, bool(x >= 0 and y >= 0 and x < f32(img_w) and y < f32(img_h))
 
 
 def neighbour_depth(f, i, o0, o1, Tcw, px, unpx, is3d, has_mp, wpt, cell_offsets, grid, cell_ptr, cell_kps):

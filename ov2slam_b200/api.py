@@ -177,6 +177,18 @@ def _ptr(a):
     raise Ov2Error(f"unsupported array type {type(a)}")
 
 
+def _typed(a, dt, name, fn):
+    """An input of ABI type dt: numpy inputs are converted; a tensor of another type is refused (its bytes would be
+    misread); None and an int (a raw address, as _ptr takes it) pass through."""
+    if a is None or isinstance(a, int):
+        return a
+    if isinstance(a, np.ndarray) or not hasattr(a, "data_ptr"):
+        return np.ascontiguousarray(a, dt)
+    if str(a.dtype) != "torch." + np.dtype(dt).name:
+        raise Ov2Error(f"{fn}: {name} must be {np.dtype(dt).name}, got {a.dtype}")
+    return a
+
+
 class Context:
     """ov2_ctx: one CUDA device + stream + scratch arena.  Not re-entrant."""
 
@@ -375,6 +387,9 @@ class FeatureTracker:
         self.nmax_iter = nmax_iter
         self.fmax_px_precision = float(np.float32(fmax_px_precision))
 
+    def _params(self, nwinsize, ferr, fmax_fbklt_dist):
+        return KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
+
     def fb_klt_tracking(self, prev: Pyramid, cur: Pyramid, nwinsize, nbpyrlvl, ferr, fmax_fbklt_dist,
                         kps, priors_inout, status_out, n=None, frame_idx=None, first_frame=0, per_frame=None, counts_out=None):
         """fbKltTracking over a (ragged or fixed-stride) batch.  nwinsize: 3 .. 31, even sizes included (Ov2Error
@@ -384,7 +399,7 @@ class FeatureTracker:
         counting kernel, which also returns each keypoint's level set-ups and iterations (forward + backward)."""
         if n is None:
             n = int(kps.shape[0])
-        prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
+        prm = self._params(nwinsize, ferr, fmax_fbklt_dist)
         if isinstance(nbpyrlvl, (int, np.integer)) and int(nbpyrlvl) < 64:
             lv_ptr, lv_all = None, int(nbpyrlvl)       # a pyramid depth; larger ints are raw addresses
         else:
@@ -411,19 +426,10 @@ class FeatureTracker:
         if out is None:
             out = dict(tracked=np.zeros((n, 2), np.float32), status=np.zeros(n, np.uint8), passes=np.zeros(n, np.uint8),
                        p3p_req=np.zeros(count, np.uint8), nbgood=np.zeros(count, np.int32), nbkps=np.zeros(count, np.int32))
-        prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
-
-        def typed(a, dt, name):
-            # numpy inputs are converted to the ABI's types; a tensor of another type is refused (its bytes would be misread)
-            if a is None or isinstance(a, int):
-                return a
-            if isinstance(a, np.ndarray) or not hasattr(a, "data_ptr"):
-                return np.ascontiguousarray(a, dt)
-            if str(a.dtype) != "torch." + np.dtype(dt).name:
-                raise Ov2Error(f"klt_tracking: {name} must be {np.dtype(dt).name}, got {a.dtype}")
-            return a
-        Tcw, K, dist, wpt = (typed(a, np.float64, nm) for a, nm in ((Tcw, "Tcw"), (K, "K"), (dist, "dist"), (wpt, "wpt")))
-        img_wh, px, is3d = typed(img_wh, np.int32, "img_wh"), typed(px, np.float32, "px"), typed(is3d, np.uint8, "is3d")
+        prm = self._params(nwinsize, ferr, fmax_fbklt_dist)
+        Tcw, K, dist, wpt, img_wh, px, is3d = (_typed(a, dt, nm, "klt_tracking") for a, dt, nm in (
+            (Tcw, np.float64, "Tcw"), (K, np.float64, "K"), (dist, np.float64, "dist"), (wpt, np.float64, "wpt"),
+            (img_wh, np.int32, "img_wh"), (px, np.float32, "px"), (is3d, np.uint8, "is3d")))
         self.ctx.check(self.ctx.lib.ov2_klt_tracking(
             self.ctx.h, prev.h_, cur.h_, C.byref(prm), int(first), count, offsets.ctypes.data, _ptr(Tcw), _ptr(K), _ptr(dist),
             _ptr(img_wh), _ptr(px), _ptr(wpt), _ptr(is3d), int(nklt_pyr_lvl), 1 if use_prior else 0, _ptr(out["tracked"]),
@@ -448,24 +454,13 @@ class FeatureTracker:
         if out is None:
             out = dict(right=np.zeros((n, 2), np.float32), stereo=np.zeros(n, np.uint8), passes=np.zeros(n, np.uint8),
                        nstereo=np.zeros(count, np.int32))
-        prm = KltParams(int(nwinsize), int(self.nmax_iter), self.fmax_px_precision, float(ferr), float(fmax_fbklt_dist))
-
-        def typed(a, dt, name):
-            # numpy inputs are converted to the ABI's types; a tensor of another type is refused (its bytes would be misread)
-            if a is None:
-                return a
-            if isinstance(a, np.ndarray) or not hasattr(a, "data_ptr"):
-                return np.ascontiguousarray(a, dt)
-            if str(a.dtype) != "torch." + np.dtype(dt).name:
-                raise Ov2Error(f"stereo_matching: {name} must be {np.dtype(dt).name}, got {a.dtype}")
-            return a
-        f64 = [typed(a, np.float64, nm) for a, nm in ((Tcw, "Tcw"), (K, "K"), (dist, "dist"), (Trl, "Trl"), (Frl, "Frl"),
-                                                       (bv, "bv"), (wpt, "wpt"))]
-        Tcw, K, dist, Trl, Frl, bv, wpt = f64
-        img_wh, grid, cell_ptr, cell_kps = (typed(a, np.int32, nm) for a, nm in ((img_wh, "img_wh"), (grid, "grid"),
-                                                                                 (cell_ptr, "cell_ptr"), (cell_kps, "cell_kps")))
-        px, unpx = typed(px, np.float32, "px"), typed(unpx, np.float32, "unpx")
-        is3d, has_mp = typed(is3d, np.uint8, "is3d"), typed(has_mp, np.uint8, "has_mp")
+        prm = self._params(nwinsize, ferr, fmax_fbklt_dist)
+        Tcw, K, dist, Trl, Frl, bv, wpt = (_typed(a, np.float64, nm, "stereo_matching") for a, nm in (
+            (Tcw, "Tcw"), (K, "K"), (dist, "dist"), (Trl, "Trl"), (Frl, "Frl"), (bv, "bv"), (wpt, "wpt")))
+        img_wh, grid, cell_ptr, cell_kps, px, unpx, is3d, has_mp = (_typed(a, dt, nm, "stereo_matching") for a, dt, nm in (
+            (img_wh, np.int32, "img_wh"), (grid, np.int32, "grid"), (cell_ptr, np.int32, "cell_ptr"),
+            (cell_kps, np.int32, "cell_kps"), (px, np.float32, "px"), (unpx, np.float32, "unpx"), (is3d, np.uint8, "is3d"),
+            (has_mp, np.uint8, "has_mp")))
         self.ctx.check(self.ctx.lib.ov2_stereo_matching(
             self.ctx.h, left.h_, right.h_, C.byref(prm), int(first), count, offsets.ctypes.data, _ptr(Tcw), _ptr(K), _ptr(dist),
             _ptr(Trl), _ptr(Frl), _ptr(img_wh), _ptr(cell_offsets), _ptr(grid), _ptr(cell_ptr), _ptr(cell_kps), _ptr(px),

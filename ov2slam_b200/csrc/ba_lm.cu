@@ -1854,7 +1854,7 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
         OV2_CUDA(ctx, cudaHostAlloc(&ctx->ba_ws, host_need * 2, cudaHostAllocDefault));
         ctx->ba_ws_cap = host_need * 2;
     }
-    void *dup = nullptr, *dwork = nullptr, *o = nullptr;
+    void *dup = nullptr, *dwork = nullptr;
     if ((st = ov2_scratch(ctx, in_bytes, &dup)) != OV2_OK) return st;
     if ((st = ov2_scratch(ctx, L.work_bytes() + 256, &dwork)) != OV2_OK) return st;
     L.place((char*)dup, (char*)dwork, (char*)ctx->ba_ws);
@@ -1936,8 +1936,8 @@ ov2_status balm_solve(ov2_ctx* ctx, int nprob, const ov2_ba_problem* pbs, const 
     // the Prob records must be contiguous for the kernel: they are the first thing of each window's block, so gather them
     std::vector<Prob> parr(nprob);
     for (int k = 0; k < nprob; ++k) memcpy(&parr[k], L.h(plans[k].prob), sizeof(Prob));
-    if ((st = ov2_scratch(ctx, sizeof(Prob) * (size_t)nprob, &o)) != OV2_OK) return st;
-    Prob* dprobs = (Prob*)o;
+    Prob* dprobs = nullptr;
+    if ((st = ov2_scratch(ctx, (size_t)nprob, dprobs)) != OV2_OK) return st;
     cudaStream_t s = ctx->stream;
     OV2_CUDA(ctx, cudaMemcpyAsync(L.dev[RG_STATE], L.host[RG_STATE], in_bytes, cudaMemcpyHostToDevice, s));
     if (nprob == 1) dprobs = (Prob*)L.d(plans[0].prob);

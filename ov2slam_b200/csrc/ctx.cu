@@ -256,6 +256,30 @@ extern "C" ov2_status ov2_batch_end(ov2_ctx* ctx) {
     return ov2_wait_stream(ctx);
 }
 
+ov2_status ov2_in_batch(ov2_ctx* ctx, const std::function<ov2_status()>& enqueue) {
+    const bool own_batch = !ctx->batch;
+    ov2_status st = own_batch ? ov2_batch_begin(ctx) : ov2_begin(ctx);
+    if (st != OV2_OK) return st;
+    st = enqueue();
+    if (!own_batch) return st;
+    ctx->batch = false;
+    if (st != OV2_OK) {
+        ctx->pending.clear();
+        return st;
+    }
+    if (ctx->pending.empty()) return OV2_OK;
+    if ((st = ov2_batch_flush_outputs(ctx)) != OV2_OK) return st;
+    return ov2_wait_stream(ctx);
+}
+
+ov2_offsets_check ov2_check_offsets(const int32_t* t, int count) {
+    if (ov2_is_device_ptr(t)) return OV2_OFFSETS_ON_DEVICE;
+    if (t[0] != 0) return OV2_OFFSETS_NOT_ASCENDING;
+    for (int k = 0; k < count; ++k)
+        if (t[k + 1] < t[k]) return OV2_OFFSETS_NOT_ASCENDING;
+    return OV2_OFFSETS_OK;
+}
+
 // ------------------------------------------------------------------------ pyramid storage
 extern "C" ov2_status ov2_pyr_create(ov2_ctx* ctx, int batch, int width, int height, int nlevels_extra,
                                      ov2_pyr** out) {

@@ -243,10 +243,8 @@ static ov2_status clahe_device(ov2_ctx* ctx, const uint8_t* src, int spitch, lon
     A.lut_scale = (float)255 / (float)area;
     A.inv_tw = 1.0f / (float)A.tw;
     A.inv_th = 1.0f / (float)A.th;
-    void* o = nullptr;
     ov2_status st;
-    if ((st = ov2_scratch(ctx, (size_t)count * tiles_x * tiles_y * 256, &o)) != OV2_OK) return st;
-    A.lut = (uint8_t*)o;
+    if ((st = ov2_scratch(ctx, (size_t)count * tiles_x * tiles_y * 256, A.lut)) != OV2_OK) return st;
     OV2_LAUNCH(ctx, "clahe_lut_kernel", clahe_lut_kernel<<<dim3((tiles_x * tiles_y + LUT_WARPS - 1) / LUT_WARPS, count), LUT_WARPS * 32, 0, ctx->stream>>>(A));
     if (tiles_x > APPLY_MAX_TX) return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_clahe: more than 64 tile columns");
     {
@@ -268,14 +266,14 @@ extern "C" ov2_status ov2_clahe(ov2_ctx* ctx, const uint8_t* src, uint8_t* dst, 
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
     const size_t bytes = frame_stride * (size_t)(count - 1) + row_stride * (size_t)(height - 1) + (size_t)width;
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, src, bytes, &d)) != OV2_OK) return st;
+    const uint8_t* d = nullptr;
+    uint8_t* o = nullptr;
+    if ((st = ov2_stage_in(ctx, src, bytes, d)) != OV2_OK) return st;
     // a host dst is copied back over the whole span: when rows or frames leave gaps (a ROI of a wider image), stage its
     // current bytes first so the gaps come back unchanged
     const bool gaps = row_stride != (size_t)width || (count > 1 && frame_stride != row_stride * (size_t)height);
-    if ((st = ov2_stage_out(ctx, dst, bytes, &o, gaps)) != OV2_OK) return st;
-    if ((st = clahe_device(ctx, (const uint8_t*)d, (int)row_stride, (long long)frame_stride, (uint8_t*)o, (int)row_stride,
+    if ((st = ov2_stage_out(ctx, dst, bytes, o, gaps)) != OV2_OK) return st;
+    if ((st = clahe_device(ctx, d, (int)row_stride, (long long)frame_stride, o, (int)row_stride,
                            (long long)frame_stride, width, height, count, clip_limit, tiles_x, tiles_y)) != OV2_OK)
         return st;
     return ov2_end(ctx);

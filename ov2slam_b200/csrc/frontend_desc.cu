@@ -397,16 +397,10 @@ extern "C" ov2_status ov2_describe(ov2_ctx* ctx, const ov2_pyr* pyr, int n, cons
     DescArgs A;
     A.img = pyr->l0; A.w = pyr->w[0]; A.h = pyr->h[0]; A.pitch = (int)pyr->l0_pitch; A.fstride = (long long)pyr->l0_fstride;
     A.n = n; A.first_frame = first_frame; A.per_frame = per_frame;
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, frame_idx, sizeof(int32_t) * (size_t)n, &d)) != OV2_OK) return st;
-    A.frame_idx = (const int32_t*)d;
-    if ((st = ov2_stage_in(ctx, pts, sizeof(float) * 2 * (size_t)n, &d)) != OV2_OK) return st;
-    A.pts = (const float2*)d;
-    if ((st = ov2_stage_out(ctx, desc32_out, (size_t)32 * n, &o)) != OV2_OK) return st;
-    A.desc = (uint8_t*)o;
-    if ((st = ov2_stage_out(ctx, valid_out, (size_t)n, &o)) != OV2_OK) return st;
-    A.valid = (uint8_t*)o;
+    if ((st = ov2_stage_in(ctx, frame_idx, (size_t)n, A.frame_idx)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, pts, (size_t)n, A.pts)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, desc32_out, (size_t)32 * n, A.desc)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, valid_out, (size_t)n, A.valid)) != OV2_OK) return st;
     if (ctx->desc_mode == OV2_DESC_BRIEF32) {
         BoxArgs B;
         B.d = A;
@@ -418,15 +412,15 @@ extern "C" ov2_status ov2_describe(ov2_ctx* ctx, const ov2_pyr* pyr, int n, cons
         D.d = A;
         D.ppitch = (A.w + 15) & ~15;
         D.pfstride = (long long)D.ppitch * A.h;
-        void* pl = nullptr;
-        if ((st = ov2_scratch(ctx, (size_t)D.pfstride * nframes, &pl)) != OV2_OK) return st;
-        D.plane = (const uint8_t*)pl;
+        uint8_t* pl = nullptr;
+        if ((st = ov2_scratch(ctx, (size_t)D.pfstride * nframes, pl)) != OV2_OK) return st;
+        D.plane = pl;
         SmoothArgs S;
         S.img = A.img; S.pitch = A.pitch; S.fstride = A.fstride;
         S.first_frame = first_frame; S.h = A.h;
         S.ncs = div_up(A.w - 34, SMOOTH_COLS);
         S.nrs = div_up(A.h - 36, SMOOTH_ROWS);
-        S.plane = (uint8_t*)pl; S.ppitch = D.ppitch; S.pfstride = D.pfstride;
+        S.plane = pl; S.ppitch = D.ppitch; S.pfstride = D.pfstride;
         OV2_LAUNCH(ctx, "desc_smooth_kernel",
                    desc_smooth_kernel<<<dim3(div_up(S.ncs * S.nrs, SMOOTH_THREADS), nframes), SMOOTH_THREADS, 0, ctx->stream>>>(S));
         OV2_LAUNCH(ctx, "describe_dense_kernel", describe_dense_kernel<<<div_up(n, WARPS), WARPS * 32, 0, ctx->stream>>>(D));

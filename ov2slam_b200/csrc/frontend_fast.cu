@@ -645,32 +645,26 @@ extern "C" ov2_status ov2_grid_fast(ov2_ctx* ctx, const ov2_pyr* pyr, int first,
         return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_grid_fast: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-    DetectArgs D;
-    if ((st = stage_detect_args(ctx, "ov2_grid_fast", count, max_per_frame, curkp_offsets, curkps, fast_th_inout, sizeof(int32_t),
-                                out_pts, out_counts, out_pts_int, &D)) != OV2_OK)
+    DetectArgs<int32_t> D;
+    if ((st = stage_detect_args(ctx, "ov2_grid_fast", count, max_per_frame, curkp_offsets, curkps, fast_th_inout, out_pts,
+                                out_counts, out_pts_int, &D)) != OV2_OK)
         return st;
-    void* o = nullptr;
     uint32_t* d_cand = nullptr;
     int32_t* d_candn = nullptr;
-    if ((st = ov2_scratch(ctx, sizeof(uint32_t) * (size_t)count * ncells * cap, &o)) != OV2_OK) return st;
-    d_cand = (uint32_t*)o;
-    if ((st = ov2_scratch(ctx, sizeof(int32_t) * (size_t)count * ncells, &o)) != OV2_OK) return st;
-    d_candn = (int32_t*)o;
+    if ((st = ov2_scratch(ctx, (size_t)count * ncells * cap, d_cand)) != OV2_OK) return st;
+    if ((st = ov2_scratch(ctx, (size_t)count * ncells, d_candn)) != OV2_OK) return st;
     int* d_skey = nullptr;      // sort keys of the cells with more candidates than the sweep keeps in registers
-    if (cap > WAVE_REG_CAND) {
-        if ((st = ov2_scratch(ctx, sizeof(int) * (size_t)count * nw * cap, &o)) != OV2_OK) return st;
-        d_skey = (int*)o;
-    }
+    if (cap > WAVE_REG_CAND && (st = ov2_scratch(ctx, (size_t)count * nw * cap, d_skey)) != OV2_OK) return st;
 
     FastArgs FA;
     FA.img = pyr->l0; FA.w = W; FA.h = H; FA.pitch = (int)pyr->l0_pitch; FA.fstride = (long long)pyr->l0_fstride;
     FA.first = first; FA.cs = cellsize; FA.nwc = nwc; FA.nhc = nhc; FA.cap = cap;
-    FA.th = (int32_t*)D.state; FA.cand = d_cand; FA.cand_n = d_candn;
+    FA.th = D.state; FA.cand = d_cand; FA.cand_n = d_candn;
     if ((st = launch_fast_cells(ctx, pyr, FA, count)) != OV2_OK) return st;
     SweepArgs SA;
     gsweep::init_base(SA, W, H, cellsize, D.kp_off, D.kps);
     SA.cap = cap; SA.max_per_frame = max_per_frame; SA.skey_g = d_skey;
-    SA.cand = d_cand; SA.cand_n = d_candn; SA.th = (int32_t*)D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
+    SA.cand = d_cand; SA.cand_n = d_candn; SA.th = D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
     static size_t smem_attr[16] = {0};
     if (smem > 48 * 1024 && smem > smem_attr[ctx->device & 15]) {
         OV2_CUDA(ctx, cudaFuncSetAttribute(fast_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -699,18 +693,15 @@ extern "C" ov2_status ov2_debug_fast_cells(ov2_ctx* ctx, const ov2_pyr* pyr, int
     if (cap_in < cap) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_debug_fast_cells: cap_in too small");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-    void* o = nullptr;
     FastArgs FA;
     FA.img = pyr->l0; FA.w = W; FA.h = H; FA.pitch = (int)pyr->l0_pitch; FA.fstride = (long long)pyr->l0_fstride;
     FA.first = frame; FA.cs = cellsize; FA.nwc = nwc; FA.nhc = nhc; FA.cap = cap;
-    if ((st = ov2_scratch(ctx, sizeof(int32_t), &o)) != OV2_OK) return st;
-    int32_t* d_th = (int32_t*)o;
+    int32_t* d_th = nullptr;
+    if ((st = ov2_scratch(ctx, 1, d_th)) != OV2_OK) return st;
     OV2_CUDA(ctx, cudaMemcpyAsync(d_th, &fast_th, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
     FA.th = d_th;
-    if ((st = ov2_stage_out(ctx, cand_out, sizeof(uint32_t) * (size_t)ncells * cap, &o)) != OV2_OK) return st;
-    FA.cand = (uint32_t*)o;
-    if ((st = ov2_stage_out(ctx, cand_n_out, sizeof(int32_t) * (size_t)ncells, &o)) != OV2_OK) return st;
-    FA.cand_n = (int32_t*)o;
+    if ((st = ov2_stage_out(ctx, cand_out, (size_t)ncells * cap, FA.cand)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, cand_n_out, (size_t)ncells, FA.cand_n)) != OV2_OK) return st;
     if ((st = launch_fast_cells(ctx, pyr, FA, 1)) != OV2_OK) return st;
     return ov2_end(ctx);
 }
@@ -741,13 +732,12 @@ extern "C" ov2_status ov2_debug_subpix_iters(ov2_ctx* ctx, const ov2_pyr* pyr, i
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
     const size_t n = (size_t)count * max_per_frame;
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, pts_int, sizeof(int32_t) * 2 * n, &d)) != OV2_OK) return st;
-    const int2* d_int = (const int2*)d;
-    if ((st = ov2_stage_out(ctx, out_pts, sizeof(float) * 2 * n, &o)) != OV2_OK) return st;
-    float2* d_out = (float2*)o;
-    if ((st = ov2_stage_out(ctx, iters_out, sizeof(int32_t) * n, &o)) != OV2_OK) return st;
-    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, 1, (int32_t*)o)) != OV2_OK) return st;
+    const int2* d_int = nullptr;
+    float2* d_out = nullptr;
+    int32_t* d_iters = nullptr;
+    if ((st = ov2_stage_in(ctx, pts_int, n, d_int)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, out_pts, n, d_out)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, iters_out, n, d_iters)) != OV2_OK) return st;
+    if ((st = ov2_subpix_launch(ctx, pyr, first, count, max_per_frame, d_int, d_out, 1, d_iters)) != OV2_OK) return st;
     return ov2_end(ctx);
 }

@@ -473,10 +473,8 @@ ov2_status klt_run(ov2_ctx* ctx, KltArgs& A, int n, int32_t* d_counts, int win) 
     OV2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fb_klt_kernel<false, Win>, threads, 0));
     const int resident = per_sm * ctx->sm_count;
     if (grid > resident) {
-        void* o = nullptr;
-        const ov2_status st = ov2_scratch(ctx, sizeof(int), &o);
+        const ov2_status st = ov2_scratch(ctx, 1, A.work_counter);
         if (st != OV2_OK) return st;
-        A.work_counter = (int*)o;
         OV2_CUDA(ctx, cudaMemsetAsync(A.work_counter, 0, sizeof(int), ctx->stream));
         grid = resident;
     }
@@ -497,8 +495,7 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: null array");
     if (prm->win < 3 || prm->win > kltsetup::WMAX)
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: nwinsize must be 3 .. 31");
-    if (prev->nlev != cur->nlev || prev->w[0] != cur->w[0] || prev->h[0] != cur->h[0] || !prev->l0 || !cur->l0)
-        return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: pyramids not built / mismatched");
+    if (!ov2_pyr_pair_ok(prev, cur)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: pyramids not built / mismatched");
     if (!frame_idx && (first_frame < 0 || first_frame + (n + per_frame - 1) / per_frame > prev->batch))
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_fb_klt: more frames than pyramid slots");
     ov2_status st = ov2_begin(ctx);
@@ -519,23 +516,13 @@ ov2_status klt_launch(ov2_ctx* ctx, const ov2_pyr* prev, const ov2_pyr* cur, con
     A.eig_q = kltsetup::klt_eig_q(prm->win, LK_MIN_EIG);
     A.ferr_q = kltsetup::klt_ferr_q(prm->win, prm->ferr);
     A.fb_s = kltsetup::klt_fb_s(prm->fb_dist);
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, frame_idx, sizeof(int32_t) * (size_t)n, &d)) != OV2_OK) return st;
-    A.frame_idx = (const int32_t*)d;
-    if ((st = ov2_stage_in(ctx, nbpyrlvl, (size_t)n, &d)) != OV2_OK) return st;
-    A.lvls = (const uint8_t*)d;
-    if ((st = ov2_stage_in(ctx, kps, sizeof(float) * 2 * (size_t)n, &d)) != OV2_OK) return st;
-    A.kps = (const float2*)d;
-    if ((st = ov2_stage_out(ctx, priors_inout, sizeof(float) * 2 * (size_t)n, &o, true)) != OV2_OK) return st;
-    A.priors = (float2*)o;
-    if ((st = ov2_stage_out(ctx, status_out, (size_t)n, &o)) != OV2_OK) return st;
-    A.status = (uint8_t*)o;
+    if ((st = ov2_stage_in(ctx, frame_idx, (size_t)n, A.frame_idx)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, nbpyrlvl, (size_t)n, A.lvls)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, kps, (size_t)n, A.kps)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, priors_inout, (size_t)n, A.priors, true)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, status_out, (size_t)n, A.status)) != OV2_OK) return st;
     int32_t* d_counts = nullptr;
-    if (counts_out) {
-        if ((st = ov2_stage_out(ctx, counts_out, sizeof(int32_t) * 2 * (size_t)n, &o)) != OV2_OK) return st;
-        d_counts = (int32_t*)o;
-    }
+    if (counts_out && (st = ov2_stage_out(ctx, counts_out, 2 * (size_t)n, d_counts)) != OV2_OK) return st;
     // 9 x 9 (every shipped configuration) keeps its own layout; every other size runs the general one
     st = prm->win == 9 ? klt_run<Win9>(ctx, A, n, d_counts, prm->win) : klt_run<WinAny>(ctx, A, n, d_counts, prm->win);
     if (st != OV2_OK) return st;

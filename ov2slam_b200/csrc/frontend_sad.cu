@@ -160,16 +160,10 @@ extern "C" ov2_status ov2_line_min_sad(ov2_ctx* ctx, const ov2_pyr* left, const 
     A.per_frame = per_frame;
     A.nwinsize = nwinsize;
     A.goleft = goleft ? 1 : 0;
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, frame_idx, sizeof(int32_t) * (size_t)n, &d)) != OV2_OK) return st;
-    A.frame_idx = (const int32_t*)d;
-    if ((st = ov2_stage_in(ctx, pts, sizeof(float) * 2 * (size_t)n, &d)) != OV2_OK) return st;
-    A.pts = (const float2*)d;
-    if ((st = ov2_stage_out(ctx, xprior_out, sizeof(float) * (size_t)n, &o)) != OV2_OK) return st;
-    A.xprior = (float*)o;
-    if ((st = ov2_stage_out(ctx, l1err_out, sizeof(float) * (size_t)n, &o)) != OV2_OK) return st;
-    A.l1err = (float*)o;
+    if ((st = ov2_stage_in(ctx, frame_idx, (size_t)n, A.frame_idx)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, pts, (size_t)n, A.pts)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, xprior_out, (size_t)n, A.xprior)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, l1err_out, (size_t)n, A.l1err)) != OV2_OK) return st;
     OV2_LAUNCH(ctx, "line_min_sad_kernel", line_min_sad_kernel<<<div_up(n, WARPS), WARPS * 32, 0, ctx->stream>>>(A));
     return ov2_end(ctx);
 }

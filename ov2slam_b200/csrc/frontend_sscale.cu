@@ -272,16 +272,15 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
         return ov2_fail(ctx, OV2_ERR_CAPACITY, "ov2_detect_single_scale: image too large for the shared-memory mask bitmap");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
-    DetectArgs D;
-    if ((st = stage_detect_args(ctx, "ov2_detect_single_scale", count, max_per_frame, curkp_offsets, curkps, quality_inout,
-                                sizeof(double), out_pts, out_counts, out_pts_int, &D)) != OV2_OK)
+    DetectArgs<double> D;
+    if ((st = stage_detect_args(ctx, "ov2_detect_single_scale", count, max_per_frame, curkp_offsets, curkps, quality_inout, out_pts,
+                                out_counts, out_pts_int, &D)) != OV2_OK)
         return st;
-    void* o = nullptr;
     const size_t cell_px = (size_t)cellsize * cellsize;
-    if ((st = ov2_scratch(ctx, sizeof(float) * (size_t)count * ncells * cell_px, &o)) != OV2_OK) return st;
-    float* d_resp = (float*)o;
-    if ((st = ov2_scratch(ctx, sizeof(float2) * (size_t)count * ncells, &o)) != OV2_OK) return st;
-    float2* d_cellmax = (float2*)o;
+    float* d_resp = nullptr;
+    float2* d_cellmax = nullptr;
+    if ((st = ov2_scratch(ctx, (size_t)count * ncells * cell_px, d_resp)) != OV2_OK) return st;
+    if ((st = ov2_scratch(ctx, (size_t)count * ncells, d_cellmax)) != OV2_OK) return st;
 
     RespArgs RA;
     RA.img = pyr->l0; RA.w = W; RA.h = H; RA.pitch = (int)pyr->l0_pitch; RA.fstride = (long long)pyr->l0_fstride;
@@ -296,7 +295,7 @@ extern "C" ov2_status ov2_detect_single_scale(ov2_ctx* ctx, const ov2_pyr* pyr, 
     gsweep::init_base(SA, W, H, cellsize, D.kp_off, D.kps);
     SA.max_per_frame = max_per_frame;
     SA.roi_x = roi[0]; SA.roi_y = roi[1]; SA.roi_w = roi[2]; SA.roi_h = roi[3];
-    SA.resp = d_resp; SA.cellmax = d_cellmax; SA.quality = (double*)D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
+    SA.resp = d_resp; SA.cellmax = d_cellmax; SA.quality = D.state; SA.out_int = D.ints; SA.out_n = D.cnt;
     if (sweep_smem > 48 * 1024)
         OV2_CUDA(ctx, cudaFuncSetAttribute(ss_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sweep_smem));
     OV2_LAUNCH(ctx, "ss_sweep_kernel", ss_sweep_kernel<<<count, nw * 32, sweep_smem, ctx->stream>>>(SA));

@@ -152,10 +152,11 @@ ov2_status ov2_subpix_launch(ov2_ctx* ctx, const ov2_pyr* pyr, int first, int co
                              float2* d_out, int do_subpix, int32_t* d_iters);
 
 // Device pointers of the arguments ov2_grid_fast and ov2_detect_single_scale share.
+template <class State>
 struct DetectArgs {
     const int32_t* kp_off = nullptr;   // NULL: no existing keypoints
     const float2* kps = nullptr;
-    void* state = nullptr;             // per-frame in/out state (FAST threshold, single-scale quality)
+    State* state = nullptr;            // per-frame in/out state (FAST threshold, single-scale quality)
     float2* out = nullptr;             // [count][max_per_frame] refined points
     int32_t* cnt = nullptr;            // [count]
     int2* ints = nullptr;              // [count][max_per_frame] integer points: the caller's out_pts_int or scratch
@@ -163,15 +164,13 @@ struct DetectArgs {
 
 // Stages the shared arguments of a detector call (`what` names it in errors).  The number of existing keypoints is
 // offsets[count], read back first when the offsets are on the device.
-inline ov2_status stage_detect_args(ov2_ctx* ctx, const char* what, int count, int max_per_frame, const int32_t* curkp_offsets,
-                                    const float* curkps, void* state_inout, size_t state_bytes, float* out_pts,
-                                    int32_t* out_counts, int32_t* out_pts_int, DetectArgs* D) {
+template <class State>
+ov2_status stage_detect_args(ov2_ctx* ctx, const char* what, int count, int max_per_frame, const int32_t* curkp_offsets,
+                             const float* curkps, State* state_inout, float* out_pts, int32_t* out_counts, int32_t* out_pts_int,
+                             DetectArgs<State>* D) {
     ov2_status st;
-    const void* d = nullptr;
-    void* o = nullptr;
     if (curkp_offsets) {
-        if ((st = ov2_stage_in(ctx, curkp_offsets, sizeof(int32_t) * (size_t)(count + 1), &d)) != OV2_OK) return st;
-        D->kp_off = (const int32_t*)d;
+        if ((st = ov2_stage_in(ctx, curkp_offsets, (size_t)(count + 1), D->kp_off)) != OV2_OK) return st;
         int nkp_total = 0;
         if (ov2_is_device_ptr(curkp_offsets)) {
             OV2_CUDA(ctx, cudaMemcpyAsync(&nkp_total, curkp_offsets + count, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -181,17 +180,12 @@ inline ov2_status stage_detect_args(ov2_ctx* ctx, const char* what, int count, i
         }
         if (nkp_total > 0) {
             if (!curkps) return ov2_fail(ctx, OV2_ERR_INVALID, (std::string(what) + ": curkps is NULL").c_str());
-            if ((st = ov2_stage_in(ctx, curkps, sizeof(float) * 2 * (size_t)nkp_total, &d)) != OV2_OK) return st;
-            D->kps = (const float2*)d;
+            if ((st = ov2_stage_in(ctx, curkps, (size_t)nkp_total, D->kps)) != OV2_OK) return st;
         }
     }
-    if ((st = ov2_stage_out(ctx, state_inout, state_bytes * (size_t)count, &D->state, true)) != OV2_OK) return st;
-    if ((st = ov2_stage_out(ctx, out_pts, sizeof(float) * 2 * (size_t)count * max_per_frame, &o)) != OV2_OK) return st;
-    D->out = (float2*)o;
-    if ((st = ov2_stage_out(ctx, out_counts, sizeof(int32_t) * (size_t)count, &o)) != OV2_OK) return st;
-    D->cnt = (int32_t*)o;
-    const size_t int_bytes = sizeof(int32_t) * 2 * (size_t)count * max_per_frame;
-    if ((st = out_pts_int ? ov2_stage_out(ctx, out_pts_int, int_bytes, &o) : ov2_scratch(ctx, int_bytes, &o)) != OV2_OK) return st;
-    D->ints = (int2*)o;
-    return OV2_OK;
+    if ((st = ov2_stage_out(ctx, state_inout, (size_t)count, D->state, true)) != OV2_OK) return st;
+    const size_t slots = (size_t)count * max_per_frame;
+    if ((st = ov2_stage_out(ctx, out_pts, slots, D->out)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, out_counts, (size_t)count, D->cnt)) != OV2_OK) return st;
+    return out_pts_int ? ov2_stage_out(ctx, out_pts_int, slots, D->ints) : ov2_scratch(ctx, slots, D->ints);
 }

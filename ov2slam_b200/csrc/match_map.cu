@@ -173,35 +173,25 @@ extern "C" ov2_status ov2_match_to_map(ov2_ctx* ctx, const ov2_match_problem* p,
     A.nkps = p->nkps; A.nmps = p->nmps; A.ncand = p->ncand;
     A.dmaxpxdist = p->dmaxpxdist; A.view_th = p->view_th;
     A.mindist = (float)((double)(32.0f * p->fdistratio) * 8.0);       // plm->desc_.cols * fdistratio * 8. (mapper.cpp:643)
-    const void* d = nullptr;
-    void* o = nullptr;
-#define IN(field, type, count) do { if ((st = ov2_stage_in(ctx, p->field, sizeof(type) * (size_t)(count), &d)) != OV2_OK) return st; A.field = (const type*)d; } while (0)
-    const int ndesc_total = p->ndesc, nobs_total = p->nobs;
-    IN(cell_ptr, int32_t, p->ncells + 1);
-    IN(cell_kp, int32_t, p->nkps);
-    if ((st = ov2_stage_in(ctx, p->kp_px, sizeof(float) * 2 * (size_t)p->nkps, &d)) != OV2_OK) return st;
-    A.kp_px = (const float2*)d;
-    IN(kp_lm, int32_t, p->nkps);
-    IN(mp_xyz, double, 3 * (size_t)p->nmps);
-    IN(mp_desc_ptr, int32_t, p->nmps + 1);
-    IN(desc, uint8_t, 32 * (size_t)ndesc_total);
-    if ((st = ov2_stage_in(ctx, p->mp_kfmask, sizeof(uint64_t) * 4 * (size_t)p->nmps, &d)) != OV2_OK) return st;
-    A.mp_kfmask = (const unsigned long long*)d;
-    IN(mp_obs_ptr, int32_t, p->nmps + 1);
-    IN(obs_kf, int32_t, nobs_total);
-    if ((st = ov2_stage_in(ctx, p->obs_px, sizeof(float) * 2 * (size_t)nobs_total, &d)) != OV2_OK) return st;
-    A.obs_px = (const float2*)d;
-    IN(kf_Tcw, double, 12 * (size_t)p->nkfs);
-    IN(cand_mp, int32_t, p->ncand);
-#undef IN
-    if ((st = ov2_stage_out(ctx, best_kp_out, sizeof(int32_t) * (size_t)(p->ncand > 0 ? p->ncand : 1), &o)) != OV2_OK) return st;
-    A.best_kp = (int32_t*)o;
-    if ((st = ov2_stage_out(ctx, best_dist_out, sizeof(float) * (size_t)(p->ncand > 0 ? p->ncand : 1), &o)) != OV2_OK) return st;
-    A.best_dist = (float*)o;
-    if ((st = ov2_stage_out(ctx, kp_match_out, sizeof(int32_t) * (size_t)(p->nkps > 0 ? p->nkps : 1), &o)) != OV2_OK) return st;
-    A.kp_match = (int32_t*)o;
-    if ((st = ov2_stage_out(ctx, kp_dist_out, sizeof(float) * (size_t)(p->nkps > 0 ? p->nkps : 1), &o)) != OV2_OK) return st;
-    A.kp_dist = (float*)o;
+    const size_t nkps = (size_t)p->nkps, nmps = (size_t)p->nmps;
+    if ((st = ov2_stage_in(ctx, p->cell_ptr, (size_t)(p->ncells + 1), A.cell_ptr)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->cell_kp, nkps, A.cell_kp)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->kp_px, nkps, A.kp_px)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->kp_lm, nkps, A.kp_lm)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->mp_xyz, 3 * nmps, A.mp_xyz)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->mp_desc_ptr, nmps + 1, A.mp_desc_ptr)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->desc, 32 * (size_t)p->ndesc, A.desc)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->mp_kfmask, 4 * nmps, A.mp_kfmask)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->mp_obs_ptr, nmps + 1, A.mp_obs_ptr)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->obs_kf, (size_t)p->nobs, A.obs_kf)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->obs_px, (size_t)p->nobs, A.obs_px)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->kf_Tcw, 12 * (size_t)p->nkfs, A.kf_Tcw)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, p->cand_mp, (size_t)p->ncand, A.cand_mp)) != OV2_OK) return st;
+    const size_t nout_cand = p->ncand > 0 ? p->ncand : 1, nout_kps = p->nkps > 0 ? p->nkps : 1;
+    if ((st = ov2_stage_out(ctx, best_kp_out, nout_cand, A.best_kp)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, best_dist_out, nout_cand, A.best_dist)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, kp_match_out, nout_kps, A.kp_match)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, kp_dist_out, nout_kps, A.kp_dist)) != OV2_OK) return st;
     if (p->ncand > 0) OV2_LAUNCH(ctx, "match_mp_kernel", match_mp_kernel<<<div_up(p->ncand, WARPS), WARPS * 32, 0, ctx->stream>>>(A));
     if (p->nkps > 0) OV2_LAUNCH(ctx, "match_kp_kernel", match_kp_kernel<<<div_up(p->nkps, 128), 128, 0, ctx->stream>>>(A));
     return ov2_end(ctx);

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -123,6 +124,41 @@ ov2_status ov2_stage_out(ov2_ctx* ctx, void* p, size_t bytes, void** dev, bool c
 ov2_status ov2_end(ov2_ctx* ctx);                                 // D2H of pending outputs + sync if any
 ov2_status ov2_wait_stream(ov2_ctx* ctx);                         // sleep-wait for the context's stream
 ov2_status ov2_batch_flush_outputs(ov2_ctx* ctx);                 // batch mode: enqueue the D2H copies (no wait)
+
+// The same, typed: counts are in elements of T.
+template <class T> ov2_status ov2_stage_in(ov2_ctx* ctx, const void* p, size_t count, const T*& dev) {
+    const void* d = nullptr;
+    const ov2_status st = ov2_stage_in(ctx, p, sizeof(T) * count, &d);
+    dev = static_cast<const T*>(d);
+    return st;
+}
+template <class T> ov2_status ov2_stage_out(ov2_ctx* ctx, void* p, size_t count, T*& dev, bool copy_in = false) {
+    void* d = nullptr;
+    const ov2_status st = ov2_stage_out(ctx, p, sizeof(T) * count, &d, copy_in);
+    dev = static_cast<T*>(d);
+    return st;
+}
+template <class T> ov2_status ov2_scratch(ov2_ctx* ctx, size_t count, T*& dev) {
+    void* d = nullptr;
+    const ov2_status st = ov2_scratch(ctx, sizeof(T) * count, &d);
+    dev = static_cast<T*>(d);
+    return st;
+}
+
+// A call composed of other calls: runs enqueue inside the caller's open batch, or inside a batch of its own, so that the
+// calls it makes only enqueue, scratch survives between them, and host outputs come back with one synchronisation at the
+// end.  With device outputs only, the call returns without waiting, as every other call with device pointers.
+ov2_status ov2_in_batch(ov2_ctx* ctx, const std::function<ov2_status()>& enqueue);
+
+// A host table of count + 1 offsets that start at 0 and never decrease: each frame of a batch owns
+// [t[f], t[f + 1]) of arrays sized t[count].
+enum ov2_offsets_check { OV2_OFFSETS_OK, OV2_OFFSETS_ON_DEVICE, OV2_OFFSETS_NOT_ASCENDING };
+ov2_offsets_check ov2_check_offsets(const int32_t* t, int count);
+
+// Two pyramids one tracker can read together: both built, same depth and level-0 size.
+static inline bool ov2_pyr_pair_ok(const ov2_pyr* a, const ov2_pyr* b) {
+    return a->nlev == b->nlev && a->w[0] == b->w[0] && a->h[0] == b->h[0] && a->l0 && b->l0;
+}
 
 // pyramid build in two halves (frontend_step.cu orders the uploads of concurrent contexts)
 ov2_status ov2_pyr_load_level0(ov2_ctx* ctx, ov2_pyr* p, const uint8_t* images, size_t row_stride, size_t frame_stride,

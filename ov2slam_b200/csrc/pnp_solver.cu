@@ -96,53 +96,34 @@ extern "C" ov2_status ov2_pnp_solve(ov2_ctx* ctx, int nprob, const int32_t* offs
     if (!ctx || nprob < 0 || (nprob > 0 && (!offsets || !K || !pose_inout || !success_out)))
         return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: bad arguments");
     if (nprob == 0) return OV2_OK;
-    if (ov2_is_device_ptr(offsets)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must be a host pointer");
     // every block reads offsets[pb] .. offsets[pb + 1] of buffers sized offsets[nprob]: a descending pair would read past them
-    if (offsets[0] != 0) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
-    for (int k = 0; k < nprob; ++k)
-        if (offsets[k + 1] < offsets[k]) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
+    const ov2_offsets_check oc = ov2_check_offsets(offsets, nprob);
+    if (oc == OV2_OFFSETS_ON_DEVICE) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must be a host pointer");
+    if (oc != OV2_OFFSETS_OK) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: offsets must start at 0 and be ascending");
     const int N = offsets[nprob];
     if (N > 0 && (!unpx || !wpts || !outlier_flags)) return ov2_fail(ctx, OV2_ERR_INVALID, "ov2_pnp_solve: null array");
     ov2_status st = ov2_begin(ctx);
     if (st != OV2_OK) return st;
     PnpArgs A;
     A.nprob = nprob; A.nmaxiter = nmaxiter; A.chi2th = chi2th; A.use_robust = use_robust; A.apply_l2 = apply_l2_after_robust;
-    const void* d = nullptr;
-    void* o = nullptr;
-    if ((st = ov2_stage_in(ctx, offsets, sizeof(int32_t) * (size_t)(nprob + 1), &d)) != OV2_OK) return st;
-    A.offsets = (const int32_t*)d;
-    if ((st = ov2_stage_in(ctx, K, sizeof(double) * 4 * (size_t)nprob, &d)) != OV2_OK) return st;
-    A.K = (const double*)d;
+    const size_t np = (size_t)nprob, nn = (size_t)N;
+    if ((st = ov2_stage_in(ctx, offsets, np + 1, A.offsets)) != OV2_OK) return st;
+    if ((st = ov2_stage_in(ctx, K, 4 * np, A.K)) != OV2_OK) return st;
     A.unpx = nullptr; A.wpts = nullptr; A.scales = nullptr; A.flags = nullptr; A.chi2 = nullptr; A.depth = nullptr; A.work = nullptr;
     if (N > 0) {
-        if ((st = ov2_stage_in(ctx, unpx, sizeof(double) * 2 * (size_t)N, &d)) != OV2_OK) return st;
-        A.unpx = (const double*)d;
-        if ((st = ov2_stage_in(ctx, wpts, sizeof(double) * 3 * (size_t)N, &d)) != OV2_OK) return st;
-        A.wpts = (const double*)d;
-        if (scales) {
-            if ((st = ov2_stage_in(ctx, scales, sizeof(int32_t) * (size_t)N, &d)) != OV2_OK) return st;
-            A.scales = (const int32_t*)d;
-        }
-        if ((st = ov2_stage_out(ctx, outlier_flags, (size_t)N, &o)) != OV2_OK) return st;
-        A.flags = (uint8_t*)o;
-        if ((st = ov2_scratch(ctx, sizeof(double) * (size_t)N, &o)) != OV2_OK) return st;
-        A.chi2 = (double*)o;
-        if ((st = ov2_scratch(ctx, (size_t)N, &o)) != OV2_OK) return st;
-        A.depth = (uint8_t*)o;
-        if ((st = ov2_scratch(ctx, (size_t)N, &o)) != OV2_OK) return st;
-        A.work = (uint8_t*)o;
-        OV2_CUDA(ctx, cudaMemsetAsync(A.flags, 0, (size_t)N, ctx->stream));
+        if ((st = ov2_stage_in(ctx, unpx, 2 * nn, A.unpx)) != OV2_OK) return st;
+        if ((st = ov2_stage_in(ctx, wpts, 3 * nn, A.wpts)) != OV2_OK) return st;
+        if (scales && (st = ov2_stage_in(ctx, scales, nn, A.scales)) != OV2_OK) return st;
+        if ((st = ov2_stage_out(ctx, outlier_flags, nn, A.flags)) != OV2_OK) return st;
+        if ((st = ov2_scratch(ctx, nn, A.chi2)) != OV2_OK) return st;
+        if ((st = ov2_scratch(ctx, nn, A.depth)) != OV2_OK) return st;
+        if ((st = ov2_scratch(ctx, nn, A.work)) != OV2_OK) return st;
+        OV2_CUDA(ctx, cudaMemsetAsync(A.flags, 0, nn, ctx->stream));
     }
-    if ((st = ov2_stage_out(ctx, pose_inout, sizeof(double) * 7 * (size_t)nprob, &o, true)) != OV2_OK) return st;
-    A.pose = (double*)o;
-    if ((st = ov2_stage_out(ctx, success_out, (size_t)nprob, &o)) != OV2_OK) return st;
-    A.success = (uint8_t*)o;
-    if (iterations_out) {
-        if ((st = ov2_stage_out(ctx, iterations_out, sizeof(int32_t) * (size_t)nprob, &o)) != OV2_OK) return st;
-    } else {
-        if ((st = ov2_scratch(ctx, sizeof(int32_t) * (size_t)nprob, &o)) != OV2_OK) return st;
-    }
-    A.iterations = (int32_t*)o;
+    if ((st = ov2_stage_out(ctx, pose_inout, 7 * np, A.pose, true)) != OV2_OK) return st;
+    if ((st = ov2_stage_out(ctx, success_out, np, A.success)) != OV2_OK) return st;
+    if ((st = iterations_out ? ov2_stage_out(ctx, iterations_out, np, A.iterations) : ov2_scratch(ctx, np, A.iterations)) != OV2_OK)
+        return st;
     OV2_LAUNCH(ctx, "pnp_kernel", pnp_kernel<<<nprob, PNP_THREADS, 0, ctx->stream>>>(A));
     return ov2_end(ctx);
 }
