@@ -318,7 +318,11 @@ OV2_API ov2_status ov2_describe_config(ov2_ctx* ctx, int mode, const int8_t* pai
  * difference to the sub-pixel patch of the left image.  xprior_out = that column (float, same fractional part as the
  * input) or -1 when the window shrinks to nothing at the border / no candidate is below 255; l1err_out = the minimum
  * (255 when xprior is -1; the reference leaves it unset there).  nwinsize must be odd (OV2_ERR_INVALID otherwise, the
- * reference prints a message and returns) and <= 15.  Frame addressing as ov2_fb_klt. */
+ * reference prints a message and returns) and <= 15.  Frame addressing as ov2_fb_klt.
+ * Within one pixel of the right / bottom edge the reference's border rule grows the half window instead of shrinking it
+ * (to at most 4 * (nwinsize / 2) - 3 for a point inside the right image, 25 for window 15).  Points outside the right image
+ * (x >= cols or y >= rows) are accepted and grow it further: the result equals the reference's while the grown half window
+ * is <= 25, and is (-1, 255) beyond.  x < 0 or a NaN x marks an empty slot: (-1, 255). */
 OV2_API ov2_status ov2_line_min_sad(ov2_ctx* ctx, const ov2_pyr* left, const ov2_pyr* right, int level, int n,
                             const int32_t* frame_idx, int first_frame, int per_frame, const float* pts, int nwinsize,
                             int goleft, float* xprior_out, float* l1err_out);

@@ -24,8 +24,11 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int WARPS = 4;
 constexpr int MAX_WS = 15;
 // The reference's border rule can GROW the half window (halfwin += x + halfwin - cols - 1 is positive within one pixel of
-// the right / bottom edge, feature_tracker.cpp:155-160): from h0 = nwinsize / 2 up to 4 h0 - 6 after both tests.
-constexpr int MAX_HW = 4 * (MAX_WS / 2) - 6;             // 22
+// the right / bottom edge, feature_tracker.cpp:155-160).  The sum is taken in float: for x just below cols, x + h can round
+// up to exactly cols + h, so each edge test takes h to 2 h - 1 (not 2 h - 2), and an in-image point reaches 4 h0 - 3 after
+// both tests (h0 = nwinsize / 2; 25 for window 15, e.g. (93.99999, 59.999996) on a 94 x 60 level).  Points past the right
+// or bottom edge can grow further; they get (-1, 255) once the half window exceeds this bound.
+constexpr int MAX_HW = 4 * (MAX_WS / 2) - 3;             // 25
 constexpr int MAX_PATCH = (2 * MAX_HW + 1) * (2 * MAX_HW + 1);
 
 struct SadArgs {
