@@ -30,11 +30,6 @@ struct FeatureTracker::ThreadState {
 namespace {
 std::mutex g_mu;
 std::unordered_map<std::thread::id, FeatureTracker::ThreadState*>* g_states = nullptr;
-int env_device() {
-    // the reference's class takes no device: OV2_DEVICE names the GPU (default 0)
-    const char* e = getenv("OV2_DEVICE");
-    return e ? atoi(e) : 0;
-}
 }  // namespace
 
 FeatureTracker::FeatureTracker(int nmax_iter, float fmax_px_precision, cv::Ptr<cv::CLAHE> pclahe)
@@ -48,7 +43,7 @@ FeatureTracker::ThreadState* FeatureTracker::state() const {
     auto it = g_states->find(std::this_thread::get_id());
     if (it != g_states->end()) return it->second;
     ThreadState* s = new ThreadState();
-    if (ov2_create(env_device(), &s->ctx) != OV2_OK) {
+    if (ov2_create(ov2shim::env_device(), &s->ctx) != OV2_OK) {
         fprintf(stderr, "[ov2b200] FeatureTracker: no CUDA device - the GPU front-end has no CPU fallback\n");
         s->ctx = nullptr;
     }
@@ -177,36 +172,6 @@ void FeatureTracker::getLineMinSAD(const cv::Mat &iml, const cv::Mat &imr, const
         }
     }
     l1err = minsad;
-}
-
-// The same search for every point of a keyframe in ONE device call (csrc/frontend_sad.cu: one warp per point, identical
-// arithmetic), on the cached device pyramids of the two images.
-bool FeatureTracker::getLineMinSADBatch(const std::vector<cv::Mat> &vleftpyr, const std::vector<cv::Mat> &vrightpyr, int pyrlvl,
-        const std::vector<cv::Point2f> &vpts, const int nwinsize, bool bgoleft, std::vector<float> &vxprior, std::vector<float> &vl1err) const
-{
-    vxprior.assign(vpts.size(), -1.f);
-    vl1err.assign(vpts.size(), 255.f);
-    if (vpts.empty()) return true;
-    ThreadState* s = state();
-    if (!s->ctx || vleftpyr.empty() || vrightpyr.empty()) return false;
-    const int nlev_extra = (int)vleftpyr.size() / 2 - 1;
-    if (pyrlvl < 0 || pyrlvl > nlev_extra || vrightpyr.size() != vleftpyr.size()) {
-        fprintf(stderr, "[ov2b200] getLineMinSADBatch: pyramid level %d not in the pyramids\n", pyrlvl);
-        return false;
-    }
-    ov2_pyr* dl = s->cache.get(s->ctx, vleftpyr[0], nlev_extra);
-    ov2_pyr* dr = dl ? s->cache.get(s->ctx, vrightpyr[0], nlev_extra) : nullptr;
-    ov2_status st = (dl && dr) ? OV2_OK : OV2_ERR_CUDA;
-    if (st == OV2_OK)
-        st = ov2_line_min_sad(s->ctx, dl, dr, pyrlvl, (int)vpts.size(), nullptr, 0, (int)vpts.size(),
-                              reinterpret_cast<const float*>(vpts.data()), nwinsize, bgoleft ? 1 : 0, vxprior.data(), vl1err.data());
-    if (st != OV2_OK) {
-        fprintf(stderr, "[ov2b200] getLineMinSADBatch: %s\n", ov2_last_error(s->ctx));
-        vxprior.assign(vpts.size(), -1.f);
-        vl1err.assign(vpts.size(), 255.f);
-        return false;
-    }
-    return true;
 }
 
 bool FeatureTracker::inBorder(const cv::Point2f &pt, const cv::Mat &im) const

@@ -26,13 +26,6 @@ public:
 
     void getLineMinSAD(const cv::Mat &iml, const cv::Mat &imr, const cv::Point2f &pt, const int nwinsize, float &xprior, float &l1err, bool bgoleft) const;
 
-    // EXTENSION (not in the reference's class): getLineMinSAD for all the points of a keyframe in one device call
-    // (ov2_line_min_sad) on pyramid level `pyrlvl` of the two image pyramids; same results as calling getLineMinSAD per point on
-    // vleftpyr[2 * pyrlvl] / vrightpyr[2 * pyrlvl] (xprior -1 where it finds nothing).  Used by the drop-in
-    // MapManager::stereoMatching (host/map_manager_stereo_gpu.cpp).  false: device failure, outputs are all -1.
-    bool getLineMinSADBatch(const std::vector<cv::Mat> &vleftpyr, const std::vector<cv::Mat> &vrightpyr, int pyrlvl,
-        const std::vector<cv::Point2f> &vpts, const int nwinsize, bool bgoleft, std::vector<float> &vxprior, std::vector<float> &vl1err) const;
-
     bool inBorder(const cv::Point2f &pt, const cv::Mat &im) const;
 
     // KLT optim. parameter

@@ -15,6 +15,7 @@
 
 #include "visual_front_end.hpp"
 #include "feature_tracker.hpp"
+#include "abi_flat.hpp"
 
 struct KpRec { int32_t lmid, is3d; float px[2]; double wpt[3]; };
 
@@ -77,11 +78,8 @@ int main(int argc, char** argv) {
 
     FILE* g = fopen(argv[2], "wb");
     if (!g) return 4;
-    const Sophus::SE3d Tcw = frame->getTcw();
-    const Eigen::Matrix3d R = Tcw.rotationMatrix();
-    const Eigen::Vector3d t = Tcw.translation();
-    const Eigen::Vector3d c0 = R * Eigen::Vector3d(1, 0, 0), c1 = R * Eigen::Vector3d(0, 1, 0), c2 = R * Eigen::Vector3d(0, 0, 1);
-    const double T[12] = {c0.x(), c1.x(), c2.x(), c0.y(), c1.y(), c2.y(), c0.z(), c1.z(), c2.z(), t.x(), t.y(), t.z()};
+    double T[12];
+    ov2shim::put_pose(frame->getTcw(), T);
     int32_t v = n;
     fwrite(&v, 4, 1, g);
     fwrite(T, 8, 12, g);

@@ -1,143 +1,97 @@
 // MapManager::stereoMatching on the GPU (8f-3): the reference's declaration (include/map_manager.hpp:83) is kept, this translation
 // unit supplies the body of /root/reference/src/map_manager.cpp:367-611.  Exclude the reference's own body with
-// #ifndef OV2_EXTERNAL_STEREOMATCHING.  What runs where:
-//   host (here)   prior generation - projection of the keypoint's own map point into the right image (:405-416), or, for
-//                 non-rectified rigs, the inverse-distance-weighted depth of the 3-D neighbours in the surrounding grid cells pushed
-//                 along the keypoint's bearing (:436-480) - list building, the retry of failed prior tracks on the full pyramid
-//                 (:528-534), the epipolar test (row difference or Sampson distance, :579-600) and the map update;
-//   device        the rectified-rig prior: FeatureTracker::getLineMinSAD for ALL the keypoints that need it in ONE call
-//                 (FeatureTracker::getLineMinSADBatch -> ov2_line_min_sad, csrc/frontend_sad.cu) instead of one call per keypoint
-//                 (:417-431); the two forward-backward KLT passes (FeatureTracker::fbKltTracking -> ov2_fb_klt), on the cached
-//                 device pyramids of the two images (each uploaded once).
-// Order of every list (and therefore of the tracker's inputs and of the map updates) is the reference's.
+// #ifndef OV2_EXTERNAL_STEREOMATCHING.
+//
+// It flattens the keyframe's keypoints (frame.getKeypoints(), in that order) with their map points, the pose, the right
+// calibration, the rig and, for rigs that are not rectified, the grid; reads the two pyramids from the device-pyramid cache
+// (pyr_cache.hpp) and makes ONE ov2_stereo_matching call: the priors, the row search, the two tracker passes, the undistortion and
+// the epipolar gate run on the device without a synchronisation between them.  Then every stereo match becomes
+// updateKeypointStereo.  3-D keypoints whose map point is gone lose their observation while flattening (:411-414), as in the
+// reference; the device drops them.
+// Not handled: fisheye right calibrations (the device projection is the pinhole / radial-tangential model): a diagnostic, and the
+// frame and the map are left as they were.  Without a CUDA device no keypoint becomes a stereo keypoint.
 // Compile-checked and self-tested against the stand-in map classes (host/standin/ref/): host/stereo_selftest.cpp.
-#include <cmath>
+#include <cstdint>
 #include <iostream>
 #include <vector>
 
 #include "map_manager.hpp"             // the reference's, unchanged
-#include "multi_view_geometry.hpp"
-#include "feature_tracker.hpp"         // the drop-in class (host/feature_tracker.hpp)
-
-namespace {
-
-// keypoints queued for one tracker call: id, left pixel, starting point in the right image
-struct TrackQueue {
-    std::vector<int> ids;
-    std::vector<cv::Point2f> left, right;
-    void push(int id, const cv::Point2f& l, const cv::Point2f& r) { ids.push_back(id); left.push_back(l); right.push_back(r); }
-    bool empty() const { return ids.empty(); }
-    size_t size() const { return ids.size(); }
-};
-
-// the inverse-distance-weighted depth of the 3-D keypoints around `kp` (the four grid cells Frame::getSurroundingKeypoints visits);
-// false when there is none (map_manager.cpp:437-463)
-bool neighbour_depth(const MapManager& map, const Frame& frame, const Keypoint& kp, double& depth) {
-    double zsum = 0., wsum = 0.;
-    size_t used = 0;
-    for (const auto& other : frame.getSurroundingKeypoints(kp)) {
-        if (!other.is3d_) continue;
-        const auto plm = map.getMapPoint(other.lmid_);
-        if (plm == nullptr) continue;
-        const float dx = other.unpx_.x - kp.unpx_.x, dy = other.unpx_.y - kp.unpx_.y;      // cv::norm(Point2f): float difference,
-        const double wgt = 1. / std::sqrt((double)dx * dx + (double)dy * dy);               // double sum of squares
-        wsum += wgt;
-        zsum += wgt * frame.projWorldToCam(plm->getPoint()).z();
-        used++;
-    }
-    if (used == 0) return false;
-    depth = zsum / wsum;
-    return true;
-}
-
-}  // namespace
+#include "feature_tracker.hpp"         // the drop-in class (host/feature_tracker.hpp): klt_convg_crit_
+#include "abi_flat.hpp"
+#include "pyr_cache.hpp"
+#include "../../include/ov2b200.h"
 
 void MapManager::stereoMatching(Frame &frame, const std::vector<cv::Mat> &vleftpyr, const std::vector<cv::Mat> &vrightpyr)
 {
     const SlamParams& cfg = *pslamstate_;
     const bool rectified = cfg.bdo_stereo_rect_;
-    const int coarsest = cfg.nklt_pyr_lvl_;                      // pyramid level of the row search (entry 2 * level of the vectors)
-    const float up = std::pow(2, coarsest), down = 1. / up;
-    if (rectified && (vleftpyr.size() <= (size_t)(2 * coarsest) || vrightpyr.size() <= (size_t)(2 * coarsest))) {
-        std::cerr << "[ov2b200] stereoMatching: the pyramids have no level " << coarsest << " for the row search\n";
+    const int nlvl = cfg.nklt_pyr_lvl_;                          // pyramid level of the row search (entry 2 * level of the vectors)
+    if (rectified && (vleftpyr.size() <= (size_t)(2 * nlvl) || vrightpyr.size() <= (size_t)(2 * nlvl))) {
+        std::cerr << "[ov2b200] stereoMatching: the pyramids have no level " << nlvl << " for the row search\n";
         return;
     }
-
-    // ---- 1. every keypoint of the frame goes to one of two queues: `guided` (a prior from geometry exists: tracked on 2 levels
-    //         first) or `blind` (full pyramid).  Keypoint order is kept inside each queue.                       (:395-493)
-    TrackQueue guided, blind;
-    std::vector<cv::Point2f> rowsearch_pts;                       // rectified rigs: coarsest-level pixels awaiting the row search
-    std::vector<size_t> rowsearch_slot;                           // ... and the entry of `blind` each one belongs to
-    for (const Keypoint& kp : frame.getKeypoints()) {
-        if (kp.is3d_) {
-            const auto plm = getMapPoint(kp.lmid_);
-            if (plm == nullptr) {                                 // dangling observation: drop it, no stereo for it (:411-414)
-                removeMapPointObs(kp.lmid_, frame.kfid_);
-                continue;
-            }
-            const cv::Point2f proj = frame.projWorldToRightImageDist(plm->getPoint());
-            if (frame.isInRightImage(proj)) { guided.push(kp.lmid_, kp.px_, proj); continue; }
-        }
-        if (rectified) {
-            rowsearch_pts.push_back(cv::Point2f(kp.px_.x * down, kp.px_.y * down));
-            rowsearch_slot.push_back(blind.size());
-        } else {
-            double depth;
-            if (neighbour_depth(*this, frame, kp, depth)) {
-                const Eigen::Vector3d campt = depth * (kp.bv_ / kp.bv_.z());
-                const cv::Point2f proj = frame.projCamToRightImageDist(campt);
-                if (frame.isInRightImage(proj)) { guided.push(kp.lmid_, kp.px_, proj); continue; }
-            }
-        }
-        blind.push(kp.lmid_, kp.px_, kp.px_);
+    const auto cal = frame.pcalib_rightcam_;
+    if (cal->model_ != CameraCalibration::Pinhole) {
+        std::cerr << "[ov2b200] stereoMatching: only the pinhole (radial-tangential) model is built; keep the reference's body for fisheye\n";
+        return;
     }
-
-    // ---- 2. rectified rigs: ONE device call finds the best column on the coarsest level for all queued keypoints; a hit to the
-    //         left of the keypoint becomes the x of its starting point                                            (:417-435)
-    if (!rowsearch_pts.empty()) {
-        std::vector<float> col, err;
-        ptracker_->getLineMinSADBatch(vleftpyr, vrightpyr, coarsest, rowsearch_pts, 7, true, col, err);
-        for (size_t k = 0; k < col.size(); ++k) {
-            const float x = col[k] * up;
-            const size_t slot = rowsearch_slot[k];
-            if (x >= 0 && x <= blind.left[slot].x) blind.right[slot].x = x;
-        }
+    const std::vector<Keypoint> vkps = frame.getKeypoints();
+    const int n = (int)vkps.size();
+    std::vector<float> px(2 * (size_t)n), unpx(2 * (size_t)n), right(2 * (size_t)n);
+    std::vector<double> bv(3 * (size_t)n), wpt(3 * (size_t)n, 0.0);
+    std::vector<uint8_t> is3d(n, 0), has_mp(n, 0), stereo(n, 0), pass(n, 0);
+    for (int i = 0; i < n; ++i) {
+        const Keypoint& kp = vkps[i];
+        px[2 * i] = kp.px_.x; px[2 * i + 1] = kp.px_.y;
+        unpx[2 * i] = kp.unpx_.x; unpx[2 * i + 1] = kp.unpx_.y;
+        bv[3 * i] = kp.bv_.x(); bv[3 * i + 1] = kp.bv_.y(); bv[3 * i + 2] = kp.bv_.z();
+        if (!kp.is3d_) continue;
+        is3d[i] = 1;
+        const auto plm = getMapPoint(kp.lmid_);
+        if (plm == nullptr) { removeMapPointObs(kp.lmid_, frame.kfid_); continue; }
+        has_mp[i] = 1;
+        const Eigen::Vector3d w = plm->getPoint();
+        wpt[3 * i] = w.x(); wpt[3 * i + 1] = w.y(); wpt[3 * i + 2] = w.z();
     }
+    std::vector<int32_t> cell_ptr, cell_kps;
+    if (!rectified && !ov2shim::grid_csr(frame, vkps, "stereoMatching", cell_ptr, cell_kps)) return;
+    const int32_t cell_offsets[2] = {0, (int32_t)frame.vgridkps_.size()};
+    const int32_t grid[2] = {(int32_t)frame.ncellsize_, (int32_t)frame.nbwcells_};
+    const int32_t offsets[2] = {0, n};
+    const int32_t wh[2] = {(int32_t)cal->img_w_, (int32_t)cal->img_h_};
+    double Tcw[12], Trl[12], Frl[9], K[4], D[5];
+    ov2shim::put_pose(frame.getTcw(), Tcw);
+    ov2shim::put_pose(cal->Tcic0_, Trl);                         // what Frame::projCamToRightImageDist applies (frame.cpp:796-799)
+    ov2shim::put_mat3(frame.Frl_, Frl);
+    const double* dist = ov2shim::put_pinhole(*cal, K, D);
+    ov2_klt_params prm;
+    prm.win = cfg.nklt_win_size_;
+    prm.max_iter = ptracker_->klt_convg_crit_.maxCount;
+    prm.eps = (float)ptracker_->klt_convg_crit_.epsilon;
+    prm.ferr = (float)cfg.nklt_err_;
+    prm.fb_dist = cfg.fmax_fbklt_dist_;
 
-    // ---- 3. the two forward-backward KLT passes; a guided track that fails is retried blind from where the tracker left it
-    TrackQueue matched;                                            // id, (unused), right pixel
-    auto track = [&](TrackQueue& q, int nlevels, TrackQueue* retry, const char* what) {
-        if (q.empty()) return;
-        std::vector<bool> ok;
-        ptracker_->fbKltTracking(vleftpyr, vrightpyr, cfg.nklt_win_size_, nlevels, cfg.nklt_err_, cfg.fmax_fbklt_dist_, q.left, q.right, ok);
-        size_t kept = 0;
-        for (size_t i = 0; i < q.size(); ++i) {
-            if (ok.at(i)) { matched.push(q.ids[i], q.left[i], q.right[i]); kept++; }
-            else if (retry) retry->push(q.ids[i], q.left[i], q.right[i]);
-        }
-        if (cfg.debug_) std::cout << "\n >>> Stereo KLT Tracking " << what << " : " << kept << " out of " << q.size() << " kps tracked!\n";
-    };
-    int guided_levels = 1;                                         // 2 levels (:499-504)
-    if (vleftpyr.size() < 2 * (size_t)(guided_levels + 1)) guided_levels = (int)(vleftpyr.size() / 2) - 1;
-    track(guided, guided_levels, &blind, "on priors");
-    track(blind, cfg.nklt_pyr_lvl_, nullptr, "w. no priors");
-
-    // ---- 4. epipolar gate and map update (:575-604)
-    size_t nstereo = 0;
-    for (size_t i = 0; i < matched.size(); ++i) {
-        const cv::Point2f lun = frame.getKeypointById(matched.ids[i]).unpx_;
-        const cv::Point2f run = frame.pcalib_rightcam_->undistortImagePoint(matched.right[i]);
-        float epi;
-        if (rectified) {
-            epi = fabs(lun.y - run.y);
-            matched.right[i].y = lun.y;                            // same row by construction of the rig
-        } else {
-            epi = MultiViewGeometry::computeSampsonDistance(frame.Frl_, lun, run);
-        }
-        if (epi <= 2.) {
-            frame.updateKeypointStereo(matched.ids[i], matched.right[i]);
-            nstereo++;
-        }
+    ov2shim::DeviceState& s = ov2shim::device_state();
+    int32_t nstereo = 0;
+    ov2_status st = n == 0 ? OV2_OK : OV2_ERR_NO_DEVICE;
+    if (n > 0 && s.ctx && !vleftpyr.empty() && !vrightpyr.empty()) {
+        const int nlev_extra = (int)vleftpyr.size() / 2 - 1;
+        ov2_pyr* dleft = s.cache.get(s.ctx, vleftpyr[0], nlev_extra);
+        ov2_pyr* dright = dleft ? s.cache.get(s.ctx, vrightpyr[0], nlev_extra) : nullptr;
+        st = dright ? ov2_stereo_matching(s.ctx, dleft, dright, &prm, 0, 1, offsets, Tcw, K, dist, Trl, Frl, wh,
+                                          rectified ? nullptr : cell_offsets, rectified ? nullptr : grid,
+                                          rectified ? nullptr : cell_ptr.data(), rectified ? nullptr : cell_kps.data(), px.data(),
+                                          unpx.data(), bv.data(), is3d.data(), has_mp.data(), wpt.data(), rectified ? 1 : 0, nlvl,
+                                          right.data(), stereo.data(), pass.data(), &nstereo)
+                    : OV2_ERR_CUDA;
     }
-    if (cfg.debug_) std::cout << "\n \t>>> Nb of stereo tracks: " << nstereo << " out of " << matched.size() << "\n";
+    if (st != OV2_OK) {
+        std::cerr << "[ov2b200] stereoMatching: " << (s.ctx ? ov2_last_error(s.ctx) : "no CUDA device (no CPU fallback)") << "\n";
+        return;
+    }
+    // map_manager.cpp:575-604.  Each call touches one keypoint id, so the order (the reference's: pass-1 tracks first) does not
+    // change the result.
+    for (int i = 0; i < n; ++i)
+        if (stereo[i]) frame.updateKeypointStereo(vkps[i].lmid_, cv::Point2f(right[2 * i], right[2 * i + 1]));
+    if (cfg.debug_) std::cout << "\n \t>>> Nb of stereo tracks: " << nstereo << "\n";
 }

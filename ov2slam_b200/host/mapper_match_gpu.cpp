@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "mapper.hpp"             // the reference's, unchanged
+#include "abi_flat.hpp"
 #include "../../include/ov2b200.h"
 
 namespace {
@@ -28,15 +29,6 @@ ov2_ctx* match_context() {
     static ov2_ctx* ctx = nullptr;                    // mapper thread only
     if (!ctx && ov2_create(0, &ctx) != OV2_OK) ctx = nullptr;
     return ctx;
-}
-
-void put_pose(const Sophus::SE3d& Tcw, std::vector<double>& out) {
-    const Eigen::Matrix3d R = Tcw.rotationMatrix();
-    const Eigen::Vector3d t = Tcw.translation();
-    const Eigen::Vector3d ex(1, 0, 0), ey(0, 1, 0), ez(0, 0, 1);
-    const Eigen::Vector3d c0 = R * ex, c1 = R * ey, c2 = R * ez;     // columns of R (works with Eigen and with the stand-in)
-    const double m[12] = {c0.x(), c1.x(), c2.x(), c0.y(), c1.y(), c2.y(), c0.z(), c1.z(), c2.z(), t.x(), t.y(), t.z()};
-    out.insert(out.end(), m, m + 12);
 }
 }  // namespace
 
@@ -83,12 +75,10 @@ std::map<int,int> Mapper::matchToMap(const Frame &frame, const float fmaxprojerr
     }
     // ---- the frame's keypoints and grid (Frame::getSurroundingKeypoints reads vgridkps_ + mapkps_, frame.cpp:624-650)
     const std::vector<Keypoint> vkps = frame.getKeypoints();
-    std::unordered_map<int, int> kp_index;
     std::vector<float> kp_px;
     std::vector<int32_t> kp_lm(vkps.size(), -1);
     for (size_t j = 0; j < vkps.size(); ++j) {
         const Keypoint& kp = vkps[j];
-        kp_index.emplace(kp.lmid_, (int)j);
         kp_px.push_back(kp.px_.x);
         kp_px.push_back(kp.px_.y);
         if (kp.lmid_ < 0) continue;                                                        // :651-653
@@ -97,22 +87,8 @@ std::map<int,int> Mapper::matchToMap(const Frame &frame, const float fmaxprojerr
         if (pkplm->desc_.empty()) continue;                                                // :674-676
         kp_lm[j] = mp_of(kp.lmid_, pkplm);
     }
-    const int ncells = (int)frame.vgridkps_.size();
-    std::vector<int32_t> cell_ptr(ncells + 1, 0), cell_kp;
-    for (int c = 0; c < ncells; ++c) {
-        for (const int id : frame.vgridkps_[c]) {
-            auto it = kp_index.find(id);
-            if (it != kp_index.end()) cell_kp.push_back(it->second);
-        }
-        cell_ptr[c + 1] = (int32_t)cell_kp.size();
-    }
-    // the ABI stages nkps grid entries: a grid that lists fewer keypoints than the frame holds is padded (the padding is never
-    // reached through cell_ptr); one that lists more (an id in two cells) is not something the reference's Frame produces
-    if (cell_kp.size() > vkps.size()) {
-        std::cerr << "[ov2b200] matchToMap: the frame's grid lists more keypoints than the frame holds\n";
-        return map_previd_newid;
-    }
-    cell_kp.resize(vkps.size(), 0);
+    std::vector<int32_t> cell_ptr, cell_kp;
+    if (!ov2shim::grid_csr(frame, vkps, "matchToMap", cell_ptr, cell_kp)) return map_previd_newid;
     // ---- per map point: world point, descriptors, keyframe set (as raw as getKfObsSet() returns it), valid observations
     std::unordered_map<int, int> kf_index;
     std::vector<std::shared_ptr<Frame>> kfs;
@@ -163,20 +139,16 @@ std::map<int,int> Mapper::matchToMap(const Frame &frame, const float fmaxprojerr
         std::cerr << "[ov2b200] matchToMap: more than 256 keyframes in the observation sets; keep the reference's body for maps this large\n";
         return map_previd_newid;
     }
-    for (const auto& kf : kfs) {
-        if (kf) put_pose(kf->getTcw(), kf_Tcw);
-        else kf_Tcw.insert(kf_Tcw.end(), 12, 0.0);
-    }
+    kf_Tcw.assign(12 * kfs.size(), 0.0);
+    for (size_t k = 0; k < kfs.size(); ++k)
+        if (kfs[k]) ov2shim::put_pose(kfs[k]->getTcw(), &kf_Tcw[12 * k]);
     // ---- one call
     ov2_match_problem p{};
-    std::vector<double> Tcw;
-    put_pose(frame.getTcw(), Tcw);
-    for (int i = 0; i < 12; ++i) p.Tcw[i] = Tcw[i];
-    p.K[0] = cal->fx_; p.K[1] = cal->fy_; p.K[2] = cal->cx_; p.K[3] = cal->cy_;
-    const double D[5] = {cal->k1_, cal->k2_, cal->p1_, cal->p2_, 0.0};
-    p.dist = cal->Dcv_.empty() ? nullptr : D;
+    ov2shim::put_pose(frame.getTcw(), p.Tcw);
+    double D[5];
+    p.dist = ov2shim::put_pinhole(*cal, p.K, D);
     p.img_w = (int)cal->img_w_; p.img_h = (int)cal->img_h_;
-    p.ncellsize = (int)frame.ncellsize_; p.nbwcells = (int)frame.nbwcells_; p.ncells = ncells;
+    p.ncellsize = (int)frame.ncellsize_; p.nbwcells = (int)frame.nbwcells_; p.ncells = (int)frame.vgridkps_.size();
     p.cell_ptr = cell_ptr.data(); p.cell_kp = cell_kp.data();
     p.nkps = (int)vkps.size(); p.kp_px = kp_px.data(); p.kp_lm = kp_lm.data();
     p.nmps = (int)mps.size(); p.mp_xyz = mp_xyz.data(); p.mp_desc_ptr = desc_ptr.data(); p.ndesc = (int)(desc.size() / 32); p.desc = desc.data();

@@ -4,10 +4,10 @@
 // entry is keyed by (data pointer, size, step) AND a 64-bit hash of the pixels: a hit means "this exact image is
 // already on the device with its pyramid levels built"; the hash (~15 us for 640x480) replaces the upload + kernels.
 // In the live loop each image is then uploaded once although fbKltTracking reads it in up to four calls (two calls per
-// frame as cur, two as prev of the next frame; src/visual_front_end.cpp:196,242) and the stereo pass reads it again
-// (src/map_manager.cpp:510,550).
+// frame as cur, two as prev of the next frame; src/visual_front_end.cpp:196,242).
 #pragma once
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 
 #include <opencv2/core.hpp>
@@ -70,5 +70,34 @@ struct PyrCache {
         for (auto& s : slots) { if (s.pyr) ov2_pyr_destroy(s.pyr); s = Slot(); }
     }
 };
+
+// The reference's classes take no device: OV2_DEVICE names the GPU (default 0).
+inline int env_device() {
+    const char* e = getenv("OV2_DEVICE");
+    return e ? atoi(e) : 0;
+}
+
+// The per-thread device state of the drop-ins that make one composed call (VisualFrontEnd::kltTracking on the front-end
+// thread, MapManager::stereoMatching on the mapper thread): a context on OV2_DEVICE and the pyramids of the images they read.
+// Three slots: prev, cur + one spare (the next frame's prev is this frame's cur), or left, right + one spare.  ctx is NULL
+// when no context could be created.
+struct DeviceState {
+    ov2_ctx* ctx = nullptr;
+    PyrCache<3> cache;
+    DeviceState() {
+        if (ov2_create(env_device(), &ctx) != OV2_OK) ctx = nullptr;
+    }
+    ~DeviceState() {
+        cache.clear();
+        if (ctx) ov2_destroy(ctx);
+    }
+    DeviceState(const DeviceState&) = delete;
+    DeviceState& operator=(const DeviceState&) = delete;
+};
+
+inline DeviceState& device_state() {
+    static thread_local DeviceState s;
+    return s;
+}
 
 }  // namespace ov2shim

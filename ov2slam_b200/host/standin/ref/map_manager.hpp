@@ -36,7 +36,7 @@ public:
     double img_w_ = 0, img_h_ = 0;
     cv::Mat Dcv_;                                       // empty: no distortion (camera_calibration.cpp:262)
     Eigen::Matrix3d iK_;
-    Sophus::SE3d Tc0ci_;
+    Sophus::SE3d Tc0ci_, Tcic0_;                        // the reference keeps Tcic0_ = Tc0ci_.inverse() (camera_calibration.cpp:197-198)
     void setK(double fx, double fy, double cx, double cy) {
         fx_ = fx; fy_ = fy; cx_ = cx; cy_ = cy;
         iK_ = Eigen::Matrix3d();
@@ -93,7 +93,7 @@ public:
     // ---- what MapManager::stereoMatching reads and writes (frame.cpp:423-433, 594-622, 830-870)
     Eigen::Matrix3d Frl_;
     cv::Point2f projCamToRightImageDist(const Eigen::Vector3d& pt) const {
-        return pcalib_rightcam_->projectCamToImageDist(pcalib_rightcam_->Tc0ci_.inverse() * pt);
+        return pcalib_rightcam_->projectCamToImageDist(pcalib_rightcam_->Tcic0_ * pt);
     }
     cv::Point2f projWorldToRightImageDist(const Eigen::Vector3d& wpt) const { return projCamToRightImageDist(projWorldToCam(wpt)); }
     bool isInRightImage(const cv::Point2f& pt) const {

@@ -8,9 +8,11 @@
 // With a disparity, the images are a smooth synthetic texture and its copy shifted by that many pixels (a fronto-parallel plane for a
 // rectified rig) instead of blank images: the GPU test checks that the stereo keypoints land `disparity` pixels to the left.
 // scene.bin: i32 nkps, rect, w, h, ncellsize, nbwcells, ncells; f64 K[4], Kr[4], Tc0c1[7] (tx ty tz qx qy qz qw), Twc[7], Frl[9];
-//            per keypoint: i32 lmid, i32 is3d, i32 has_mp; f32 px[2], unpx[2]; f64 bv[3], wpt[3]
+//            per keypoint: i32 lmid, i32 is3d, i32 has_mp; f32 px[2], unpx[2]; f64 bv[3], wpt[3];
+//            optionally f64 Dr[4] (k1 k2 p1 p2 of the right camera; absent or all zero: no distortion model)
 // result.bin: i32 nkps, order[nkps] (the lmids as Frame::getKeypoints() returned them - the order of all the lists);
-//             per keypoint in that order: i32 is_stereo, f32 rpx[2]; i32 n_removed_obs
+//             per keypoint in that order: i32 is_stereo, f32 rpx[2]; i32 n_removed_obs;
+//             f64 Tcw[12], Trl[12] (the keyframe's pose and the rig as the drop-in flattens them)
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +21,7 @@
 
 #include "map_manager.hpp"
 #include "feature_tracker.hpp"
+#include "abi_flat.hpp"
 
 struct KpRec { int32_t lmid, is3d, has_mp; float px[2], unpx[2]; double bv[3], wpt[3]; };
 
@@ -31,7 +34,7 @@ int main(int argc, char** argv) {
     FILE* f = fopen(argv[1], "rb");
     if (!f) return 3;
     int32_t hd[7];
-    double K[4], Kr[4], Trig[7], Twc[7], Frl[9];
+    double K[4], Kr[4], Dr[4] = {0, 0, 0, 0}, Trig[7], Twc[7], Frl[9];
     if (fread(hd, 4, 7, f) != 7 || fread(K, 8, 4, f) != 4 || fread(Kr, 8, 4, f) != 4 || fread(Trig, 8, 7, f) != 7 || fread(Twc, 8, 7, f) != 7 ||
         fread(Frl, 8, 9, f) != 9)
         return 3;
@@ -39,6 +42,7 @@ int main(int argc, char** argv) {
     std::vector<KpRec> recs(nkps);
     for (auto& r : recs)
         if (fread(&r.lmid, 4, 3, f) != 3 || fread(r.px, 4, 4, f) != 4 || fread(r.bv, 8, 6, f) != 6) return 3;
+    if (fread(Dr, 8, 4, f) != 4 && ferror(f)) return 3;
     fclose(f);
 
     auto params = std::make_shared<SlamParams>();
@@ -50,7 +54,12 @@ int main(int argc, char** argv) {
     auto lcal = std::make_shared<CameraCalibration>(), rcal = std::make_shared<CameraCalibration>();
     lcal->setK(K[0], K[1], K[2], K[3]); lcal->img_w_ = w; lcal->img_h_ = h;
     rcal->setK(Kr[0], Kr[1], Kr[2], Kr[3]); rcal->img_w_ = w; rcal->img_h_ = h;
+    if (Dr[0] != 0 || Dr[1] != 0 || Dr[2] != 0 || Dr[3] != 0) {
+        rcal->k1_ = Dr[0]; rcal->k2_ = Dr[1]; rcal->p1_ = Dr[2]; rcal->p2_ = Dr[3];
+        rcal->Dcv_ = cv::Mat(1, 4, CV_8UC1);                  // non-empty: the calibration has a distortion model
+    }
     rcal->Tc0ci_ = se3_of(Trig);
+    rcal->Tcic0_ = rcal->Tc0ci_.inverse();
     Frame frame;
     frame.id_ = frame.kfid_ = 7;
     frame.pcalib_leftcam_ = lcal; frame.pcalib_rightcam_ = rcal;
@@ -113,6 +122,10 @@ int main(int argc, char** argv) {
     }
     n = (int32_t)map->removed_obs_.size();
     fwrite(&n, 4, 1, g);
+    double T[24];
+    ov2shim::put_pose(frame.getTcw(), T);
+    ov2shim::put_pose(rcal->Tcic0_, T + 12);
+    fwrite(T, 8, 24, g);
     fclose(g);
     printf("stereoMatching: %d keypoints, %d stereo, %d observations dropped\n", nkps, nstereo, n);
     return 0;

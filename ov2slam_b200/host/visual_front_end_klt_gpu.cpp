@@ -16,29 +16,9 @@
 
 #include "visual_front_end.hpp"       // the reference's, unchanged
 #include "feature_tracker.hpp"        // the drop-in class (host/feature_tracker.hpp): klt_convg_crit_
+#include "abi_flat.hpp"
 #include "pyr_cache.hpp"
 #include "../../include/ov2b200.h"
-
-namespace {
-struct KltTrackingState {
-    ov2_ctx* ctx = nullptr;
-    ov2shim::PyrCache<3> cache;     // prev, cur + one spare (the next frame's prev is this frame's cur)
-    bool tried = false;
-    ~KltTrackingState() {
-        cache.clear();
-        if (ctx) ov2_destroy(ctx);
-    }
-};
-
-KltTrackingState& klt_state() {
-    static thread_local KltTrackingState s;   // front-end thread
-    if (!s.tried) {
-        s.tried = true;
-        if (ov2_create(0, &s.ctx) != OV2_OK) s.ctx = nullptr;
-    }
-    return s;
-}
-}  // namespace
 
 void VisualFrontEnd::kltTracking()
 {
@@ -52,7 +32,7 @@ void VisualFrontEnd::kltTracking()
         fprintf(stderr, "[ov2b200] kltTracking: only the pinhole (radial-tangential) model is built; keep the reference's body for fisheye\n");
         return;
     }
-    KltTrackingState& s = klt_state();
+    ov2shim::DeviceState& s = ov2shim::device_state();
     ov2_pyr* dprev = nullptr;
     ov2_pyr* dcur = nullptr;
     const int nlev_extra = (int)prev_pyr_.size() / 2 - 1;
@@ -81,13 +61,9 @@ void VisualFrontEnd::kltTracking()
     int32_t nbgood = 0, nbkps = 0;
     ov2_status st = OV2_ERR_NO_DEVICE;
     if (dprev && dcur) {
-        const Sophus::SE3d Tcw = frame.getTcw();
-        const Eigen::Matrix3d R = Tcw.rotationMatrix();
-        const Eigen::Vector3d t = Tcw.translation();
-        const Eigen::Vector3d c0 = R * Eigen::Vector3d(1, 0, 0), c1 = R * Eigen::Vector3d(0, 1, 0), c2 = R * Eigen::Vector3d(0, 0, 1);
-        const double T[12] = {c0.x(), c1.x(), c2.x(), c0.y(), c1.y(), c2.y(), c0.z(), c1.z(), c2.z(), t.x(), t.y(), t.z()};
-        const double K[4] = {cal->fx_, cal->fy_, cal->cx_, cal->cy_};
-        const double D[5] = {cal->k1_, cal->k2_, cal->p1_, cal->p2_, 0.0};   // CameraCalibration keeps four coefficients
+        double T[12], K[4], D[5];
+        ov2shim::put_pose(frame.getTcw(), T);
+        const double* dist = ov2shim::put_pinhole(*cal, K, D);
         const int32_t wh[2] = {(int32_t)cal->img_w_, (int32_t)cal->img_h_};
         const int32_t offsets[2] = {0, n};
         ov2_klt_params prm;
@@ -96,7 +72,7 @@ void VisualFrontEnd::kltTracking()
         prm.eps = (float)ptracker_->klt_convg_crit_.epsilon;
         prm.ferr = (float)pslamstate_->nklt_err_;
         prm.fb_dist = pslamstate_->fmax_fbklt_dist_;
-        st = ov2_klt_tracking(s.ctx, dprev, dcur, &prm, 0, 1, offsets, T, K, cal->Dcv_.empty() ? nullptr : D, wh, px.data(),
+        st = ov2_klt_tracking(s.ctx, dprev, dcur, &prm, 0, 1, offsets, T, K, dist, wh, px.data(),
                               wpt.data(), is3d.data(), pslamstate_->nklt_pyr_lvl_, pslamstate_->klt_use_prior_ ? 1 : 0,
                               tracked.data(), status.data(), pass.data(), &p3p, &nbgood, &nbkps);
     }

@@ -1,4 +1,4 @@
-"""MapManager::stereoMatching on a C4-shaped stereo stage, on one GPU: ov2_stereo_matching against today's flow.
+"""MapManager::stereoMatching on a C4-shaped stereo stage, on one GPU: ov2_stereo_matching against the flow keyframe by keyframe.
 
     python scripts/bench_stereo_matching.py [--keyframes 132] [--steps 10] [--warmup 2] [--cv2-keyframes 8]
 
@@ -9,7 +9,7 @@ Three paths, each reported as ms per keyframe:
 
   device_ms   one ov2_stereo_matching call over all keyframes, every array on the device: the median of `steps` calls,
               each timed by the host clock from its start to the end of a stream synchronisation
-  binding_ms  today's flow through the Python binding, keyframe by keyframe: the projected priors on the host (numpy), the
+  binding_ms  the flow through the Python binding, keyframe by keyframe: the projected priors on the host (numpy), the
               row search (rectified rig) and the two tracker calls on host arrays, each waiting for its result, the retry
               lists and the epipolar gate on the host.  The neighbour-depth prior of the other rig is not computed here
               (those keypoints start blind), so that path does less host work than the reference

@@ -7,8 +7,9 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from ov2slam_b200 import api, build, synth
+import stereo_scenes as SS
 from oracle import image_ref as R_img
+from ov2slam_b200 import api, build, synth
 
 ROOT = Path(__file__).resolve().parents[1]
 
@@ -348,227 +349,91 @@ def test_mapper_match_shim_with_150_keyframes(ctx, tmp_path):
 
 
 # ---------------------------------------------------------------------------------------------- MapManager::stereoMatching drop-in
-def _quat_of(R):
-    """Unit quaternion (x, y, z, w) of a rotation matrix with positive trace (small rotations only)."""
-    w = 0.5 * np.sqrt(1.0 + np.trace(R))
-    return np.array([(R[2, 1] - R[1, 2]) / (4 * w), (R[0, 2] - R[2, 0]) / (4 * w), (R[1, 0] - R[0, 1]) / (4 * w), w])
-
-
-def _stereo_scene(seed, rect, nkps=320, w=752, h=480, cs=35, depth=None):
-    rng = np.random.default_rng(seed)
-    K = np.array([458.654, 457.296, 367.215, 248.375])
-    Rrig = np.eye(3) if rect else synth._so3_exp(np.array([0.004, -0.006, 0.003]))
-    trig = np.array([0.11, 0.0, 0.0]) if rect else np.array([0.11, 0.002, -0.001])        # right camera in the left camera's frame
-    Rwc, twc = synth._so3_exp(rng.normal(0, 0.2, 3)), rng.normal(0, 1.0, 3)
-    px = np.stack([rng.uniform(4, w - 4, nkps), rng.uniform(4, h - 4, nkps)], 1).astype(np.float32)
-    bv = np.stack([(px[:, 0].astype(np.float64) - K[2]) / K[0], (px[:, 1].astype(np.float64) - K[3]) / K[1], np.ones(nkps)], 1)
-    bv /= np.linalg.norm(bv, axis=1, keepdims=True)
-    is3d = rng.random(nkps) < 0.6
-    has_mp = is3d & (rng.random(nkps) > 0.08)
-    z = rng.uniform(0.8, 8.0, nkps)
-    cam = bv / bv[:, 2:3] * z[:, None] + rng.normal(0, 0.002, (nkps, 3))
-    if depth is not None:
-        cam = bv / bv[:, 2:3] * depth
-    wpt = cam @ Rwc.T + twc
-    # p_right = R_rl p_left + t_rl ;  F with  r^T F l = 0
-    Rrl, trl = Rrig.T, -Rrig.T @ trig
-    tx = np.array([[0, -trl[2], trl[1]], [trl[2], 0, -trl[0]], [-trl[1], trl[0], 0]])
-    Kmat = np.array([[K[0], 0, K[2]], [0, K[1], K[3]], [0, 0, 1]])
-    Frl = np.linalg.inv(Kmat).T @ tx @ Rrl @ np.linalg.inv(Kmat)
-    return dict(rect=rect, w=w, h=h, cs=cs, nbw=int(np.ceil(w / cs)), nbh=int(np.ceil(h / cs)), K=K, Rrig=Rrig, trig=trig, Rwc=Rwc, twc=twc,
-                Frl=Frl, lmid=(100 + np.arange(nkps)).astype(np.int32), is3d=is3d, has_mp=has_mp, px=px, unpx=px.copy(), bv=bv, wpt=wpt)
-
-
-def _write_stereo_scene(path, sc):
-    n = len(sc["lmid"])
-    with open(path, "wb") as f:
-        f.write(np.array([n, sc["rect"], sc["w"], sc["h"], sc["cs"], sc["nbw"], sc["nbw"] * sc["nbh"]], np.int32).tobytes())
-        for a in (sc["K"], sc["K"], np.concatenate([sc["trig"], _quat_of(sc["Rrig"])]), np.concatenate([sc["twc"], _quat_of(sc["Rwc"])]), sc["Frl"]):
-            f.write(np.ascontiguousarray(a, np.float64).tobytes())
-        for i in range(n):
-            f.write(np.array([sc["lmid"][i], sc["is3d"][i], sc["has_mp"][i]], np.int32).tobytes())
-            f.write(np.concatenate([sc["px"][i], sc["unpx"][i]]).astype(np.float32).tobytes())
-            f.write(np.concatenate([sc["bv"][i], sc["wpt"][i]]).astype(np.float64).tobytes())
-
-
-def _read_mock_log(path):
+def _read_stereo_log(path):
+    """The calls tests/helpers/frontend_mock.c recorded: ("build",) per pyramid upload, ("stereo", {argument: value}) per
+    ov2_stereo_matching."""
     raw = np.fromfile(path, np.uint8)
     off, calls = 0, []
+
+    def take(k, t):
+        nonlocal off
+        a = raw[off:off + k * np.dtype(t).itemsize].view(t).copy()
+        off += k * np.dtype(t).itemsize
+        return a
     while off < len(raw):
-        tag = int(raw[off:off + 4].view(np.int32)[0])
+        tag = int(take(1, np.int32)[0])
         if tag == 3:
             calls.append(("build",))
-            off += 4
-        elif tag == 1:
-            _, level, n, win, goleft = (int(v) for v in raw[off:off + 20].view(np.int32))
-            pts = raw[off + 20:off + 20 + 8 * n].view(np.float32).reshape(n, 2).copy()
-            calls.append(("sad", level, win, goleft, pts))
-            off += 20 + 8 * n
-        else:
-            assert tag == 2
-            _, n, nlv, win = (int(v) for v in raw[off:off + 16].view(np.int32))
-            pts = raw[off + 16:off + 16 + 8 * n].view(np.float32).reshape(n, 2).copy()
-            pri = raw[off + 16 + 8 * n:off + 16 + 16 * n].view(np.float32).reshape(n, 2).copy()
-            calls.append(("klt", nlv, win, pts, pri))
-            off += 16 + 16 * n
+            continue
+        assert tag == 5
+        first, count, n, win, max_iter, rectified, nlvl, has_dist, has_grid, iw, ih, ncells = (int(v) for v in take(12, np.int32))
+        a = dict(first=first, count=count, win=win, max_iter=max_iter, rectified=rectified, nklt_pyr_lvl=nlvl, img_wh=(iw, ih))
+        a["eps"], a["ferr"], a["fb_dist"] = take(3, np.float32)
+        a["Tcw"], a["K"], dist, a["Trl"], a["Frl"] = take(12, np.float64), take(4, np.float64), take(5, np.float64), take(12, np.float64), take(9, np.float64)
+        a["dist"] = dist if has_dist else None
+        grid = take(2, np.int32)
+        a["grid"] = grid if has_grid else None
+        a["cell_ptr"], a["cell_kps"] = (take(ncells + 1, np.int32), take(n, np.int32)) if has_grid else (None, None)
+        a["px"], a["unpx"] = take(2 * n, np.float32).reshape(n, 2), take(2 * n, np.float32).reshape(n, 2)
+        a["bv"] = take(3 * n, np.float64).reshape(n, 3)
+        a["is3d"], a["has_mp"] = take(n, np.uint8), take(n, np.uint8)
+        a["wpt"] = take(3 * n, np.float64).reshape(n, 3)
+        calls.append(("stereo", a))
     return calls
 
 
-def _mock_klt(pts, pri, nlv):
-    """The canned tracker of tests/helpers/frontend_mock.c."""
-    f32 = np.float32
-    out = pri.copy()
-    out[:, 0] += f32(-0.5)
-    out[:, 1] += np.where(np.floor(pts[:, 0]).astype(int) % 7 == 0, f32(4.0), f32(0.25)).astype(np.float32)
-    if nlv == 1:
-        st = np.floor(f32(3.0) * pts[:, 0] + pts[:, 1]).astype(int) % 4 != 0
-    else:
-        st = np.floor(pts[:, 0] + f32(2.0) * pts[:, 1]).astype(int) % 6 != 0
-    return out, st
-
-
-def _mock_sad(sp):
-    """The canned row search of tests/helpers/frontend_mock.c (coarsest-level pixels in, best column out)."""
-    fx, fy = np.floor(sp[:, 0]).astype(int), np.floor(sp[:, 1]).astype(int)
-    return np.where((fx >= 3) & (fy % 4 != 0), (fx - 2).astype(np.float32), np.float32(-1))
-
-
-def _stereo_flow(sc, order, klt=None, sad=None):
-    """MapManager::stereoMatching (map_manager.cpp:367-611) restated over the scene: the expected tracker / row-search calls and the
-    expected stereo keypoints.  klt(pts, priors, nlevels) -> (moved priors, status) and sad(coarsest-level pts) -> columns default to the
-    mock's rules; tests/test_oracle_vs_reference_map.py passes the real library's functions to compare with the reference's own code."""
-    klt = klt or _mock_klt
-    sad = sad or _mock_sad
-    f32 = np.float32
-    K, idx = sc["K"], {int(l): i for i, l in enumerate(sc["lmid"])}
-    Rcw, Rrl = sc["Rwc"].T, sc["Rrig"].T
-
-    def right_px(cam):
-        p = Rrl @ (cam - sc["trig"])
-        return np.array([f32(K[0] * p[0] / p[2] + K[2]), f32(K[1] * p[1] / p[2] + K[3])], np.float32)
-
-    def in_right(p):
-        return p[0] >= 0 and p[1] >= 0 and p[0] < sc["w"] and p[1] < sc["h"]
-    cell = {}
-    for i in range(len(sc["lmid"])):
-        cell.setdefault((int(np.floor(sc["px"][i, 1] / f32(sc["cs"]))), int(np.floor(sc["px"][i, 0] / f32(sc["cs"])))), []).append(i)
-    v3 = dict(ids=[], pts=[], pri=[])
-    v2 = dict(ids=[], pts=[], pri=[])
-    sad_pts, sad_slot, removed = [], [], 0
-    for lm in order:
-        i = idx[int(lm)]
-        px = sc["px"][i]
-        if sc["is3d"][i]:
-            if sc["has_mp"][i]:
-                proj = right_px(Rcw @ (sc["wpt"][i] - sc["twc"]))
-                if in_right(proj):
-                    v3["ids"].append(int(lm)); v3["pts"].append(px); v3["pri"].append(proj)
-                    continue
-            else:
-                removed += 1
-                continue
-        if sc["rect"]:
-            sad_pts.append(px * f32(0.125))
-            sad_slot.append(len(v2["ids"]))
-        else:
-            r0, c0 = int(np.floor(px[1] / f32(sc["cs"]))), int(np.floor(px[0] / f32(sc["cs"])))
-            nb, mean_z, wsum = 0, 0.0, 0.0
-            for r in (r0 - 1, r0):
-                for c in (c0 - 1, c0):
-                    if r < 0 or c < 0 or r * sc["nbw"] + c >= sc["nbw"] * sc["nbh"]:
-                        continue
-                    for j in cell.get((r, c), []):
-                        if j == i or not sc["is3d"][j] or not sc["has_mp"][j]:
-                            continue
-                        d = sc["unpx"][j] - sc["unpx"][i]
-                        coef = 1.0 / np.sqrt(float(d[0]) ** 2 + float(d[1]) ** 2)
-                        nb += 1
-                        wsum += coef
-                        mean_z += coef * (Rcw @ (sc["wpt"][j] - sc["twc"]))[2]
-            if nb >= 1:
-                proj = right_px(mean_z / wsum * (sc["bv"][i] / sc["bv"][i][2]))
-                if in_right(proj):
-                    v3["ids"].append(int(lm)); v3["pts"].append(px); v3["pri"].append(proj)
-                    continue
-        v2["ids"].append(int(lm)); v2["pts"].append(px); v2["pri"].append(px.copy())
-    calls = []
-    if sad_pts:
-        sp = np.asarray(sad_pts, np.float32)
-        calls.append(("sad", 3, 7, 1, sp))
-        xpr = np.asarray(sad(sp), np.float32) * f32(8.0)
-        for k, slot in enumerate(sad_slot):
-            if xpr[k] >= 0 and xpr[k] <= v2["pts"][slot][0]:
-                v2["pri"][slot][0] = xpr[k]
-    good = []
-    if v3["ids"]:
-        pts, pri = np.asarray(v3["pts"], np.float32), np.asarray(v3["pri"], np.float32)
-        calls.append(("klt", 1, 9, pts, pri))
-        out, st = klt(pts, pri, 1)
-        for k, lm in enumerate(v3["ids"]):
-            if st[k]:
-                good.append((lm, out[k]))
-            else:
-                v2["ids"].append(lm); v2["pts"].append(pts[k]); v2["pri"].append(out[k])
-    if v2["ids"]:
-        pts, pri = np.asarray(v2["pts"], np.float32), np.asarray(v2["pri"], np.float32)
-        calls.append(("klt", 3, 9, pts, pri))
-        out, st = klt(pts, pri, 3)
-        good += [(lm, out[k]) for k, lm in enumerate(v2["ids"]) if st[k]]
-    stereo = {}
-    for lm, rp in good:
-        lun = sc["unpx"][idx[lm]]
-        rp = rp.copy()
-        if sc["rect"]:
-            err = abs(f32(lun[1] - rp[1]))
-            rp[1] = lun[1]
-        else:
-            l, r = np.array([lun[0], lun[1], 1.0], np.float64), np.array([rp[0], rp[1], 1.0], np.float64)
-            Fl, Ftr = sc["Frl"] @ l, sc["Frl"].T @ r
-            err = np.sqrt(float(r @ Fl) ** 2 / (Ftr[0] ** 2 + Ftr[1] ** 2 + Fl[0] ** 2 + Fl[1] ** 2))
-        if err <= 2.0:
-            stereo[lm] = rp
-    return calls, stereo, removed
-
-
+@pytest.mark.parametrize("distorted", [False, True])
 @pytest.mark.parametrize("rect", [1, 0])
-def test_stereo_matching_shim_flow(tmp_path, rect):
-    """The drop-in MapManager::stereoMatching (host/map_manager_stereo_gpu.cpp + the drop-in FeatureTracker, against the stand-in map
-    classes) on a synthetic stereo keyframe, with the device calls replaced by a recorder with rule-based answers
-    (tests/helpers/frontend_mock.c, LD_PRELOAD): each image is uploaded once; rectified rigs make ONE batched row search on the
-    coarsest level for exactly the keypoints without a usable map-point prior; the 2-level tracker call gets the projected /
-    neighbour-depth priors, the full-pyramid call the rest plus the failed ones with their moved priors, in the reference's order;
-    the epipolar test (row difference / Sampson distance) and the row correction decide the stereo keypoints the frame ends up with;
-    keypoints whose map point is gone are dropped from the map."""
+def test_stereo_matching_shim_makes_one_call(tmp_path, rect, distorted):
+    """The drop-in MapManager::stereoMatching (host/map_manager_stereo_gpu.cpp, against the stand-in map classes) on a synthetic stereo
+    keyframe, the right camera undistorted or distorted, with the device calls replaced by a recorder with rule-based answers
+    (tests/helpers/frontend_mock.c, LD_PRELOAD): each image is uploaded once and ONE ov2_stereo_matching call carries the keyframe's
+    keypoints in Frame::getKeypoints() order with their map points, the pose, the rig, the right calibration, the grid (rigs that
+    are not rectified) and the SlamParams / FeatureTracker settings; keypoints whose map point is gone are dropped from the map; exactly
+    the recorder's stereo answers become stereo keypoints, at its right pixels."""
     exe = build.build_stereo_shim()
     mock = tmp_path / "libmock.so"
-    subprocess.check_call(["gcc", "-shared", "-fPIC", "-O1", "-o", str(mock), str(ROOT / "tests" / "helpers" / "frontend_mock.c"), "-lm"])
-    sc = _stereo_scene(31 + rect, rect)
-    _write_stereo_scene(tmp_path / "s.bin", sc)
-    env = dict(os.environ, LD_PRELOAD=str(mock), OV2_MOCK_LOG=str(tmp_path / "log.bin"))
+    subprocess.check_call(["gcc", "-shared", "-fPIC", "-O1", "-o", str(mock), str(ROOT / "tests" / "helpers" / "frontend_mock.c")])
+    sc = SS.stereo_scene(31 + rect, rect, Dr=[-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05] if distorted else None)
+    SS.write_stereo_scene(tmp_path / "s.bin", sc)
+    log = tmp_path / "log.bin"
+    env = dict(os.environ, LD_PRELOAD=str(mock), OV2_MOCK_LOG=str(log))
     out = subprocess.run([str(exe), str(tmp_path / "s.bin"), str(tmp_path / "r.bin")], capture_output=True, text=True, timeout=120, env=env)
     assert out.returncode == 0, out.stdout + out.stderr
-    raw = np.fromfile(tmp_path / "r.bin", np.uint8)
-    n = int(raw[:4].view(np.int32)[0])
-    order = raw[4:4 + 4 * n].view(np.int32)
-    rec = raw[4 + 4 * n:4 + 16 * n].reshape(n, 12)
-    is_stereo = rec[:, :4].copy().view(np.int32).reshape(n) != 0
-    rpx = rec[:, 4:].copy().view(np.float32).reshape(n, 2)
-    removed = int(raw[4 + 16 * n:].view(np.int32)[0])
-    calls = _read_mock_log(tmp_path / "log.bin")
-    want_calls, want_stereo, want_removed = _stereo_flow(sc, order)
-    assert sum(c[0] == "build" for c in calls) == 2                      # left and right image: one upload each
-    calls = [c for c in calls if c[0] != "build"]
-    assert [c[:3] if c[0] == "klt" else c[:4] for c in calls] == [c[:3] if c[0] == "klt" else c[:4] for c in want_calls]
-    assert len(calls) == (3 if rect else 2)
-    for got, want in zip(calls, want_calls):
-        for a, b in zip(got[3:] if got[0] == "klt" else got[4:], want[3:] if want[0] == "klt" else want[4:]):
-            assert a.shape == b.shape and np.abs(a - b).max() <= 1e-3
-    assert removed == want_removed and removed > 5
-    got_ids = {int(l) for l, s in zip(order, is_stereo) if s}
-    assert got_ids == set(want_stereo) and 60 < len(got_ids) < n - 40
-    for l, p in zip(order, rpx):
-        if int(l) in want_stereo:
-            assert np.abs(p - want_stereo[int(l)]).max() <= 1e-3
+    r = SS.read_stereo_result(tmp_path / "r.bin")
+    order, is_stereo, rpx, removed = r["order"], r["is_stereo"], r["rpx"], r["removed"]
+    calls = _read_stereo_log(log)
+    assert [c[0] for c in calls] == ["build", "build", "stereo"]          # left and right image: one upload each; one call
+    a = calls[2][1]
+    fl = SS.flat_scene(sc, order)
+    n = len(order)
+    assert (a["first"], a["count"], a["rectified"], a["nklt_pyr_lvl"], a["img_wh"]) == (0, 1, rect, 3, (sc["w"], sc["h"]))
+    assert (a["win"], a["max_iter"], a["eps"], a["ferr"], a["fb_dist"]) == (9, 30, np.float32(0.01), 30.0, np.float32(0.5))
+    for k in ("px", "unpx", "bv", "is3d", "has_mp"):
+        assert np.array_equal(a[k], fl[k]), k
+    mp = fl["has_mp"] == 1
+    assert np.array_equal(a["wpt"][mp], fl["wpt"][mp]) and not a["wpt"][~mp].any()
+    assert np.array_equal(a["K"], fl["K"][0]) and np.array_equal(a["Frl"], fl["Frl"][0])
+    if distorted:
+        assert np.array_equal(a["dist"], fl["dist"][0]) and a["dist"][4] == 0.0
+    else:
+        assert a["dist"] is None
+    # the poses travel through unit quaternions (as in the reference's map)
+    assert np.array_equal(a["Tcw"], r["Tcw"]) and np.array_equal(a["Trl"], r["Trl"])
+    assert np.abs(a["Tcw"] - fl["Tcw"][0]).max() < 1e-12 and np.abs(a["Trl"] - fl["Trl"][0]).max() < 1e-12
+    if rect:
+        assert a["grid"] is None and a["cell_ptr"] is None
+    else:
+        assert np.array_equal(a["grid"], fl["grid"][0]) and np.array_equal(a["cell_ptr"], fl["cell_ptr"])
+        assert np.array_equal(a["cell_kps"], np.concatenate([fl["cell_kps"], np.zeros(n - len(fl["cell_kps"]), np.int32)]))
+    # the recorder's answers applied: keypoint i is a stereo match iff it was tracked and i % 3 != 0
+    gone = (fl["is3d"] == 1) & ~mp
+    assert removed == int(gone.sum()) and removed > 5
+    i = np.arange(n)
+    want = ~gone & (i % 3 != 0)
+    assert np.array_equal(is_stereo, want) and 60 < want.sum() < n - 40
+    want_rpx = fl["px"] + np.stack([np.float32(-10) - (i % 7).astype(np.float32), np.full(n, 0.25, np.float32)], 1)
+    assert np.array_equal(rpx[want], want_rpx[want]) and not rpx[~want].any()
 
 
 @pytest.mark.gpu
@@ -580,16 +445,12 @@ def test_stereo_matching_shim_on_the_device(tmp_path):
     exe = build.build_stereo_shim()
     disp = 16.0
     K0, base = 458.654, 0.11
-    sc = _stereo_scene(77, 1, depth=K0 * base / disp)
-    _write_stereo_scene(tmp_path / "s.bin", sc)
+    sc = SS.stereo_scene(77, 1, depth=K0 * base / disp)
+    SS.write_stereo_scene(tmp_path / "s.bin", sc)
     out = subprocess.run([str(exe), str(tmp_path / "s.bin"), str(tmp_path / "r.bin"), str(disp)], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
-    raw = np.fromfile(tmp_path / "r.bin", np.uint8)
-    n = int(raw[:4].view(np.int32)[0])
-    order = raw[4:4 + 4 * n].view(np.int32)
-    rec = raw[4 + 4 * n:4 + 16 * n].reshape(n, 12)
-    is_stereo = rec[:, :4].copy().view(np.int32).reshape(n) != 0
-    rpx = rec[:, 4:].copy().view(np.float32).reshape(n, 2)
+    r = SS.read_stereo_result(tmp_path / "r.bin")
+    order, is_stereo, rpx = r["order"], r["is_stereo"], r["rpx"]
     idx = {int(l): i for i, l in enumerate(sc["lmid"])}
     px = np.stack([sc["px"][idx[int(l)]] for l in order])
     alive = np.array([not (sc["is3d"][idx[int(l)]] and not sc["has_mp"][idx[int(l)]]) for l in order])

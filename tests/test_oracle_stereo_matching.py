@@ -5,18 +5,16 @@
     compiled in place (oracle/_ref/libov2ref_map.so, or its outputs stored in tests/golden/reference_map.npz), on both branches:
     the same stereo keypoints, and right pixels within 1e-4 px."""
 import ctypes as C
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import stereo_scenes as SS
 from oracle import image_ref as R
 from oracle import stereo_matching_ref as S
 from reference_golden import ReferenceOutputs
 
 cv2 = pytest.importorskip("cv2")
-sys.path.insert(0, str(Path(__file__).parent))
 
 CALIBS = {
     "euroc": ([458.654, 457.296, 367.215, 248.375], [-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05, 0.0]),
@@ -60,41 +58,16 @@ def lib():
     return ReferenceOutputs("map", handle)
 
 
-def flat_scene(sc, order):
-    """A stereo scene of tests/test_host_shim.py (_stereo_scene) as ov2_stereo_matching's arrays for one keyframe, keypoints in
-    the reference's Frame::getKeypoints() order, the grid lists in insertion (scene) order."""
-    idx = {int(l): i for i, l in enumerate(sc["lmid"])}
-    perm = np.array([idx[int(l)] for l in order], np.int64)
-    pos = np.empty(len(perm), np.int64)
-    pos[perm] = np.arange(len(perm))
-    Rcw = sc["Rwc"].T
-    Rrl = sc["Rrig"].T
-    cs, nbw, nbh = sc["cs"], sc["nbw"], sc["nbh"]
-    cells = [[] for _ in range(nbw * nbh)]
-    for i in range(len(sc["lmid"])):
-        p = sc["px"][i]
-        cells[int(np.floor(p[1] / np.float32(cs))) * nbw + int(np.floor(p[0] / np.float32(cs)))].append(int(pos[i]))
-    return dict(offsets=np.array([0, len(perm)], np.int32), Tcw=np.concatenate([Rcw.reshape(-1), -Rcw @ sc["twc"]])[None],
-                K=np.asarray(sc["K"], np.float64)[None], Trl=np.concatenate([Rrl.reshape(-1), -Rrl @ sc["trig"]])[None],
-                Frl=np.asarray(sc["Frl"]).reshape(1, 9), img_wh=np.array([[sc["w"], sc["h"]]], np.int32),
-                px=sc["px"][perm], unpx=sc["unpx"][perm], bv=sc["bv"][perm], is3d=sc["is3d"][perm].astype(np.uint8),
-                has_mp=sc["has_mp"][perm].astype(np.uint8), wpt=sc["wpt"][perm], rectified=int(sc["rect"]),
-                cell_offsets=np.array([0, nbw * nbh], np.int32), grid=np.array([[cs, nbw]], np.int32),
-                cell_ptr=np.concatenate([[0], np.cumsum([len(c) for c in cells])]).astype(np.int32),
-                cell_kps=np.array([j for c in cells for j in c], np.int32))
-
-
 @pytest.mark.parametrize("rect", [1, 0])
 def test_stereo_matching_flow_equals_the_reference_source(lib, rect):
-    """The reference's stereoMatching on the scene of tests/test_oracle_vs_reference_map.py::test_stereo_matching_equals_the_reference_source
-    (a textured pair 16 px apart, 260 keypoints): the oracle's flow, around the same cv2 functions, makes the same keypoints stereo
-    keypoints, with the same right pixels."""
-    import test_host_shim as H
+    """The reference's stereoMatching on a synthetic stereo keyframe (tests/stereo_scenes.py) over a textured pair 16 px apart, 260
+    keypoints: the oracle's flow, around the same cv2 functions, makes the same keypoints stereo keypoints, with the same right
+    pixels."""
     w, h, disp = 752, 480, 16.0
     yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
     tex = lambda u: np.rint(128 + 50 * np.sin(0.11 * u + 0.07 * yy) + 40 * np.sin(0.05 * u - 0.13 * yy + 1) + 30 * np.sin(0.31 * u + 0.23 * yy + 2)).astype(np.uint8)
     left, right = tex(xx), tex(xx + disp)
-    sc = H._stereo_scene(91 + rect, rect, nkps=260, depth=458.654 * 0.11 / disp)
+    sc = SS.stereo_scene(91 + rect, rect, nkps=260, depth=458.654 * 0.11 / disp)
     lv_l, lv_r = [left], [right]
     for _ in range(3):
         lv_l.append(cv2.pyrDown(lv_l[-1]))
@@ -107,8 +80,8 @@ def test_stereo_matching_flow_equals_the_reference_source(lib, rect):
         pl, pr = PP(*[a.ctypes.data_as(U) for a in lv_l]), PP(*[a.ctypes.data_as(U) for a in lv_r])
         rows, cols = np.array([a.shape[0] for a in lv_l], np.int32), np.array([a.shape[1] for a in lv_l], np.int32)
         order, st, rpx = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros((n, 2), np.float32)
-        a = dict(K=np.ascontiguousarray(sc["K"], np.float64), rig=np.ascontiguousarray(np.concatenate([sc["trig"], H._quat_of(sc["Rrig"])]), np.float64),
-                 Twc=np.ascontiguousarray(np.concatenate([sc["twc"], H._quat_of(sc["Rwc"])]), np.float64), lmid=np.ascontiguousarray(sc["lmid"], np.int32),
+        a = dict(K=np.ascontiguousarray(sc["K"], np.float64), rig=np.ascontiguousarray(np.concatenate([sc["trig"], SS.quat_of(sc["Rrig"])]), np.float64),
+                 Twc=np.ascontiguousarray(np.concatenate([sc["twc"], SS.quat_of(sc["Rwc"])]), np.float64), lmid=np.ascontiguousarray(sc["lmid"], np.int32),
                  is3d=np.ascontiguousarray(sc["is3d"], np.int32), has=np.ascontiguousarray(sc["has_mp"], np.int32), px=np.ascontiguousarray(sc["px"], np.float32),
                  wpt=np.ascontiguousarray(sc["wpt"], np.float64))
         L.ov2ref_stereo_matching.restype = C.c_int
@@ -120,7 +93,7 @@ def test_stereo_matching_flow_equals_the_reference_source(lib, rect):
     r = lib(f"stereo_matching{rect}", live)
     order, st, rpx = r["order"], r["st"], r["rpx"]
     assert int(r["m"]) == n
-    fl = flat_scene(sc, order)
+    fl = SS.flat_scene(sc, order)
     subpix = lambda src, ws, cx, cy: cv2.getRectSubPix(src, (ws, ws), (float(cx), float(cy)))
     out = S.stereo_matching_ref([left], [right], fl.pop("offsets"), fl.pop("Tcw"), fl.pop("K"), fl.pop("Trl"), fl.pop("img_wh"),
                                 fl.pop("px"), fl.pop("unpx"), fl.pop("bv"), fl.pop("is3d"), fl.pop("has_mp"), fl.pop("wpt"),

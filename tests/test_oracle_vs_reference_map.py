@@ -193,63 +193,6 @@ def test_match_to_map_equals_the_reference_source(lib, seed, nkps, ncand):
     assert len(want ^ got) <= max(1, len(want) // 100)
 
 
-@pytest.mark.parametrize("rect", [1, 0])
-def test_stereo_matching_equals_the_reference_source(lib, rect):
-    """The REFERENCE'S OWN MapManager::stereoMatching (src/map_manager.cpp:367-611, calling its own fbKltTracking / getLineMinSAD) on a synthetic
-    stereo keyframe over a textured pair (16 px disparity), the arithmetic answered by the real library: the keypoints that become stereo
-    keypoints and their right pixels are those of the flow restatement tests/test_host_shim.py checks the drop-in against
-    (`_stereo_flow`), fed with the same library functions - so the drop-in's flow is the reference's."""
-    import sys
-    import cv2
-    sys.path.insert(0, str(Path(__file__).parent))
-    import test_host_shim as H
-    from oracle import image_ref as R
-    w, h, disp = 752, 480, 16.0
-    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
-    tex = lambda u: np.rint(128 + 50 * np.sin(0.11 * u + 0.07 * yy) + 40 * np.sin(0.05 * u - 0.13 * yy + 1) + 30 * np.sin(0.31 * u + 0.23 * yy + 2)).astype(np.uint8)
-    left, right = tex(xx), tex(xx + disp)
-    sc = H._stereo_scene(91 + rect, rect, nkps=260, depth=458.654 * 0.11 / disp)
-    lv_l, lv_r = [left], [right]
-    for _ in range(3):
-        lv_l.append(cv2.pyrDown(lv_l[-1]))
-        lv_r.append(cv2.pyrDown(lv_r[-1]))
-    n = len(sc["lmid"])
-
-    def live(lib):
-        PP = C.POINTER(C.c_uint8) * 4
-        pl, pr = PP(*[a.ctypes.data_as(U) for a in lv_l]), PP(*[a.ctypes.data_as(U) for a in lv_r])
-        rows, cols = np.array([a.shape[0] for a in lv_l], np.int32), np.array([a.shape[1] for a in lv_l], np.int32)
-        order, st, rpx = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros((n, 2), np.float32)
-        a = dict(K=np.ascontiguousarray(sc["K"], np.float64), rig=np.ascontiguousarray(np.concatenate([sc["trig"], H._quat_of(sc["Rrig"])]), np.float64),
-                 Twc=np.ascontiguousarray(np.concatenate([sc["twc"], H._quat_of(sc["Rwc"])]), np.float64), lmid=np.ascontiguousarray(sc["lmid"], np.int32),
-                 is3d=np.ascontiguousarray(sc["is3d"], np.int32), has=np.ascontiguousarray(sc["has_mp"], np.int32), px=np.ascontiguousarray(sc["px"], np.float32),
-                 wpt=np.ascontiguousarray(sc["wpt"], np.float64))
-        lib.ov2ref_stereo_matching.restype = C.c_int
-        m = lib.ov2ref_stereo_matching(n, rect, a["K"].ctypes.data_as(D), a["K"].ctypes.data_as(D), a["rig"].ctypes.data_as(D), a["Twc"].ctypes.data_as(D), w, h, 35,
-                                       a["lmid"].ctypes.data_as(I), a["is3d"].ctypes.data_as(I), a["has"].ctypes.data_as(I), a["px"].ctypes.data_as(C.POINTER(C.c_float)),
-                                       a["wpt"].ctypes.data_as(D), pl, pr, rows.ctypes.data_as(I), cols.ctypes.data_as(I), order.ctypes.data_as(I),
-                                       st.ctypes.data_as(I), rpx.ctypes.data_as(C.POINTER(C.c_float)))
-        return dict(m=m, order=order, st=st, rpx=rpx)
-    r = lib(f"stereo_matching{rect}", live)
-    m, order, st, rpx = int(r["m"]), r["order"], r["st"], r["rpx"]
-    assert m == n
-
-    def klt(pts, pri, nlv):
-        out, status = R._fb_klt(R._lk_cv2, left, right, pts, pri, 9, nlv, 30.0, 0.5, 30, R.KLT_EPS)
-        return out, status.astype(bool)
-
-    def sad(sp):
-        subpix = lambda src, ws, cx, cy: cv2.getRectSubPix(src, (ws, ws), (float(cx), float(cy)))
-        return np.array([R.line_min_sad_ref(lv_l[3], lv_r[3], (float(p[0]), float(p[1])), 7, True, subpix=subpix)[0] for p in sp], np.float32)
-
-    _, want, _ = H._stereo_flow(sc, order, klt=klt, sad=sad)
-    got = {int(l) for l, s in zip(order, st) if s}
-    assert got == set(want) and len(got) > 0.6 * n
-    for l, p in zip(order, rpx):
-        if int(l) in want:
-            assert np.abs(p - want[int(l)]).max() <= 1e-4
-
-
 @pytest.mark.parametrize("detector,w,h,cs", [(0, 640, 480, 50), (1, 752, 480, 35)])
 def test_extract_keypoints_equals_the_reference_source(lib, detector, w, h, cs):
     """The REFERENCE'S OWN MapManager::extractKeypoints (src/map_manager.cpp:286-341) - the caller of the detector and the descriptor that

@@ -8,24 +8,22 @@ prior) and keypoints without a 3-D neighbour; row-search columns equal to px.x a
 arise: the scan starts at px.x * downpyrcoef and moves left, and both scalings are exact); epipolar errors exactly 2 and one
 float step above; failed guided tracks retried at full depth; host and device arrays, run-to-run equality and a first slot
 above 0; every refusal.  A second test runs the drop-in MapManager::stereoMatching (host/stereo_selftest.cpp) on the GPU and
-checks that the batched call gives the same stereo keypoints and right pixels.
+checks that the batched call gives the same stereo keypoints and bit-equal right pixels.
 
 Scenes whose oracle decisions (epipolar errors) lie within a relative 1e-6 of the threshold are redrawn.
 """
 import os
 import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import stereo_scenes as SS
 from ov2slam_b200 import api, build, synth
 from oracle import image_ref as R
 from oracle import stereo_matching_ref as S
 
 pytestmark = pytest.mark.gpu
-sys.path.insert(0, str(Path(__file__).parent))
 
 W, H = 320, 240
 KEYS = ("right", "stereo", "passes", "nstereo")
@@ -315,34 +313,33 @@ def test_stereo_matching_refusals(ctx):
 @pytest.mark.parametrize("rect", [1, 0])
 def test_batched_call_equals_the_drop_in(ctx, tmp_path, rect):
     """host/stereo_selftest.cpp's synthetic keyframe (a smooth texture and its copy 16 px to the left) through the drop-in
-    MapManager::stereoMatching on the GPU, and through one ov2_stereo_matching call: the same stereo keypoints and right pixels."""
-    import test_host_shim as H
-    from test_oracle_stereo_matching import flat_scene
+    MapManager::stereoMatching on the GPU, and through one ov2_stereo_matching call on the same keyframe flattened here: the drop-in
+    makes that very call (with the pose and the rig as it flattened them), so the stereo keypoints and their right pixels are
+    bit-equal, and the observations it removed are those of the 3-D keypoints without a map point."""
     exe = build.build_stereo_shim()
     disp = 16.0
-    sc = H._stereo_scene(77 + rect, rect, depth=458.654 * 0.11 / disp)
-    H._write_stereo_scene(tmp_path / "s.bin", sc)
+    sc = SS.stereo_scene(77 + rect, rect, depth=458.654 * 0.11 / disp)
+    SS.write_stereo_scene(tmp_path / "s.bin", sc)
     res = subprocess.run([str(exe), str(tmp_path / "s.bin"), str(tmp_path / "r.bin"), str(disp)], capture_output=True, text=True,
                          timeout=120, env=dict(os.environ))
     assert res.returncode == 0, res.stdout + res.stderr
-    raw = np.fromfile(tmp_path / "r.bin", np.uint8)
-    n = int(raw[:4].view(np.int32)[0])
-    order = raw[4:4 + 4 * n].view(np.int32)
-    rec = raw[4 + 4 * n:4 + 16 * n].reshape(n, 12)
-    is_stereo = rec[:, :4].copy().view(np.int32).reshape(n) != 0
-    rpx = rec[:, 4:].copy().view(np.float32).reshape(n, 2)
+    r = SS.read_stereo_result(tmp_path / "r.bin")
+    order, is_stereo, rpx = r["order"], r["is_stereo"], r["rpx"]
+    n = len(order)
     w, h = sc["w"], sc["h"]
     yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
     tex = lambda u: np.rint(128 + 50 * np.sin(0.11 * u + 0.07 * yy) + 40 * np.sin(0.05 * u - 0.13 * yy + 1) + 30 * np.sin(0.31 * u + 0.23 * yy + 2)).astype(np.uint8)
     lp, rp = api.Pyramid(ctx, 1, w, h, 3), api.Pyramid(ctx, 1, w, h, 3)
     lp.build(tex(xx)[None])
     rp.build(tex(xx + disp)[None])
-    fl = flat_scene(sc, order)
+    fl = SS.flat_scene(sc, order)
+    fl["Tcw"], fl["Trl"] = r["Tcw"][None], r["Trl"][None]          # as the drop-in flattens them (through unit quaternions)
     got = api.FeatureTracker(ctx, 30, 0.01).stereo_matching(
         lp, rp, 9, 3, 30.0, 0.5, fl["rectified"], fl["offsets"], fl["Tcw"], fl["K"], fl["Trl"], fl["img_wh"], fl["px"], fl["unpx"],
-        fl["bv"], fl["is3d"], fl["has_mp"], fl["wpt"], Frl=fl["Frl"], cell_offsets=fl["cell_offsets"], grid=fl["grid"],
+        fl["bv"], fl["is3d"], fl["has_mp"], fl["wpt"], dist=fl["dist"], Frl=fl["Frl"], cell_offsets=fl["cell_offsets"], grid=fl["grid"],
         cell_ptr=fl["cell_ptr"], cell_kps=fl["cell_kps"])
     st = got["stereo"].astype(bool)
     assert np.array_equal(st, is_stereo) and st.sum() > 0.5 * n, (st.sum(), is_stereo.sum())
-    assert np.abs(got["right"][st] - rpx[st]).max() <= 1e-4
+    assert np.array_equal(got["right"][st].view(np.uint32), rpx[st].view(np.uint32))
     assert got["nstereo"][0] == is_stereo.sum()
+    assert r["removed"] == int(((fl["is3d"] == 1) & (fl["has_mp"] == 0)).sum()) and r["removed"] > 0
